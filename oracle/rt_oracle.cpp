@@ -950,6 +950,158 @@ int orRaySphere(const float pos[3], const float dir[3], const float centre[3], f
 
 } // extern "C"
 
+/* Batched primitive evaluation, the oracle's side of the device probe (tests/gpu_probe/rt_probe.cu, rtpRun): same function codes,
+ * same records, same index mode and digest.  Every value comes from an orc:: or Shader:: function of this file. */
+namespace probe {
+
+static unsigned long long mix64(unsigned long long z)
+{
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    return z ^ (z >> 31);
+}
+static unsigned long long digest_term(unsigned long long i, uint w, bool isFloat)
+{
+    if (isFloat && (w & 0x7fffffffu) > 0x7f800000u) w = 0x7fc00000u;
+    return mix64((i << 32) ^ w);                              // i < 2^32 within one call: injective in (i, w)
+}
+static float3 F3(const uint* a) { return mk3(u2f(a[0]), u2f(a[1]), u2f(a[2])); }
+static void put3(uint* r, float3 v) { r[0] = f2u(v.x); r[1] = f2u(v.y); r[2] = f2u(v.z); }
+
+static int arity(int fn, int& nin, int& nout)
+{
+    switch (fn)
+    {
+    case 0: case 1: case 2: case 3: case 6: case 9: case 10: nin = 1; nout = 1; return 1;     // log exp sin cos saturate f2uint_rz DisplayEncode
+    case 4: case 11: case 12: case 13: nin = 1; nout = 2; return 1;                          // sin+cos, NextRandom, RandomValue, normal draw
+    case 5: case 7: case 8: nin = 2; nout = 1; return 1;                                     // pow min max
+    case 14: nin = 1; nout = 4; return 1;                                                    // RandomDirection
+    case 15: nin = 1; nout = 3; return 1;                                                    // RandomPointInCircle
+    case 20: nin = 12; nout = 1; return 1;                                                   // RayBoundingBoxDst
+    case 21: nin = 25; nout = 5; return 1;                                                   // RayTriangle
+    case 22: nin = 10; nout = 2; return 1;                                                   // RaySphere
+    case 23: case 24: nin = 8; nout = fn == 23 ? 1 : 3; return 1;                            // CalculateReflectance, Refract
+    case 25: nin = 6; nout = 3; return 1;                                                    // Reflect
+    case 26: nin = 17; nout = 3; return 1;                                                   // GetMaterialColour
+    case 27: nin = 11; nout = 3; return 1;                                                   // GetEnvironmentLight
+    default: return 0;
+    }
+}
+
+static void eval(int fn, const uint* a, uint* r)
+{
+    switch (fn)
+    {
+    case 0: r[0] = f2u(orc::log(u2f(a[0]))); break;
+    case 1: r[0] = f2u(orc::exp(u2f(a[0]))); break;
+    case 2: r[0] = f2u(orc::sin(u2f(a[0]))); break;
+    case 3: r[0] = f2u(orc::cos(u2f(a[0]))); break;
+    case 4: r[0] = f2u(orc::sin(u2f(a[0]))); r[1] = f2u(orc::cos(u2f(a[0]))); break;
+    case 5: r[0] = f2u(orc::pow(u2f(a[0]), u2f(a[1]))); break;
+    case 6: r[0] = f2u(orc::saturate(u2f(a[0]))); break;
+    case 7: r[0] = f2u(orc::min(u2f(a[0]), u2f(a[1]))); break;
+    case 8: r[0] = f2u(orc::max(u2f(a[0]), u2f(a[1]))); break;
+    case 9: r[0] = orc::f2uint_rz(u2f(a[0])); break;
+    case 10: r[0] = DisplayEncode(u2f(a[0])); break;
+    case 11: { uint s = a[0]; r[0] = Shader::NextRandom(s); r[1] = s; break; }
+    case 12: { uint s = a[0]; r[0] = f2u(Shader::RandomValue(s)); r[1] = s; break; }
+    case 13: { uint s = a[0]; r[0] = f2u(Shader::RandomValueNormalDistribution(s)); r[1] = s; break; }
+    case 14: { uint s = a[0]; put3(r, Shader::RandomDirection(s)); r[3] = s; break; }
+    case 15: { uint s = a[0]; const float2 p = Shader::RandomPointInCircle(s); r[0] = f2u(p.x); r[1] = f2u(p.y); r[2] = s; break; }
+    case 20:
+    {
+        Shader::Ray ray; ray.pos = F3(a); ray.dir = F3(a + 3); ray.invDir = 1.0f / ray.dir;
+        r[0] = f2u(Shader::RayBoundingBoxDst(ray, F3(a + 6), F3(a + 9)));
+        break;
+    }
+    case 21:
+    {
+        Shader::Ray ray; ray.pos = F3(a); ray.dir = F3(a + 3); ray.invDir = 1.0f / ray.dir;
+        RtTriangle tri; memcpy(&tri, a + 6, sizeof(tri));
+        const Shader::TriangleHitInfo h = Shader::RayTriangle(ray, tri, a[24] != 0u);
+        r[0] = (h.didHit ? 1u : 0u) | (h.isBackface ? 2u : 0u);
+        r[1] = f2u(h.dst);
+        put3(r + 2, h.normal);
+        break;
+    }
+    case 22:
+    {
+        const Shader::ModelHitInfo h = Shader::RaySphere(F3(a), F3(a + 3), F3(a + 6), u2f(a[9]));
+        r[0] = (h.didHit ? 1u : 0u) | (h.isBackface ? 2u : 0u);
+        r[1] = f2u(h.dst);
+        break;
+    }
+    case 23: r[0] = f2u(Shader::CalculateReflectance(F3(a), F3(a + 3), u2f(a[6]), u2f(a[7]))); break;
+    case 24: put3(r, Shader::Refract(F3(a), F3(a + 3), u2f(a[6]), u2f(a[7]))); break;
+    case 25: put3(r, Shader::Reflect(F3(a), F3(a + 3))); break;
+    case 26:
+    {
+        RtMaterial m; memset(&m, 0, sizeof(m));
+        m.flag = (int)a[7];
+        for (int k = 0; k < 3; k++) { m.diffuseCol[k] = u2f(a[8 + k]); m.emissionCol[k] = u2f(a[11 + k]); m.specularCol[k] = u2f(a[14 + k]); }
+        put3(r, Shader::GetMaterialColour(m, F3(a), F3(a + 3), a[6] != 0u));
+        break;
+    }
+    case 27:
+    {
+        Shader s; s.UseSky = 1; s.SunFocus = u2f(a[3]); s.SunIntensity = u2f(a[4]); s.dirToSun = F3(a + 5); s.SunColour = F3(a + 8);
+        put3(r, s.GetEnvironmentLight(F3(a)));
+        break;
+    }
+    default: break;
+    }
+}
+
+} // namespace probe
+
+extern "C" {
+
+/* n cases of primitive `fn` (codes and records: tests/gpu_probe/rt_probe.cu).  in: n * nin words, or NULL for index mode (word 0 of case
+ * i = base + i * stride, the others = partner); out: n * nout words or NULL; digest: nout sums or NULL.  `threads` worker threads
+ * (0 = all cores).  Returns 0, or 1 for an unknown function / wrong arity. */
+int orProbe(int fn, int nin, int nout, const uint* in, uint base, uint stride, uint partner, uint* out, uint floatMask, size_t n,
+            unsigned long long* digest, int threads)
+{
+    int ein = 0, eout = 0;
+    if (!probe::arity(fn, ein, eout) || ein != nin || eout != nout) return 1;
+    int nt = threads > 0 ? threads : (int)std::thread::hardware_concurrency();
+    if (nt < 1) nt = 1;
+    if ((size_t)nt > n / 4096 + 1) nt = (int)(n / 4096 + 1);
+    std::vector<unsigned long long> part((size_t)nt * 8, 0ull);
+    std::vector<std::thread> pool;
+    for (int t = 0; t < nt; t++)
+    {
+        pool.emplace_back([&, t]() {
+            const size_t i0 = n * (size_t)t / (size_t)nt, i1 = n * (size_t)(t + 1) / (size_t)nt;
+            unsigned long long* h = &part[(size_t)t * 8];
+            uint a[32], r[8];
+            for (size_t i = i0; i < i1; i++)
+            {
+                if (in) memcpy(a, in + i * nin, (size_t)nin * 4);
+                else { a[0] = base + (uint)i * stride; for (int k = 1; k < nin; k++) a[k] = partner; }
+                memset(r, 0, sizeof(r));
+                probe::eval(fn, a, r);
+                for (int j = 0; j < nout; j++)
+                {
+                    if (out) out[i * nout + j] = r[j];
+                    h[j] += probe::digest_term(i, r[j], (floatMask >> j) & 1u);
+                }
+            }
+        });
+    }
+    for (auto& th : pool) th.join();
+    if (digest)
+        for (int j = 0; j < nout; j++)
+        {
+            unsigned long long s = 0;
+            for (int t = 0; t < nt; t++) s += part[(size_t)t * 8 + j];
+            digest[j] = s;
+        }
+    return 0;
+}
+
+} // extern "C"
+
 // ---- BVH builder: CPU restatement of Assets/Scripts/Types/BVH.cs:26-318 (BC below), the oracle of rtBuildBVH -------------------
 // Plain single-threaded recursion in the reference's own shape: one flat node list, in-place swap partition.  Test
 // infrastructure like the rest of this file.

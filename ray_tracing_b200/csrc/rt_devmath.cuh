@@ -9,7 +9,7 @@
 //   smoothstep(a,b,x): t = saturate((x-a)/(b-a)); t*t*(3-2t)                   (SURVEY.md §8a Q11)
 // and log / exp / sin / cos / pow are polynomial routines made only of those IEEE ops (Cody–Waite
 // range reduction + published minimax kernels), so they need no libdevice and are reproducible on any
-// conforming FP32 machine.  Accuracy ~1 ulp (log, exp) and < 1e-7 absolute (sin, cos on |x| < 1e5).
+// conforming FP32 machine.  Accuracy, exhaustive (DESIGN.md §2): < 1 ulp (log, exp); sin / cos < 1.5e-7 absolute on [0, 2π], the only angles the path uses (6.2831852 · RandomValue), but up to ~1e-6 on (2π, 1e5], NaN beyond ±1e5.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -171,6 +171,61 @@ inline void BuildMedianSplitPairs(const std::vector<float>& lo, const std::vecto
     }
 }
 
+#ifndef RT_ORIGIN_PAD_SCALE
+#define RT_ORIGIN_PAD_SCALE 2e-5      // of the largest coordinate R a ray origin can have (~170 ulp(R)); see buildModels.  Measured on the interpreter
+                                      // build: 144 differing values with 0, none with 1e-7 (about 1 ulp) and above; the error estimate is <= 40 ulp(R)
+#endif
+
+// Padding of a model's world box (RepackState::buildModels; the reasoning is there).  originPadOf: the part that covers rays starting far
+// away, RT_ORIGIN_PAD_SCALE of the largest coordinate of the origin box (infinite when that box is not finite).  paddedModelBox: the
+// box handed to WorldBoxOutOfReach for the exact world box lo..hi of the model's geometry (placed = false: nothing is known, +-inf).
+inline double originPadOf(const float originLo[3], const float originHi[3])
+{
+    double originExtent = 0;
+    for (int a = 0; a < 3; a++)
+    {
+        originExtent = std::max(originExtent, std::max(std::fabs((double)originLo[a]), std::fabs((double)originHi[a])));
+        if (!std::isfinite(originLo[a]) || !std::isfinite(originHi[a])) originExtent = INFINITY;
+    }
+    return RT_ORIGIN_PAD_SCALE * originExtent;
+}
+inline void paddedModelBox(bool placed, const double lo[3], const double hi[3], double originPad, float bmin[3], float bmax[3])
+{
+    for (int a = 0; a < 3; a++)
+    {
+        const double pad = placed ? 1e-4 * ((hi[a] - lo[a]) + std::fabs(lo[a]) + std::fabs(hi[a])) + 1e-5 + originPad : (double)INFINITY;
+        if (!std::isfinite(pad)) { bmin[a] = -INFINITY; bmax[a] = INFINITY; continue; }
+        bmin[a] = std::nextafterf((float)(lo[a] - pad), -INFINITY); bmax[a] = std::nextafterf((float)(hi[a] + pad), INFINITY);
+    }
+}
+
+// r*r of a sphere as DevSphere::r2 holds it: one host multiply (HL:299).  Host code is built without FMA contraction, so this is that product.
+inline float sphereR2(float radius) { volatile float r = radius; return r * r; }
+
+// Box of sphere (centre, radius) in the sphere accelerator (RepackState::buildSpheres): the reference's discriminant carries an absolute
+// error of at most ~2e-6 (D^2 + r^2) (D = distance from the ray origin to the centre), which moves a computed hit point about
+// 2.5e-7 (D^2 + r^2) / r off the sphere (measured worst 2.53e-7, DESIGN.md §5); pad by 16 * 2^-23 * (Dmax^2 + r^2) / r (7.5x that)
+// plus 1e-5 of the scene size for the slab test itself.  originLo / originHi: a box containing every possible ray origin.
+inline void paddedSphereBox(const float centre[3], float radius, const float originLo[3], const float originHi[3], float lo[3], float hi[3])
+{
+    double sceneSize = 0;
+    for (int a = 0; a < 3; a++) sceneSize = std::max(sceneSize, (double)originHi[a] - originLo[a]);
+    double dmax2 = 0;
+    for (int a = 0; a < 3; a++)
+    {
+        const double c = centre[a];
+        const double far = std::max(std::fabs(c - originLo[a]), std::fabs(c - originHi[a]));
+        dmax2 += far * far;
+    }
+    const double r = std::fabs((double)radius);
+    const double pad = 16.0 * 1.1920929e-7 * (dmax2 + r * r) / std::max(r, 1e-30) + 1e-5 * sceneSize + 1e-6;
+    for (int a = 0; a < 3; a++)
+    {
+        lo[a] = (float)(centre[a] - r - pad); hi[a] = (float)(centre[a] + r + pad);
+        lo[a] = std::nextafterf(lo[a], -INFINITY); hi[a] = std::nextafterf(hi[a], INFINITY);
+    }
+}
+
 struct RepackState
 {
     RBuf<NodePair> pairs; RBuf<TriGeom> triGeom; RBuf<TriNormals> triNormals; RBuf<DevModel> models; RBuf<DevSphere> spheres;
@@ -422,10 +477,6 @@ struct RepackState
         return cudaSuccess;
     }
 
-#ifndef RT_ORIGIN_PAD_SCALE
-#define RT_ORIGIN_PAD_SCALE 2e-5      // of the largest coordinate R a ray origin can have (~170 ulp(R)); see buildModels.  Measured on the interpreter
-                                      // build: 144 differing values with 0, none with 1e-7 (about 1 ulp) and above; the error estimate is <= 40 ulp(R)
-#endif
     // Region of ray origins the padding of the current model boxes is valid for (see buildModels); models are rebuilt when the
     // camera or the geometry leaves it.
     float modelBoundLo[3] = {0, 0, 0}, modelBoundHi[3] = {0, 0, 0};
@@ -484,15 +535,9 @@ struct RepackState
     {
         std::vector<DevModel> out(std::max(modelCount, 1));
         memset(out.data(), 0, out.size() * sizeof(DevModel));
-        double originExtent = 0;
-        for (int a = 0; a < 3; a++)
-        {
-            modelBoundLo[a] = originLo[a]; modelBoundHi[a] = originHi[a];
-            originExtent = std::max(originExtent, std::max(std::fabs((double)originLo[a]), std::fabs((double)originHi[a])));
-            if (!std::isfinite(originLo[a]) || !std::isfinite(originHi[a])) originExtent = INFINITY;
-        }
+        for (int a = 0; a < 3; a++) { modelBoundLo[a] = originLo[a]; modelBoundHi[a] = originHi[a]; }
         modelBoundValid = true;
-        const double originPad = RT_ORIGIN_PAD_SCALE * originExtent;     // infinite when the origins are unbounded
+        const double originPad = originPadOf(originLo, originHi);       // infinite when the origins are unbounded
         for (int i = 0; i < modelCount; i++)
         {
             DevModel d; memset(&d, 0, sizeof(d));
@@ -509,12 +554,7 @@ struct RepackState
                 double lo[3], hi[3];
                 const bool placed = worldBoxOfModel(mdl[i], r, lo, hi);
                 float bmin[3], bmax[3];
-                for (int a = 0; a < 3; a++)
-                {
-                    const double pad = placed ? 1e-4 * ((hi[a] - lo[a]) + std::fabs(lo[a]) + std::fabs(hi[a])) + 1e-5 + originPad : (double)INFINITY;
-                    if (!std::isfinite(pad)) { bmin[a] = -INFINITY; bmax[a] = INFINITY; continue; }
-                    bmin[a] = std::nextafterf((float)(lo[a] - pad), -INFINITY); bmax[a] = std::nextafterf((float)(hi[a] + pad), INFINITY);
-                }
+                paddedModelBox(placed, lo, hi, originPad, bmin, bmax);
                 d.wmin[0] = bmin[0]; d.wmin[1] = bmin[1]; d.wmin[2] = bmin[2]; d.wmaxx = bmax[0]; d.wmaxy = bmax[1]; d.wmaxz = bmax[2];
             }
             out[i] = d;
@@ -554,8 +594,7 @@ struct RepackState
         {
             DevSphere d; memset(&d, 0, sizeof(d));
             d.cx = sp[i].centre[0]; d.cy = sp[i].centre[1]; d.cz = sp[i].centre[2]; d.radius = sp[i].radius;
-            // r*r is one IEEE multiply (HL:299).  Host code is built without FMA contraction, so this is that product.
-            volatile float r = sp[i].radius; d.r2 = r * r;
+            d.r2 = sphereR2(sp[i].radius);
             d.pad0 = sp[i].material.flag;                       // material flag, for sorting hits by kind without touching HBM
             d.pad1 = (int)i;
             out[i] = d;
@@ -570,31 +609,14 @@ struct RepackState
         if (sp.size() <= SPHERE_BVH_THRESHOLD) return cudaSuccess;
 
         // ---- BVH over padded sphere boxes (see TraverseSpheres in rt_device.cuh for the exactness argument) ----
-        // padding of sphere i: the reference's discriminant carries an absolute error of at most ~2e-6 (D^2 + r^2) (D = distance
-        // from the ray origin to the centre), which moves a computed hit point at most 2.5e-7 (D^2 + r^2) / r off the sphere;
-        // pad by 16 * 2^-23 * (Dmax^2 + r^2) / r (7.6x that bound) plus 1e-5 of the scene size for the slab test itself.
+        // padding of sphere i: paddedSphereBox
         for (int a = 0; a < 3; a++) { sphBoundLo[a] = originLo[a]; sphBoundHi[a] = originHi[a]; }
         const size_t n = sp.size();
         std::vector<float> lo(3 * n), hi(3 * n), cen(3 * n);
-        double sceneSize = 0;
-        for (int a = 0; a < 3; a++) sceneSize = std::max(sceneSize, (double)originHi[a] - originLo[a]);
         for (size_t i = 0; i < n; i++)
         {
-            double dmax2 = 0;
-            for (int a = 0; a < 3; a++)
-            {
-                const double c = sp[i].centre[a];
-                const double far = std::max(std::fabs(c - originLo[a]), std::fabs(c - originHi[a]));
-                dmax2 += far * far;
-            }
-            const double r = std::fabs((double)sp[i].radius);
-            const double pad = 16.0 * 1.1920929e-7 * (dmax2 + r * r) / std::max(r, 1e-30) + 1e-5 * sceneSize + 1e-6;
-            for (int a = 0; a < 3; a++)
-            {
-                lo[3 * i + a] = (float)(sp[i].centre[a] - r - pad); hi[3 * i + a] = (float)(sp[i].centre[a] + r + pad);
-                lo[3 * i + a] = std::nextafterf(lo[3 * i + a], -INFINITY); hi[3 * i + a] = std::nextafterf(hi[3 * i + a], INFINITY);
-                cen[3 * i + a] = sp[i].centre[a];
-            }
+            paddedSphereBox(sp[i].centre, sp[i].radius, originLo, originHi, &lo[3 * i], &hi[3 * i]);
+            for (int a = 0; a < 3; a++) cen[3 * i + a] = sp[i].centre[a];
         }
         // median split on the widest centroid axis, leaves of <= 4 spheres; pairs emitted parent-before-children
         std::vector<int> order;

@@ -151,6 +151,21 @@ def test_product_does_not_reference_the_simt_build():
     assert "simt" not in syms
 
 
+def test_product_does_not_reference_the_probe():
+    """tests/gpu_probe (the primitive probe of the arithmetic tests) is test infrastructure: it includes the product's device headers,
+    never the other way round, and neither the package, its sources nor the bench build or load it (building it next to the oracle
+    in __graft_entry__.build() is not using it)."""
+    pkg = os.path.join(REPO, "ray_tracing_b200")
+    files = [os.path.join(REPO, "bench.py")] + [os.path.join(pkg, f) for f in os.listdir(pkg) if f.endswith(".py")]
+    for d in ("host", "csrc"):
+        files += [os.path.join(pkg, d, f) for f in os.listdir(os.path.join(pkg, d))]
+    for f in files:
+        text = open(f).read()
+        assert "gpu_probe" not in text and "rt_probe" not in text and "rtpRun" not in text, f
+    syms = subprocess.run(["nm", "-D", "--defined-only", CUDA_LIB], capture_output=True, text=True).stdout
+    assert "rtpRun" not in syms and "orProbe" not in syms
+
+
 @pytest.mark.skipif(os.path.exists("/dev/nvidiactl"), reason="a GPU is present")
 def test_cuda_library_fails_loudly_without_a_gpu():
     with pytest.raises(capi.RtError) as e:
