@@ -46,6 +46,11 @@ public static class RtB200
     public struct Stats { public ulong rays, boxTests, triTests, sphereTests, dispatches; public double kernelMs; public ulong sphereBoxTests; public double exchangeMs; }
     [DllImport(Lib)] public static extern int rtGetStats(IntPtr ctx, out Stats stats);
     [DllImport(Lib)] public static extern int rtResetStats(IntPtr ctx);
+    // the reference's debug view (visMode / debugVisScale, RayCommon.hlsl:24-26): per-pixel counters of the "countStats" = 1 launches and their heat map
+    [StructLayout(LayoutKind.Sequential)]
+    public struct PixelStats { public uint rays, boxTests, triTests, sphereTests, sphereBoxTests; }
+    [DllImport(Lib)] public static extern int rtReadbackPixelStats(IntPtr ctx, [Out] PixelStats[] dst, UIntPtr bytes);
+    [DllImport(Lib)] public static extern int rtDisplayPixelStats(IntPtr ctx, int visMode, float debugVisScale, byte[] rgba, UIntPtr bytes);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

@@ -167,7 +167,7 @@ int rtCommDestroy(RtContext* ctx);
 int rtExchangeTiles(RtContext* ctx);
 
 /* Device address + size of a named device object, for zero-copy plumbing (NCCL, torch views).
- * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv"}. */
+ * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv","PixelStats"}. */
 int rtGetDevicePointer(RtContext* ctx, const char* name, void** devPtr, size_t* bytes);
 
 /* Replaces `new BVH(mesh.vertices, mesh.triangles, mesh.normals, quality)` (BVH.cs:26; called once per shared mesh from
@@ -234,9 +234,32 @@ typedef struct RtStats {
                                rtDispatch / rtExchangeTiles since the last reset (sum)                              */
 } RtStats;
 
-/* Synchronises, then reports the counters accumulated since the last rtResetStats. */
+/* Synchronises, then reports the counters accumulated since the last rtResetStats (which also zeroes "PixelStats"). */
 int rtGetStats(RtContext* ctx, RtStats* out);
 int rtResetStats(RtContext* ctx);
+
+/* ---- per-pixel cost (the reference's debug view, HL:24-26,119: visMode / debugVisScale / stats, never written out there) ----
+ * Every RT_KERNEL_RAYTRACE dispatch with "countStats" = 1 also adds each traced pixel's counts into the device image
+ * "PixelStats": W*H RtPixelStats (rt_types.h), [y][x], row 0 = bottom, covering all samples and bounces of the pixel.  The image
+ * is allocated (zero-filled) by the first counting dispatch, zeroed by rtResetStats and by rtResize to a new size, and accumulates
+ * across dispatches in between, like RtStats.  Counts wrap modulo 2^32.  Pixels outside a partial dispatch or outside this
+ * context's row bands (rtSetTile / rtCommInit) are not touched.  Not available on a group context (rtCreateMulti): RT_E_STATE.
+ * rtGetDevicePointer also accepts "PixelStats" (after the first counting dispatch). */
+
+/* W*H RtPixelStats, [y][x], row 0 = bottom; bytes must equal W*H*20.  RT_E_STATE before any counting dispatch.  Synchronises. */
+int rtReadbackPixelStats(RtContext* ctx, RtPixelStats* dst, size_t bytes);
+
+/* Heat map of PixelStats as W*H RGBA8 ([y][x], row 0 = bottom); bytes must equal W*H*4.  Synchronises.
+ *   visMode 1: boxTests / rays   2: triTests / rays   3: (sphereTests + sphereBoxTests) / rays   4: rays (segments per pixel)
+ *   debugVisScale: the value shown as full white; above it the pixel is red.  Must be finite and > 0.
+ * Encode, binary32 with round-to-nearest-even, one operation at a time (so that any implementation restates it bit for bit):
+ *   rays == 0                        -> (0, 0, 0, 255)
+ *   v = (float)count / (float)rays   (mode 3: count = sphereTests + sphereBoxTests in uint32, wrapping; mode 4: v = (float)rays)
+ *   t = v / debugVisScale
+ *   t > 1                            -> (255, 0, 0, 255)
+ *   else g = (uint8)trunc(t * 255 + 0.5)  -> (g, g, g, 255)
+ * RT_E_INVALID for visMode outside 1..4, a bad debugVisScale or a wrong bytes; RT_E_STATE before any counting dispatch. */
+int rtDisplayPixelStats(RtContext* ctx, int visMode, float debugVisScale, uint8_t* dst, size_t bytes);
 
 /* ABI version of this header: (major << 16) | minor. */
 int rtGetVersion(void);

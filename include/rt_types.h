@@ -66,10 +66,18 @@ typedef struct RtSphere {
     RtMaterial material;
 } RtSphere;
 
+/* Per-pixel traversal counters of the counting launch ("countStats" = 1; no counterpart in the reference, whose `stats`
+ * (RayCommon.hlsl:254,271) are never written out).  The fields mean what the RtStats fields of the same names mean, summed
+ * over all samples and bounces of that pixel since the last rtResetStats.  Unsigned 32-bit: they wrap modulo 2^32. */
+typedef struct RtPixelStats {
+    uint32_t rays, boxTests, triTests, sphereTests, sphereBoxTests;
+} RtPixelStats;
+
 #pragma pack(pop)
 
 #ifdef __cplusplus
 }
+static_assert(sizeof(RtPixelStats) == 20, "PixelStats record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

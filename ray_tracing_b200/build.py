@@ -18,6 +18,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 HOST = os.path.join(PKG_DIR, "host")
 INCLUDE = os.path.join(REPO_DIR, "include")
 ORACLE = os.path.join(REPO_DIR, "oracle")
+ORACLE_EXT = os.path.join(REPO_DIR, "tests", "oracle_ext")
 
 LIB_CUDA = os.path.join(PKG_DIR, "librt_b200.so")
 LIB_HOST = os.path.join(PKG_DIR, "librt_host.so")
@@ -87,9 +88,11 @@ def build_host(force: bool = False) -> str:
 
 
 def build_oracle(force: bool = False) -> str:
-    srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(INCLUDE, (".h",))
+    # the oracle (oracle/rt_oracle.cpp) with its per-pixel counters (PixelStats) around it: the extension includes the oracle's
+    # source unchanged and wraps the entry points that reach the counters (tests/oracle_ext/rt_oracle_pixel_stats.cpp)
+    srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(ORACLE_EXT, (".cpp",)) + _glob(INCLUDE, (".h",))
     if force or _newer(LIB_ORACLE, srcs):
-        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE, "rt_oracle.cpp")])
+        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_pixel_stats.cpp")])
     return LIB_ORACLE
 
 

@@ -35,6 +35,12 @@ assert MODEL_DTYPE.itemsize == 224 and SPHERE_DTYPE.itemsize == 104
 
 BUFFER_DTYPES = {"Triangles": TRIANGLE_DTYPE, "Nodes": NODE_DTYPE, "ModelInfo": MODEL_DTYPE, "Spheres": SPHERE_DTYPE}
 
+# RtPixelStats: the per-pixel counters of the counting launches ("countStats" = 1), uint32, wrapping modulo 2^32
+PIXEL_STATS_DTYPE = np.dtype([("rays", "<u4"), ("boxTests", "<u4"), ("triTests", "<u4"), ("sphereTests", "<u4"), ("sphereBoxTests", "<u4")])
+assert PIXEL_STATS_DTYPE.itemsize == 20
+# rtDisplayPixelStats visMode: what the heat map shows per pixel
+VIS_MODES = {1: "boxTests per ray", 2: "triTests per ray", 3: "sphere tests per ray", 4: "rays"}
+
 
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
@@ -94,10 +100,13 @@ class RtLib:
             "rtReadbackAsync": ([vp, cp, vp, C.c_size_t], ci),
             "rtDisplayAsync": ([vp, ci, ci, vp, C.c_size_t], ci),
             "rtReadbackWait": ([vp], ci),
+            "rtReadbackPixelStats": ([vp, vp, C.c_size_t], ci),
+            "rtDisplayPixelStats": ([vp, ci, cf, vp, C.c_size_t], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
-                if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait"):      # absent from older experimental builds used in A/B runs
+                if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
+                            "rtReadbackPixelStats", "rtDisplayPixelStats"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -292,4 +301,19 @@ class RtContext:
         return {k: getattr(s, k) for k, _ in RtStats._fields_}
 
     def reset_stats(self):
+        """rtResetStats: zeroes RtStats and the PixelStats image."""
         self._ck(self._L.rtResetStats(self._h))
+
+    def pixel_stats(self) -> np.ndarray:
+        """rtReadbackPixelStats: (H, W) array of PIXEL_STATS_DTYPE, row 0 = bottom — each pixel's counts over the counting
+        dispatches ("countStats" = 1) since the last reset_stats()."""
+        out = np.empty((self.height, self.width), dtype=PIXEL_STATS_DTYPE)
+        self._ck(self._L.rtReadbackPixelStats(self._h, out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out
+
+    def display_pixel_stats(self, vis_mode: int, debug_vis_scale: float) -> np.ndarray:
+        """rtDisplayPixelStats: heat map of the PixelStats image as (H, W, 4) uint8, row 0 = bottom (VIS_MODES; values above
+        debug_vis_scale are red)."""
+        out = np.empty((self.height, self.width, 4), dtype=np.uint8)
+        self._ck(self._L.rtDisplayPixelStats(self._h, int(vis_mode), float(debug_vis_scale), out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out

@@ -97,6 +97,7 @@ struct RtContext
     // counters / timing
     unsigned long long* dCounters = nullptr;   // 5
     unsigned int* dWork = nullptr;
+    DevBuf<RtPixelStats> pixelStats;           // "PixelStats": W*H per-pixel counters of the counting launches (allocated by the first one)
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -205,6 +206,7 @@ int rtDestroy(RtContext* c)
     c->buildArena.release(); c->handoff.release(); c->poolCold.release();
     for (int k = 0; k < 2; k++) { if (c->stageBuf[k]) cudaFreeHost(c->stageBuf[k]); if (c->stageEv[k]) cudaEventDestroy(c->stageEv[k]); }
     c->frame.release(); c->accum.release(); c->tileSend.release(); c->tileRecv.release(); c->display.release();
+    c->pixelStats.release();
     c->repack.release();
     closePeers(c);
     for (auto& ev : c->pending) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
@@ -362,6 +364,11 @@ static int one_rtResize(RtContext* c, int w, int h)
         CK(c->frame.ensure(n)); CK(c->accum.ensure(n));
         CK(cudaMemsetAsync(c->frame.p, 0, n * 16, c->stream));
         CK(cudaMemsetAsync(c->accum.p, 0, n * 16, c->stream));
+        if (c->pixelStats.p)                                // the per-pixel counters follow the image size, zero-filled
+        {
+            CK(c->pixelStats.ensure(n));
+            CK(cudaMemsetAsync(c->pixelStats.p, 0, n * sizeof(RtPixelStats), c->stream));
+        }
         c->width = w; c->height = h;
         c->tileSend.release(); c->tileRecv.release();
         closePeers(c);                                      // peer mappings refer to images of the old size
@@ -645,6 +652,12 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     int rc = prepareScene(c);
     if (rc != RT_OK) return rc;
     applyL2Persistence(c);
+    if (c->optCountStats && !c->pixelStats.p)              // the first counting dispatch allocates the per-pixel counters
+    {
+        const size_t n = (size_t)W * H;
+        CK(c->pixelStats.ensure(n));
+        CK(cudaMemsetAsync(c->pixelStats.p, 0, n * sizeof(RtPixelStats), c->stream));
+    }
 
     DevParams P = c->P;
     P.limX = limX; P.limY = limY;
@@ -657,6 +670,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     P.sphRootStart = c->repack.sphRootStart; P.sphRootCount = c->repack.sphRootCount; P.smemPairs = c->repack.smemPairs; P.tailLanes = c->optTailLanes; P.sortRays = c->optSortRays; P.gridFit = c->optGridFit;
     P.FrameRender = c->frame.p; P.AccumulatedRender = c->accum.p;
     P.counters = c->dCounters; P.workCounter = c->dWork;
+    P.pixelStats = c->optCountStats ? c->pixelStats.p : nullptr;
     P.nPeers = c->nPeers; P.forceExt = c->optForceExt; P.modelSkip = c->optModelSkip;
     P.tlasPairs = c->repack.tlasPairs.p; P.tlasLeaves = c->repack.tlasLeaves.p; P.tlas = c->repack.tlas;
     P.tlasRootStart = c->repack.tlasRootStart; P.tlasRootCount = c->repack.tlasRootCount;
@@ -697,7 +711,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
             CK(cudaMemsetAsync(c->handoff.p, 0, c->handoff.count * sizeof(unsigned long long), c->stream));
             if (c->chunkSerial == 0u) c->chunkSerial = 1u;
         }
-        P.handoff = c->handoff.p; P.handoffFlags = nullptr; P.chunkSerial = (int)c->chunkSerial;
+        P.handoff = c->handoff.p; P.chunkSerial = (int)c->chunkSerial;
     }
     if (kernel == 0)
     {
@@ -1057,6 +1071,11 @@ int rtGetDevicePointer(RtContext* c, const char* name, void** devPtr, size_t* by
     CK(cudaSetDevice(c->device));
     if (n == "FrameRender") { *devPtr = c->frame.p; *bytes = c->frame.count * 16; }
     else if (n == "AccumulatedRender") { *devPtr = c->accum.p; *bytes = c->accum.count * 16; }
+    else if (n == "PixelStats")
+    {
+        if (!c->pixelStats.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: PixelStats is allocated by the first counting dispatch");
+        *devPtr = c->pixelStats.p; *bytes = c->pixelStats.count * sizeof(RtPixelStats);
+    }
     else if (n == "TileSend" || n == "TileRecv")
     {
         int rc = ensureTileBuffers(c); if (rc != RT_OK) return rc;
@@ -1352,7 +1371,45 @@ static int one_rtResetStats(RtContext* c)
     CK(cudaStreamSynchronize(c->stream));
     int rc = drainEvents(c); if (rc != RT_OK) return rc;
     CK(cudaMemset(c->dCounters, 0, 8 * sizeof(unsigned long long)));
+    if (c->pixelStats.p) CK(cudaMemset(c->pixelStats.p, 0, c->pixelStats.count * sizeof(RtPixelStats)));
     memset(&c->stats, 0, sizeof(c->stats));
+    return RT_OK;
+}
+
+// ---- per-pixel counters ("PixelStats") ----------------------------------------------------------------------------------------
+static int pixelStatsReady(RtContext* c, const char* what)
+{
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, std::string(what) + ": not available on a group context (rtCreateMulti)");
+    if (!c->pixelStats.p) return fail(c, RT_E_STATE, std::string(what) + ": no counting dispatch yet (rtSetOption(\"countStats\", 1))");
+    return RT_OK;
+}
+
+int rtReadbackPixelStats(RtContext* c, RtPixelStats* dst, size_t bytes)
+{
+    if (!c || !dst) return fail(c, RT_E_INVALID, "rtReadbackPixelStats: bad argument");
+    int rc = pixelStatsReady(c, "rtReadbackPixelStats"); if (rc != RT_OK) return rc;
+    if (bytes != c->pixelStats.count * sizeof(RtPixelStats)) return fail(c, RT_E_INVALID, "rtReadbackPixelStats: bytes must equal W*H*20");
+    CK(cudaSetDevice(c->device));
+    CK(cudaMemcpyAsync(dst, c->pixelStats.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rtDisplayPixelStats(RtContext* c, int visMode, float debugVisScale, uint8_t* dst, size_t bytes)
+{
+    if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: bad argument");
+    if (visMode < 1 || visMode > 4) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: visMode must be 1 (box tests), 2 (triangle tests), 3 (sphere tests) or 4 (rays)");
+    if (!std::isfinite(debugVisScale) || !(debugVisScale > 0.0f)) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: debugVisScale must be finite and > 0");
+    int rc = pixelStatsReady(c, "rtDisplayPixelStats"); if (rc != RT_OK) return rc;
+    const size_t n = c->pixelStats.count;
+    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: bytes must equal W*H*4");
+    CK(cudaSetDevice(c->device));
+    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }     // rtDisplayAsync may still read the buffer
+    CK(c->display.ensure(n));
+    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_pixel_stats_display, c->pixelStats.p, c->display.p, n, visMode, debugVisScale);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
     return RT_OK;
 }
 

@@ -206,11 +206,27 @@ struct DevParams
     // kernel 1 on small tiles: a pixel's samples in `chunks` consecutive jobs (1 = whole pixels); the RNG state and the running sum travel
     // from one chunk to the next through `handoff`: four 64-bit words per pixel job, each {tag, value} with tag = chunkSerial << 8 | chunks
     // completed, so that every word validates itself (aligned 8-byte stores are single-copy atomic: no fence, no flag)
-    int   chunks, chunkSerial; unsigned long long* handoff; int* handoffFlags;
+    int   chunks, chunkSerial; unsigned long long* handoff;
+    // "countStats" launches: the W*H per-pixel counters ([y][x], RtPixelStats).  Only the instrumented code reads it (kept at the
+    // offset of a retired pointer so that the parameter layout of every kernel stays where it was)
+    RtPixelStats* pixelStats;
     float* poolCold;                        // kernel 2 built with RT_POOL_COLD_GLOBAL: the per-warp blocks of the slot fields kept out of shared memory
 };
 
 struct Counters { unsigned int rays, box, tri, sph, sbox; };
+
+// Instrumented launches: add one pixel's share of the counters (`now` - `before`, all of it by the lane that traced it) into its
+// PixelStats record.  Relaxed atomics: several lanes may add to one pixel in the same launch (sample chunks, the pooled kernel's
+// rays of one pixel traced by different lanes); the sums are order-independent and wrap modulo 2^32.
+RT_DI void AddPixelStats(const DevParams& P, size_t o, const Counters& now, const Counters& before)
+{
+    unsigned int* r = reinterpret_cast<unsigned int*>(P.pixelStats + o);
+    atomicAdd(r + 0, now.rays - before.rays);
+    atomicAdd(r + 1, now.box - before.box);
+    atomicAdd(r + 2, now.tri - before.tri);
+    atomicAdd(r + 3, now.sph - before.sph);
+    atomicAdd(r + 4, now.sbox - before.sbox);
+}
 
 // RC:18-23: write the pixel of this frame and accumulate; with peers, also store both values into every peer GPU's copy
 // (the all-gather of finished tiles fused into the producing kernel: 32 bytes per pixel per peer over NVLink).

@@ -163,6 +163,7 @@ __global__ void __launch_bounds__(64) k_raytrace_mega(const __grid_constant__ De
 
     const size_t o = (size_t)idy * P.W + idx;
     WritePixel<true>(P, o, pixelCol.x, pixelCol.y, pixelCol.z);
+    if (P.countStats) { Counters zero; zero.rays = zero.box = zero.tri = zero.sph = zero.sbox = 0; AddPixelStats(P, o, cnt, zero); }
     FlushCounters(P, cnt);
 }
 

@@ -280,6 +280,9 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
     __syncthreads();
 
     Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
+    // STATS: the counters when this lane fetched the ray it traces (which may stay in flight across shade phases); the difference
+    // goes to the ray's pixel (the slot's F_XY) when the ray finishes
+    Counters rayStart = cnt;
     bool exhausted = false;                     // warp-uniform: the global pixel queue is empty
     // Fair share: when the image is small for the machine (multi-GPU tiles, small images) a warp fills at most its share of the
     // pixels, so that every SM gets work and — a pixel's samples being one sequential chain — all pixels start in the first round
@@ -493,6 +496,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     myEntry = pool.order[idx];
                     pool.u(F_INFO, myEntry) = (pool.u(F_INFO, myEntry) & ~15u) | PS_FLIGHT;
                     rayPos = pool.get3(F_POS, myEntry); rayDir = pool.get3(F_DIR, myEntry);
+                    if (STATS) rayStart = cnt;
                     cnt.rays++;
 #ifdef RT_CACHE_RAYINV
                     rayInvW = rcp3(rayDir);
@@ -598,6 +602,11 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         pool.f(F_HU, myEntry) = resU; pool.f(F_HV, myEntry) = resV; pool.f(F_HDET, myEntry) = resDet; pool.i(F_HMODEL, myEntry) = resModel;
                         const unsigned info = pool.u(F_INFO, myEntry);
                         pool.u(F_INFO, myEntry) = (info & ~15u) | resKind;
+                        if (STATS)
+                        {
+                            const unsigned xy = pool.u(F_XY, myEntry);
+                            AddPixelStats(P, (size_t)(xy >> 16) * P.W + (xy & 0xffffu), cnt, rayStart);
+                        }
                         mode = T_IDLE; myEntry = -1; fin = true;
                     }
                 }

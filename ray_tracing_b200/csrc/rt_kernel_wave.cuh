@@ -289,6 +289,7 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
     const unsigned int lane = threadIdx.x & 31u;
     const unsigned int laneMaskLt = (1u << lane) - 1u;
     Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
+    Counters pixelStart = cnt;       // STATS: the counters when this lane took its pixel (or chunk); the difference goes to PixelStats
 
     bool exhausted = false;          // no more jobs for this lane
     bool havePixel = false;
@@ -341,6 +342,7 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
                         sample = 0; sampleEnd = P.NumRaysPerPixel;
                         pixelOffset = (size_t)y * P.W + x;
                         havePixel = true; pathActive = false;
+                        if (STATS) pixelStart = cnt;
                         if (CHUNKED && chunks > 1)
                         {
                             chunk = (int)(jobAll / totalJobs); pixJob = job;
@@ -411,6 +413,7 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
                 h[0] = tag | rngState; h[1] = tag | __float_as_uint(totalIncomingLight.x);
                 h[2] = tag | __float_as_uint(totalIncomingLight.y); h[3] = tag | __float_as_uint(totalIncomingLight.z);
             }
+            if (STATS) AddPixelStats(P, pixelOffset, cnt, pixelStart);      // this lane's share: the whole pixel, or this chunk of it
             havePixel = false;
         }
     }

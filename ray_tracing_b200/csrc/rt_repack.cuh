@@ -680,6 +680,22 @@ __global__ void k_display(const float4* __restrict__ tex, uchar4* __restrict__ o
                          (unsigned char)DisplayEncode(t.z / frame), (unsigned char)DisplayEncode(t.w / frame));
 }
 
+// Heat map of the per-pixel counters (rtDisplayPixelStats; the encode is pinned in include/rt_b200.h so that the oracle restates it
+// bit for bit).  The clamp is written as comparisons: t > 1 is red, every other t lies in [0, 1] and needs no saturation.
+__global__ void k_pixel_stats_display(const RtPixelStats* __restrict__ st, uchar4* __restrict__ out, size_t n, int visMode, float scale)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const RtPixelStats s = st[i];
+    if (s.rays == 0u) { out[i] = make_uchar4(0, 0, 0, 255); return; }
+    const unsigned int count = visMode == 1 ? s.boxTests : visMode == 2 ? s.triTests : s.sphereTests + s.sphereBoxTests;
+    const float v = visMode == 4 ? __uint2float_rn(s.rays) : __uint2float_rn(count) / __uint2float_rn(s.rays);
+    const float t = v / scale;
+    if (t > 1.0f) { out[i] = make_uchar4(255, 0, 0, 255); return; }
+    const unsigned char g = (unsigned char)__float2uint_rz(t * 255.0f + 0.5f);
+    out[i] = make_uchar4(g, g, g, 255);
+}
+
 inline void launch_pack_tile(const float4* frame, const float4* accum, float4* send, int W, int H, int rank, int world, int bandRows, int rowsPerRank, cudaStream_t s)
 {
     dim3 grid((W + 255) / 256, rowsPerRank, 1);

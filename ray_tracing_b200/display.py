@@ -24,6 +24,14 @@ class RayTraceDisplay:
     def save_screenshot(self, path: str) -> None:
         write_png(path, self.OnRenderImage()[..., :3])
 
+    def DebugView(self, visMode: int, debugVisScale: float) -> np.ndarray:
+        """The reference's debug view (visMode / debugVisScale, RayCommon.hlsl:24-26): heat map of the per-pixel traversal counters
+        of the counting launches, (H, W, 4) uint8, top row first.  See RayComputeManager.debug_view."""
+        return self.raytracer.debug_view(visMode, debugVisScale)[::-1]
+
+    def save_debug_view(self, path: str, visMode: int, debugVisScale: float) -> None:
+        write_png(path, self.DebugView(visMode, debugVisScale)[..., :3])
+
 
 def write_png(path: str, rgb8: np.ndarray) -> None:
     h, w, _ = rgb8.shape

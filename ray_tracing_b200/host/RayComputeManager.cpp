@@ -26,6 +26,8 @@ std::string RtApi::Load(const char* path)
     CreateMulti = reinterpret_cast<decltype(CreateMulti)>(dlsym(dl, "rtCreateMulti"));
     ReadbackAsync = reinterpret_cast<decltype(ReadbackAsync)>(dlsym(dl, "rtReadbackAsync"));
     ReadbackWait = reinterpret_cast<decltype(ReadbackWait)>(dlsym(dl, "rtReadbackWait"));
+    ReadbackPixelStats = reinterpret_cast<decltype(ReadbackPixelStats)>(dlsym(dl, "rtReadbackPixelStats"));
+    DisplayPixelStats = reinterpret_cast<decltype(DisplayPixelStats)>(dlsym(dl, "rtDisplayPixelStats"));
     return "";
 }
 
@@ -251,6 +253,22 @@ int RayComputeManager::ReadAccumulatedAsync(float* dst, size_t bytes)
     if (!ctx) return RT_E_STATE;
     if (!api.ReadbackAsync) return ReadAccumulated(dst, bytes);
     TRY(api.ReadbackAsync(ctx, "AccumulatedRender", dst, bytes));
+    return RT_OK;
+}
+
+int RayComputeManager::ReadPixelStats(RtPixelStats* dst, size_t bytes)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.ReadbackPixelStats) { lastError = "the library does not export rtReadbackPixelStats"; return RT_E_STATE; }
+    TRY(api.ReadbackPixelStats(ctx, dst, bytes));
+    return RT_OK;
+}
+
+int RayComputeManager::DisplayDebugView(int visMode, float debugVisScale, uint8_t* dst, size_t bytes)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.DisplayPixelStats) { lastError = "the library does not export rtDisplayPixelStats"; return RT_E_STATE; }
+    TRY(api.DisplayPixelStats(ctx, visMode, debugVisScale, dst, bytes));
     return RT_OK;
 }
 

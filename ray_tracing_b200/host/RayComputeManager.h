@@ -55,6 +55,7 @@ struct RtApi
     decltype(&rtBuildBVH) BuildBVH = nullptr;   // optional: absent from older builds of the library
     decltype(&rtReadbackAsync) ReadbackAsync = nullptr; decltype(&rtReadbackWait) ReadbackWait = nullptr;   // optional: pipelined readback
     decltype(&rtCreateMulti) CreateMulti = nullptr;   // optional: several GPUs behind one context (the all-gather of tiles inside rtDispatch)
+    decltype(&rtReadbackPixelStats) ReadbackPixelStats = nullptr; decltype(&rtDisplayPixelStats) DisplayPixelStats = nullptr;   // optional: debug view
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -116,6 +117,10 @@ public:
     int ReadAccumulated(float* dst, size_t bytes);
     int ReadAccumulatedAsync(float* dst, size_t bytes);      // returns at once; dst is valid after WaitReadback()
     int WaitReadback();
+    // the reference's debug view (HL:24-26): per-pixel traversal counters of the counting launches (rtSetOption "countStats" = 1) and
+    // their heat map (visMode 1 box tests / ray, 2 triangle tests / ray, 3 sphere tests / ray, 4 rays; debugVisScale = full white)
+    int ReadPixelStats(RtPixelStats* dst, size_t bytes);
+    int DisplayDebugView(int visMode, float debugVisScale, uint8_t* dst, size_t bytes);
     RtContext* Context() const { return ctx; }
     const RtApi& Api() const { return api; }
 

@@ -230,6 +230,9 @@ int rcmResetAccumulatedRender(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try
 int rcmRenderFrame(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFrame(); } CATCH_ALL(h) }
 int rcmReadFrame(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadFrame(dst, bytes); }
 int rcmReadAccumulated(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadAccumulated(dst, bytes); }
+int rcmReadPixelStats(void* hv, RtPixelStats* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadPixelStats(dst, bytes); }
+int rcmDisplayDebugView(void* hv, int visMode, float debugVisScale, uint8_t* dst, size_t bytes)
+{ Handle* h = (Handle*)hv; GUARD(h); return h->mgr->DisplayDebugView(visMode, debugVisScale, dst, bytes); }
 
 /* BVH statistics of the last build: writes up to cap entries of 9 ints each (see rthBuildBVH); returns the mesh count */
 int rcmGetBVHStats(void* hv, int* out, int cap)

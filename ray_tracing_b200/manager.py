@@ -60,6 +60,8 @@ def host_lib() -> C.CDLL:
         L.rcmReadFrame.argtypes = [vp, vp, C.c_size_t]
         L.rcmReadAccumulated.argtypes = [vp, vp, C.c_size_t]
         L.rcmGetBVHStats.argtypes = [vp, vp, ci]
+        L.rcmReadPixelStats.argtypes = [vp, vp, C.c_size_t]
+        L.rcmDisplayDebugView.argtypes = [vp, ci, cf, vp, C.c_size_t]
         _host = L
     return _host
 
@@ -248,6 +250,23 @@ class RayComputeManager:
 
     def read_accumulated_into(self, ptr: int, nbytes: int):
         self._ck(self._L.rcmReadAccumulated(self._h, C.c_void_p(ptr), nbytes))
+
+    # -- the reference's debug view (visMode / debugVisScale, RayCommon.hlsl:24-26): per-pixel cost of the counting launches
+    def pixel_stats(self) -> np.ndarray:
+        """(H, W) array of capi.PIXEL_STATS_DTYPE, row 0 = bottom: each pixel's rays, box / triangle / sphere tests over the frames
+        rendered with context.set_option("countStats", 1) since the last context.reset_stats()."""
+        w, h = self._size
+        out = np.empty((h, w), dtype=capi.PIXEL_STATS_DTYPE)
+        self._ck(self._L.rcmReadPixelStats(self._h, out.ctypes.data, out.nbytes))
+        return out
+
+    def debug_view(self, visMode: int, debugVisScale: float) -> np.ndarray:
+        """Heat map of pixel_stats() as (H, W, 4) uint8, row 0 = bottom.  visMode 1: box tests per ray, 2: triangle tests per ray,
+        3: sphere tests per ray, 4: rays per pixel; debugVisScale is shown as white, anything above it as red."""
+        w, h = self._size
+        out = np.empty((h, w, 4), dtype=np.uint8)
+        self._ck(self._L.rcmDisplayDebugView(self._h, int(visMode), float(debugVisScale), out.ctypes.data, out.nbytes))
+        return out
 
     def bvh_stats(self) -> list[dict]:
         buf = np.zeros(9 * 64, dtype=np.int32)

@@ -4,7 +4,10 @@ emissive materials, sky, defocus, near / far / inside cameras, extreme scales) r
 interpreter build (tests/simt) with random options, compared bit for bit with the oracle.  Found the distant-camera defect of the
 model skipping in round 1 by hand-made cases; this keeps looking.  Every failure prints the seed that reproduces it.
 
-    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so]
+    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats]
+
+--pixel-stats: wherever the traversal totals are compared (counting launches of whole images), also compare the per-pixel counters
+(PixelStats: rays, box and triangle tests everywhere; sphere tests too when the Spheres buffer is below the accelerator's threshold).
 """
 import argparse
 import os
@@ -19,7 +22,32 @@ sys.path.insert(0, os.path.join(REPO, "tests"))
 sys.path.insert(0, os.path.join(REPO, "tests", "simt"))
 import build as simt_build                      # noqa: E402
 from conftest import ORACLE_LIB, render        # noqa: E402
+import ray_tracing_b200 as rt                   # noqa: E402
 from ray_tracing_b200 import scenes             # noqa: E402
+
+
+def render_pixel_stats(lib, sc, frames, options, tile=None):
+    """conftest.render plus the PixelStats image of the frames (None unless the launch counts)."""
+    mgr = rt.RayComputeManager(lib)
+    scenes.apply(sc, mgr)
+    ctx = mgr.context
+    for k, v in (options or {}).items():
+        ctx.set_option(k, v)
+    if tile:
+        ctx.set_tile(*tile)
+    mgr.OnEnable()
+    ctx.reset_stats()
+    for _ in range(frames):
+        mgr.RenderFrame()
+    out = (mgr.raytraceFrameTex, mgr.accumulatedResult, ctx.stats(), mgr.pixel_stats() if (options or {}).get("countStats") else None)
+    mgr.OnDestroy()
+    return out
+
+
+def pixel_stats_differ(a, b, spheres):
+    """Fields of two PixelStats images that differ (sphere tests only below the 65 spheres where the accelerator starts)."""
+    keys = ("rays", "boxTests", "triTests") + (("sphereTests",) if spheres <= 64 else ())
+    return [k for k in keys if not np.array_equal(a[k], b[k])]
 
 
 def random_material(rng):
@@ -163,9 +191,10 @@ def main():
     ap.add_argument("--odd", type=float, default=0.06, help="share of cases with NaN / inf / zero / negative numbers in spheres, matrices, materials, camera")
     ap.add_argument("--spheres", type=float, default=0.05, help="share of cases of the large-Spheres-buffer class")
     ap.add_argument("--far", type=float, default=0.05, help="share of cases of the many-small-models-from-afar class")
+    ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters wherever the totals are compared")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
-    bad, t0 = 0, time.time()
+    bad, pix_cases, t0 = 0, 0, time.time()
     for case in range(args.cases):
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
@@ -175,9 +204,14 @@ def main():
         # (the pooled kernel is slow on the interpreter with 1,000 models: it gets the smaller far scenes only)
         opts = {"kernel": 2 if len(sc.models) <= 150 and rng.rand() < 0.5 else 1, "tlas": int(rng.choice([0, 1]))} if far else random_options(rng)
         tile = (int(rng.randint(0, 3)), 3, int(rng.choice([1, 4, 8]))) if rng.rand() < 0.15 else None
+        pix_case = args.pixel_stats and tile is None and bool(opts.get("countStats"))
         try:
-            fo, ao, so = render(ORACLE_LIB, sc, frames=frames, want_stats=True)
-            fg, ag, sg = render(lib, sc, frames=frames, options=opts, want_stats=True, tile=tile)
+            if pix_case:
+                fo, ao, so, po = render_pixel_stats(ORACLE_LIB, sc, frames, {"countStats": 1})
+                fg, ag, sg, pg = render_pixel_stats(lib, sc, frames, opts)
+            else:
+                fo, ao, so = render(ORACLE_LIB, sc, frames=frames, want_stats=True)
+                fg, ag, sg = render(lib, sc, frames=frames, options=opts, want_stats=True, tile=tile)
         except Exception as e:                    # an error code from either side is a finding too
             print(f"case seed {seed}: {type(e).__name__}: {e}   options {opts}", flush=True)
             bad += 1
@@ -186,13 +220,16 @@ def main():
         a, b = ag[rows], ao[rows]
         diff = (a.view(np.uint32) != b.view(np.uint32)) & ~(np.isnan(a) & np.isnan(b))
         counters_ok = tile is not None or not opts.get("countStats") or all(sg[k] == so[k] for k in ("rays", "boxTests", "triTests"))
-        if diff.any() or not counters_ok:
+        pix_bad = pixel_stats_differ(pg, po, len(sc.spheres)) if pix_case else []
+        if pix_case:
+            pix_cases += 1
+        if diff.any() or not counters_ok or pix_bad:
             bad += 1
-            print(f"case seed {seed}: {int(diff.sum())} values differ, counters {'ok' if counters_ok else 'DIFFER'}; {len(sc.models)} models, {len(sc.spheres)} spheres, "
+            print(f"case seed {seed}: {int(diff.sum())} values differ, counters {'ok' if counters_ok else 'DIFFER'}, PixelStats {pix_bad or 'ok'}; {len(sc.models)} models, {len(sc.spheres)} spheres, "
                   f"{sc.width}x{sc.height}, frames {frames}, options {opts}, tile {tile}, settings {sc.settings}", flush=True)
         if (case + 1) % 25 == 0:
             print(f"  {case + 1} cases, {bad} findings, {time.time() - t0:.0f} s", flush=True)
-    print(f"{args.cases} cases, {bad} findings")
+    print(f"{args.cases} cases, {bad} findings" + (f"; PixelStats compared in {pix_cases} cases" if args.pixel_stats else ""))
     return 1 if bad else 0
 
 

@@ -5,7 +5,11 @@ resizes, accumulation resets, settings and kernel options that change between fr
 manager against the oracle and against the kernels, compared bit for bit after every frame.  What it exercises is the host-side
 state of csrc/rt_api.cu: dirty flags, cached repacks, the regions the padded boxes were built for, kernel selection.
 
-    python tools/simt_fuzz_session.py [--cases 100] [--seed 1] [--steps 8]
+    python tools/simt_fuzz_session.py [--cases 100] [--seed 1] [--steps 8] [--pixel-stats]
+
+--pixel-stats: both sides count from the start ("countStats" = 1, and the script's countStats switches reach the oracle too), and after
+every frame the per-pixel counters (PixelStats rays, box and triangle tests) are compared as well: accumulation across frames, resizes,
+partial state changes.
 """
 import argparse
 import os
@@ -69,7 +73,7 @@ def make_script(rng, sc, steps):
     return script
 
 
-def apply(mgr, action, args, kernels_side):
+def apply(mgr, action, args, kernels_side, pixel_stats=False):
     if action == "camera":
         mgr.set_camera(*args)
     elif action == "model":
@@ -87,8 +91,16 @@ def apply(mgr, action, args, kernels_side):
         value = {"maxBounceCount": int(u * 7), "numRaysPerPixel": 1 + int(u * 3), "useSky": u < 0.5, "accumulate": u < 0.7,
                  "divergeStrength": float(u * 2), "defocusStrength": float(u < 0.3) * 30.0}[name]
         setattr(mgr, name, value)
-    elif action == "option" and kernels_side:
+    elif action == "option" and (kernels_side or (pixel_stats and args[0] == "countStats")):
         mgr.context.set_option(*args)
+
+
+def read_pixel_stats(mgr):
+    """The manager's PixelStats image, or the RT_E_* code when it has none (no counting frame yet)."""
+    try:
+        return mgr.pixel_stats()
+    except rt.capi.RtError as e:
+        return e.code
 
 
 def main():
@@ -97,6 +109,7 @@ def main():
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--steps", type=int, default=8)
     ap.add_argument("--lib", default=None)
+    ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters after every frame")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
     bad = 0
@@ -109,6 +122,8 @@ def main():
         for backend in (ORACLE_LIB, lib):
             m = rt.RayComputeManager(backend)
             scenes.apply(sc, m)
+            if args.pixel_stats:
+                m.context.set_option("countStats", 1)
             m.OnEnable()
             mgrs.append(m)
         frame_no, failed, resized = 0, None, False
@@ -133,11 +148,22 @@ def main():
                         if x.shape != y.shape or diff.any():
                             failed = f"{what} differs after frame {frame_no} ({int(diff.sum()) if x.shape == y.shape else 'shape'})"
                             break
+                    if not failed and args.pixel_stats:
+                        # before the first counting frame (the script may switch counting off at once) both sides answer RT_E_STATE
+                        got = [read_pixel_stats(m) for m in mgrs]
+                        po, pg = got
+                        if isinstance(po, int) or isinstance(pg, int):
+                            if po != pg:
+                                failed = f"PixelStats readable on one side only after frame {frame_no} ({po if isinstance(po, int) else 'ok'} vs {pg if isinstance(pg, int) else 'ok'})"
+                        else:
+                            bad_fields = [k for k in ("rays", "boxTests", "triTests") if po.shape != pg.shape or not np.array_equal(po[k], pg[k])]
+                            if bad_fields:
+                                failed = f"PixelStats {bad_fields} differ after frame {frame_no}"
                     if failed:
                         break
                 else:
-                    apply(mgrs[0], action, a, False)
-                    apply(mgrs[1], action, a, True)
+                    apply(mgrs[0], action, a, False, args.pixel_stats)
+                    apply(mgrs[1], action, a, True, args.pixel_stats)
         except Exception as e:
             failed = f"{type(e).__name__}: {e}"
         for m in mgrs:
