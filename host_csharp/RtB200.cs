@@ -24,6 +24,7 @@ public static class RtB200
     [DllImport(Lib)] public static extern int rtSetBool(IntPtr ctx, string name, int value);
     [DllImport(Lib)] public static extern int rtResize(IntPtr ctx, int width, int height);
     [DllImport(Lib)] public static extern int rtDispatch(IntPtr ctx, int kernelIndex, int gx, int gy, int gz);
+    [DllImport(Lib)] public static extern int rtDispatchFrames(IntPtr ctx, int gx, int gy, int gz, int frameCount);
     [DllImport(Lib)] public static extern int rtReadback(IntPtr ctx, string tex, float[] dst, UIntPtr bytes);
     [DllImport(Lib)] public static extern int rtSynchronize(IntPtr ctx);
     // optional: new BVH(verts, indices, normals, quality) built on the GPU — the same Triangles / Nodes arrays (BVH.cs:26)

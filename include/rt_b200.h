@@ -83,6 +83,25 @@ int rtResize(RtContext* ctx, int width, int height);
  * are left untouched, like threads that were never launched.  Asynchronous. */
 int rtDispatch(RtContext* ctx, int kernelIndex, int groupsX, int groupsY, int groupsZ);
 
+/* Extension: n = frameCount accumulated frames of RayTrace in one launch (a still rendered to many frames, RCM:84-95 called n times).
+ * With F the current "Frame" uniform, the call is equal, in every byte the context exposes, to
+ *     for k in 0 .. n-1:  rtSetInt("Frame", F + k); rtDispatch(RT_KERNEL_RAYTRACE, groupsX, groupsY, groupsZ)
+ *     rtSetInt("Frame", F)
+ * with F + k taken modulo 2^32 like the seed (HL:552):
+ *   - FrameRender holds frame F + n - 1; AccumulatedRender receives the n frames' (col, 1) per pixel in frame order, with the same
+ *     float additions (one thread or pool slot owns a pixel for all n frames);
+ *   - RtStats rays / boxTests / triTests / sphereTests / sphereBoxTests and PixelStats equal the n dispatches' totals; dispatches
+ *     grows by n; kernelMs is the one launch's time;
+ *   - "Frame" is unchanged afterwards.
+ * Partial dispatch, rtSetTile row bands, peers and the sphere accelerator behave as in rtDispatch.  On a group context (rtCreateMulti,
+ * rtCommInit) the call reaches every GPU and, with "exchange" = 1, ends with ONE exchange of the tiles for the whole batch.
+ * n = 1 is rtDispatch(RT_KERNEL_RAYTRACE, ...).  Asynchronous.
+ * Refused: frameCount < 1 or frameCount * max(1, NumRaysPerPixel) > RT_MAX_BATCH_SAMPLES (the pooled kernel counts a slot's samples
+ * across the batch in a 20-bit field) -> RT_E_INVALID; "accumulate" = 0 (only the last frame would be observable) -> RT_E_STATE;
+ * n > 1 with "sampleChunks" forced to 2 or more (a batch runs whole pixels; the automatic setting does) -> RT_E_STATE. */
+#define RT_MAX_BATCH_SAMPLES ((1 << 20) - 1)
+int rtDispatchFrames(RtContext* ctx, int groupsX, int groupsY, int groupsZ, int frameCount);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),

@@ -18,6 +18,7 @@ DEFAULT_LIB = os.path.join(PKG_DIR, "librt_b200.so")
 RT_OK = 0
 RT_E_INVALID, RT_E_UNKNOWN_NAME, RT_E_NO_DEVICE, RT_E_CUDA, RT_E_STATE = -1, -2, -3, -4, -5
 RT_KERNEL_RAYTRACE, RT_KERNEL_RESET_ACCUMULATED = 0, 1
+RT_MAX_BATCH_SAMPLES = (1 << 20) - 1      # rtDispatchFrames: frameCount * max(1, NumRaysPerPixel) at most this
 
 # numpy dtypes of the blittable structs in include/rt_types.h
 MATERIAL_DTYPE = np.dtype([
@@ -102,11 +103,12 @@ class RtLib:
             "rtReadbackWait": ([vp], ci),
             "rtReadbackPixelStats": ([vp, vp, C.c_size_t], ci),
             "rtDisplayPixelStats": ([vp, ci, cf, vp, C.c_size_t], ci),
+            "rtDispatchFrames": ([vp, ci, ci, ci, ci], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
-                            "rtReadbackPixelStats", "rtDisplayPixelStats"):      # absent from older experimental builds used in A/B runs
+                            "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -210,6 +212,13 @@ class RtContext:
     def dispatch_full(self, kernel: int = RT_KERNEL_RAYTRACE):
         """ComputeHelper.Dispatch(cs, width, height, kernelIndex) (ComputeHelper.cs:25-32)."""
         self.dispatch(kernel, (self.width + 7) // 8, (self.height + 7) // 8, 1)
+
+    def dispatch_frames(self, n: int, gx: Optional[int] = None, gy: Optional[int] = None, gz: int = 1):
+        """rtDispatchFrames: n accumulated RayTrace frames, Frame .. Frame + n - 1, in one launch — the same bytes as n dispatch()
+        calls with "Frame" stepped by one each time; "Frame" is left unchanged.  Groups default to the whole image."""
+        gx = (self.width + 7) // 8 if gx is None else gx
+        gy = (self.height + 7) // 8 if gy is None else gy
+        self._ck(self._L.rtDispatchFrames(self._h, int(gx), int(gy), int(gz), int(n)))
 
     def readback(self, tex: str, out: Optional[np.ndarray] = None) -> np.ndarray:
         if out is None:

@@ -48,6 +48,7 @@ struct RtContext
     cudaStream_t ownStream = nullptr, stream = nullptr;
     int numSMs = 0;
     unsigned long long dispatchPixels = 0;     // pixels of the RayTrace dispatch being prepared (this rank's tile): enters the automatic kernel choice
+    int dispatchFrames = 1;                    // frames of that dispatch (rtDispatchFrames): a pixel's chain is dispatchFrames * NumRaysPerPixel samples
     std::string err;
 
     // uniforms (host copy)
@@ -518,7 +519,8 @@ static int effectiveKernel(const RtContext* c)
     if (c->optKernel >= 0) return c->optKernel;
     if (c->P.modelCount <= 0) return 1;
     const double slots = (double)c->numSMs * POOL_WARPS * 64.0;
-    const double threshold = c->P.NumRaysPerPixel <= 1 ? RT_SMALL_TILE_PIXELS_PER_SLOT_1SPP : RT_SMALL_TILE_PIXELS_PER_SLOT;
+    const long long chain = (long long)c->P.NumRaysPerPixel * c->dispatchFrames;      // samples one slot runs for a pixel
+    const double threshold = chain <= 1 ? RT_SMALL_TILE_PIXELS_PER_SLOT_1SPP : RT_SMALL_TILE_PIXELS_PER_SLOT;
     if (c->dispatchPixels > 0 && (double)c->dispatchPixels < threshold * slots) return 1;
     return 2;
 }
@@ -620,7 +622,8 @@ static int prepareScene(RtContext* c)
 }
 
 // One GPU's share of a dispatch: the RayTrace kernel over this context's tile (the whole image without rtSetTile).
-static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
+// frames > 1 (rtDispatchFrames, RayTrace only): frames Frame .. Frame + frames - 1 in one launch of a FRAMES kernel.
+static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, int frames = 1)
 {
     if (!c || gx < 0 || gy < 0 || gz < 0) return fail(c, RT_E_INVALID, "rtDispatch: bad argument");
     if (c->width == 0) return fail(c, RT_E_STATE, "rtDispatch: rtResize has not been called");
@@ -649,6 +652,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
             if ((int)(b % (unsigned int)c->tileWorld) == c->tileRank) rows += (limY - y0) < (unsigned int)c->bandRows ? (limY - y0) : (unsigned int)c->bandRows;
         c->dispatchPixels = rows * limX;
     }
+    c->dispatchFrames = frames;
     int rc = prepareScene(c);
     if (rc != RT_OK) return rc;
     applyL2Persistence(c);
@@ -674,6 +678,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     P.nPeers = c->nPeers; P.forceExt = c->optForceExt; P.modelSkip = c->optModelSkip;
     P.tlasPairs = c->repack.tlasPairs.p; P.tlasLeaves = c->repack.tlasLeaves.p; P.tlas = c->repack.tlas;
     P.tlasRootStart = c->repack.tlasRootStart; P.tlasRootCount = c->repack.tlasRootCount;
+    P.frames = frames;
     {
         // camOrigin = M * (0,0,0,1) as SetupPixel computes it (left to right, unfused): exact zero components and non-finite axes rule the shortcut out
         bool ok = c->P.DefocusStrength == 0.0f && c->optZeroDefocus != 0;
@@ -696,7 +701,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     // sample chunks (small tiles): a pixel's chain may change lanes / slots between samples; the hand-off buffers belong to the context
     // (kernel 1 only: in the pooled kernel the same hand-off was slower than whole pixels on small tiles and was taken out again)
     P.chunks = kernel == 1 ? wave_chunks(c->optSampleChunks, c->numSMs, c->dispatchPixels, P.NumRaysPerPixel, P.modelCount) : 1;
-    if (c->dispatchPixels == 0) P.chunks = 1;        // a rank whose tile is empty (an image lower than the band pattern)
+    if (c->dispatchPixels == 0 || frames > 1) P.chunks = 1;      // a rank whose tile is empty (an image lower than the band pattern); a batch of frames runs whole pixels
     if (P.chunks > 1)
     {
         unsigned long long rows = limX ? c->dispatchPixels / limX : 0;
@@ -717,7 +722,8 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     {
         CK(cudaEventRecord(ev.a, c->stream));
         dim3 grid((limX + 7) / 8, (limY + 7) / 8, 1), block(8, 8, 1);
-        RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega, P);
+        if (frames > 1) RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega_frames, P);
+        else RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega, P);
         CK(cudaEventRecord(ev.b, c->stream));
     }
     else if (kernel == 1)
@@ -737,7 +743,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     }
     CK(cudaGetLastError());
     c->pending.push_back(ev);
-    c->stats.dispatches++;
+    c->stats.dispatches += (unsigned long long)frames;
     return RT_OK;
 }
 
@@ -956,6 +962,28 @@ int rtDispatch(RtContext* c, int kernelIndex, int gx, int gy, int gz)
     const bool traced = kernelIndex == RT_KERNEL_RAYTRACE && gz != 0 && gx > 0 && gy > 0;
     if (!traced || !exchanges(c)) return RT_OK;
     std::vector<RtContext*> all(1, c);
+    all.insert(all.end(), c->followers.begin(), c->followers.end());
+    return exchangeTiles(all.data(), (int)all.size());
+}
+
+int rtDispatchFrames(RtContext* c, int gx, int gy, int gz, int frameCount)
+{
+    if (!c) return RT_E_INVALID;
+    if (c->leader) return fail(c, RT_E_STATE, "rtDispatchFrames: this context belongs to a group; dispatch on the context rtCreateMulti returned");
+    const long long chain = (long long)frameCount * (c->P.NumRaysPerPixel > 1 ? c->P.NumRaysPerPixel : 1);
+    if (frameCount < 1 || chain > RT_MAX_BATCH_SAMPLES)
+        return fail(c, RT_E_INVALID, "rtDispatchFrames: frameCount must be >= 1 and frameCount * max(1, NumRaysPerPixel) at most RT_MAX_BATCH_SAMPLES");
+    if (!c->P.accumulate) return fail(c, RT_E_STATE, "rtDispatchFrames: needs accumulate = 1 (without accumulation only the last frame is observable)");
+    if (frameCount == 1) return rtDispatch(c, RT_KERNEL_RAYTRACE, gx, gy, gz);
+    if (c->optSampleChunks >= 2) return fail(c, RT_E_STATE, "rtDispatchFrames: a batch of frames runs whole pixels; sampleChunks is forced to 2 or more");
+    int rc = dispatchLocal(c, RT_KERNEL_RAYTRACE, gx, gy, gz, frameCount);
+    if (rc != RT_OK) return rc;
+    for (RtContext* m : c->followers)
+        if ((rc = dispatchLocal(m, RT_KERNEL_RAYTRACE, gx, gy, gz, frameCount)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
+    if (!c->followers.empty()) CK(cudaSetDevice(c->device));
+    const bool traced = gz != 0 && gx > 0 && gy > 0;
+    if (!traced || !exchanges(c)) return RT_OK;
+    std::vector<RtContext*> all(1, c);                      // one exchange for the whole batch: it carries the last frame and the sum
     all.insert(all.end(), c->followers.begin(), c->followers.end());
     return exchangeTiles(all.data(), (int)all.size());
 }

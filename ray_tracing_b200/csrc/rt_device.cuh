@@ -194,7 +194,7 @@ struct DevParams
     float4* peerAccum[RT_MAX_PEERS];
     int   nPeers;
     int   modelSkip;                        // skip models whose padded world box the ray cannot reach (exact; default on)
-    int   pad7;
+    int   frames;                           // rtDispatchFrames: frames Frame .. Frame + frames - 1 of every pixel in one launch (only the FRAMES kernels read it)
     int   forceExt;                         // testing: run the <EXT = true> instantiation although no extension is active
     unsigned long long* counters;           // [0] rays [1] boxTests [2] triTests [3] sphereTests [4] sphere-accelerator box tests
     unsigned int* workCounter;              // persistent kernel: next job
@@ -741,6 +741,9 @@ RT_DI PixelSetup SetupPixel(const DevParams& P, unsigned int idx, unsigned int i
     s.camUp = make_f3(P.cam[4], P.cam[5], P.cam[6]);
     return s;
 }
+
+// Seed of frame Frame + k of the pixel whose frame-Frame seed is `seed` (HL:552: the frame enters as Frame * 719393, modulo 2^32)
+RT_DI uint32_t FrameSeed(uint32_t seed, unsigned int k) { return seed + k * 719393u; }
 
 // One camera sample (HL:567-576): consumes four draws, returns the path's initial state
 RT_DI void GenerateCameraRay(const DevParams& P, const PixelSetup& s, uint32_t& rngState, PathState& ray)

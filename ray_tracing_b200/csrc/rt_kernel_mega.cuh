@@ -167,4 +167,38 @@ __global__ void __launch_bounds__(64) k_raytrace_mega(const __grid_constant__ De
     FlushCounters(P, cnt);
 }
 
+// rtDispatchFrames: k_raytrace_mega for frames Frame .. Frame + P.frames - 1 of the thread's pixel, one after the other, each written
+// and accumulated as its own dispatch would.  (A kernel of its own: folding the frame loop into k_raytrace_mega changed that kernel's code.)
+__global__ void __launch_bounds__(64) k_raytrace_mega_frames(const __grid_constant__ DevParams P)
+{
+    const unsigned int idx = blockIdx.x * 8u + threadIdx.x;
+    const unsigned int idy = blockIdx.y * 8u + threadIdx.y;
+    if (idx >= P.limX || idy >= P.limY) return;
+    if ((int)((idy / (unsigned int)P.bandRows) % (unsigned int)P.tileWorld) != P.tileRank) return;
+
+    Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
+    const PixelSetup px = SetupPixel(P, idx, idy);
+    const size_t o = (size_t)idy * P.W + idx;
+    for (int frame = 0; frame < P.frames; frame++)
+    {
+        uint32_t rngState = FrameSeed(px.rngState, (unsigned int)frame);
+        f3 totalIncomingLight = splat3(0.0f);
+        for (int rayIndex = 0; rayIndex < P.NumRaysPerPixel; rayIndex++)
+        {
+            PathState ray;
+            GenerateCameraRay(P, px, rngState, ray);
+            for (int i = 0; i <= P.MaxBounceCount; i++)
+            {
+                const Hit hit = CalculateRayCollision_ref(P, ray.pos, ray.dir, cnt);
+                if (!ShadeSegment(P, hit, ray, rngState)) break;
+            }
+            totalIncomingLight = totalIncomingLight + ray.totalLight;
+        }
+        const f3 pixelCol = totalIncomingLight / __int2float_rn(P.NumRaysPerPixel);
+        WritePixel<true>(P, o, pixelCol.x, pixelCol.y, pixelCol.z);
+    }
+    if (P.countStats) { Counters zero; zero.rays = zero.box = zero.tri = zero.sph = zero.sbox = 0; AddPixelStats(P, o, cnt, zero); }
+    FlushCounters(P, cnt);
+}
+
 } // namespace rtd

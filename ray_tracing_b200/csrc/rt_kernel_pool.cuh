@@ -230,7 +230,10 @@ template <int M> RT_DI int CompactRaysByOctant(const PoolView<M>& pool, unsigned
 // The kernel body.  TLAS = the many-model instantiation (k_raytrace_pool_tlas): at the start of a ray's model loop one walk of the
 // TLAS marks the models the ray can reach (TlasCollect, rt_device.cuh); the T_NEXT step then jumps from marked model to marked model,
 // in buffer order, re-testing each against the running result.  The kernels measured in round 1 are the TLAS = false instantiations.
-template <bool STATS, bool EXT, bool TLAS, int M>
+// FRAMES = the batch instantiations of rtDispatchFrames: a slot keeps its pixel for frames Frame .. Frame + P.frames - 1.  The sample
+// field of the info word counts the samples of all of them (frame = sample / NumRaysPerPixel); when a frame's samples end the slot
+// writes and accumulates that frame, reseeds and starts the next one instead of freeing itself.
+template <bool STATS, bool EXT, bool TLAS, int M, bool FRAMES = false>
 RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const unsigned int tilesX, const unsigned int ownedRows)
 {
     RT_DYNAMIC_SMEM(smemRaw);
@@ -374,7 +377,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     {
                         const f3 sum = pool.get3(F_SUM, e) + ray.totalLight;              // HL:578
                         sample++;
-                        if ((int)sample >= P.NumRaysPerPixel)
+                        if (FRAMES ? sample % (unsigned)P.NumRaysPerPixel == 0u : (int)sample >= P.NumRaysPerPixel)
                         {
                             // pixel finished (RC:18-23)
                             const unsigned xy = pool.u(F_XY, e);
@@ -382,6 +385,13 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                             const f3 pixelCol = sum / __int2float_rn(P.NumRaysPerPixel);
                             WritePixel<EXT>(P, o, pixelCol.x, pixelCol.y, pixelCol.z);
                             state = PS_EMPTY;
+                            if (FRAMES && sample < (unsigned)P.NumRaysPerPixel * (unsigned)P.frames)
+                            {
+                                // the pixel's next frame on the same slot
+                                pool.u(F_RNG, e) = FrameSeed(SetupPixel(P, xy & 0xffffu, xy >> 16).rngState, sample / (unsigned)P.NumRaysPerPixel);
+                                pool.set3(F_SUM, e, splat3(0.0f));
+                                state = PS_GEN;
+                            }
                         }
                         else { pool.set3(F_SUM, e, sum); state = PS_GEN; }
                         bounce = 0;
@@ -774,6 +784,21 @@ __global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_tlas(const __
     pool_body<false, true, true, M>(P, totalJobs, tilesX, ownedRows);
 }
 
+// rtDispatchFrames: P.frames frames of every pixel in one launch (kernels of their own, so that the kernels above keep their code)
+template <bool STATS, bool EXT, int M>
+__global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_frames(const __grid_constant__ DevParams P, const unsigned int totalJobs,
+                                                                         const unsigned int tilesX, const unsigned int ownedRows)
+{
+    pool_body<STATS, EXT, false, M, true>(P, totalJobs, tilesX, ownedRows);
+}
+
+template <int M>
+__global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_tlas_frames(const __grid_constant__ DevParams P, const unsigned int totalJobs,
+                                                                              const unsigned int tilesX, const unsigned int ownedRows)
+{
+    pool_body<false, true, true, M, true>(P, totalJobs, tilesX, ownedRows);
+}
+
 template <int M> inline size_t pool_smem_bytes(const DevParams& P)
 {
     const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
@@ -787,6 +812,11 @@ template <int M> inline cudaError_t pool_configure_one()
     if ((e = cudaFuncSetAttribute(k_raytrace_pool<true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_pool<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<false, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas_frames<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
     return cudaFuncSetAttribute(k_raytrace_pool<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
 }
 inline cudaError_t pool_configure()
@@ -820,7 +850,15 @@ template <int M> inline cudaError_t pool_launch_m(const DevParams& P, int numSMs
     if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
     if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
     const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;   // extensions (peer stores, sphere accelerator, staged tree tops) compiled into their own instantiation
-    if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<true, true, M>), P, totalJobs, tilesX, ownedRows);
+    if (P.frames > 1)      // a batch of frames (rtDispatchFrames): the FRAMES kernels, chosen like the single-frame ones
+    {
+        if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<true, true, M>), P, totalJobs, tilesX, ownedRows);
+                            else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<true, false, M>), P, totalJobs, tilesX, ownedRows); }
+        else if (P.tlas && P.modelSkip) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_tlas_frames<M>), P, totalJobs, tilesX, ownedRows);
+        else { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<false, true, M>), P, totalJobs, tilesX, ownedRows);
+               else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<false, false, M>), P, totalJobs, tilesX, ownedRows); }
+    }
+    else if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<true, true, M>), P, totalJobs, tilesX, ownedRows);
                         else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<true, false, M>), P, totalJobs, tilesX, ownedRows); }
     else if (P.tlas && P.modelSkip) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_tlas<M>), P, totalJobs, tilesX, ownedRows);
     else { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<false, true, M>), P, totalJobs, tilesX, ownedRows);

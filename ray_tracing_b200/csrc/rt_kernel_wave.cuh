@@ -248,8 +248,9 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
 #define RT_WAVE_MINBLOCKS 6      // <= 85 registers: 24 warps per SM (faster than 16 warps on config 2)
 #endif
 // The kernel body.  TLAS = the many-model instantiation (its own kernel, k_raytrace_wave_tlas, so that the kernels measured in
-// round 1 keep their code: the TLAS walk and its mask exist only there).
-template <bool STATS, bool EXT, bool TLAS, bool CHUNKED>
+// round 1 keep their code: the TLAS walk and its mask exist only there).  FRAMES = the batch instantiations of rtDispatchFrames (never
+// CHUNKED): a lane keeps its pixel for frames Frame .. Frame + P.frames - 1, writing and accumulating each frame when its samples end.
+template <bool STATS, bool EXT, bool TLAS, bool CHUNKED, bool FRAMES = false>
 RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const unsigned int tilesX, const unsigned int ownedRows)
 {
     RT_DYNAMIC_SMEM(smemRaw);
@@ -310,6 +311,9 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
     const int chunks = CHUNKED && P.chunks > 1 && totalJobs > 0u ? P.chunks : 1;
     const unsigned int chunkJobs = totalJobs * (unsigned int)chunks;
     int chunk = 0, sampleEnd = P.NumRaysPerPixel; unsigned int pixJob = 0; bool waiting = false;
+    static_assert(!(FRAMES && CHUNKED), "a batch of frames runs whole pixels");
+    unsigned int frame = 0;          // FRAMES: frame of the batch the lane's pixel is in
+    (void)frame;
 
     for (;;)
     {
@@ -342,6 +346,7 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
                         sample = 0; sampleEnd = P.NumRaysPerPixel;
                         pixelOffset = (size_t)y * P.W + x;
                         havePixel = true; pathActive = false;
+                        if constexpr (FRAMES) frame = 0;
                         if (STATS) pixelStart = cnt;
                         if (CHUNKED && chunks > 1)
                         {
@@ -413,8 +418,26 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
                 h[0] = tag | rngState; h[1] = tag | __float_as_uint(totalIncomingLight.x);
                 h[2] = tag | __float_as_uint(totalIncomingLight.y); h[3] = tag | __float_as_uint(totalIncomingLight.z);
             }
-            if (STATS) AddPixelStats(P, pixelOffset, cnt, pixelStart);      // this lane's share: the whole pixel, or this chunk of it
-            havePixel = false;
+            if constexpr (FRAMES)
+            {
+                if (++frame < (unsigned int)P.frames)
+                {
+                    // the pixel's next frame: reseeded, a fresh sum, the same lane (frames accumulate in order)
+                    rngState = FrameSeed(px.rngState, frame);
+                    totalIncomingLight = splat3(0.0f);
+                    sample = 0;
+                }
+                else
+                {
+                    if (STATS) AddPixelStats(P, pixelOffset, cnt, pixelStart);      // all the pixel's frames
+                    havePixel = false;
+                }
+            }
+            else
+            {
+                if (STATS) AddPixelStats(P, pixelOffset, cnt, pixelStart);      // this lane's share: the whole pixel, or this chunk of it
+                havePixel = false;
+            }
         }
     }
 
@@ -440,6 +463,20 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wa
                                                                     const unsigned int tilesX, const unsigned int ownedRows)
 {
     wave_body<false, true, true, true>(P, totalJobs, tilesX, ownedRows);      // (the many-model kernel carries the chunk hand-off: it is never the Cornell-box kernel)
+}
+
+// rtDispatchFrames: P.frames frames of every pixel in one launch (kernels of their own, so that the kernels above keep their code)
+template <bool STATS, bool EXT>
+__global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wave_frames(const __grid_constant__ DevParams P, const unsigned int totalJobs,
+                                                                      const unsigned int tilesX, const unsigned int ownedRows)
+{
+    wave_body<STATS, EXT, false, false, true>(P, totalJobs, tilesX, ownedRows);
+}
+
+__global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wave_tlas_frames(const __grid_constant__ DevParams P, const unsigned int totalJobs,
+                                                                           const unsigned int tilesX, const unsigned int ownedRows)
+{
+    wave_body<false, true, true, false, true>(P, totalJobs, tilesX, ownedRows);
 }
 
 // "gridFit": a pixel's samples cannot be split (one RNG chain), so a persistent lane works through whole pixels.  When the image
@@ -488,14 +525,22 @@ inline cudaError_t wave_configure()
     if ((e = cudaFuncSetAttribute(k_raytrace_wave_tlas, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_wave<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_wave<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_tlas_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
     return wave_configure_one<true, true>();
 }
 
-template <bool S, bool X, bool T = false, bool C = false> inline cudaError_t wave_launch_one(const DevParams& P, int numSMs, size_t smemBytes, unsigned totalJobs, unsigned tilesX, unsigned ownedRows,
+// F = the batch kernels of rtDispatchFrames (k_raytrace_wave_frames, k_raytrace_wave_tlas_frames)
+template <bool S, bool X, bool T = false, bool C = false, bool F = false> inline cudaError_t wave_launch_one(const DevParams& P, int numSMs, size_t smemBytes, unsigned totalJobs, unsigned tilesX, unsigned ownedRows,
                                                              cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
 {
     int ctasPerSM = 0;
-    cudaError_t e = T ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_tlas, WAVE_THREADS, smemBytes)
+    cudaError_t e = F ? (T ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_tlas_frames, WAVE_THREADS, smemBytes)
+                           : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_frames<S, X>, WAVE_THREADS, smemBytes))
+                      : T ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_tlas, WAVE_THREADS, smemBytes)
                       : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave<S, X, C>, WAVE_THREADS, smemBytes);
     if (e != cudaSuccess) return e;
     if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
@@ -506,7 +551,9 @@ template <bool S, bool X, bool T = false, bool C = false> inline cudaError_t wav
     grid = fit_persistent_grid(P.gridFit, grid, WAVE_THREADS, totalJobs);
     if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
     if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
-    if (T) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, k_raytrace_wave_tlas, P, totalJobs, tilesX, ownedRows);
+    if (F && T) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, k_raytrace_wave_tlas_frames, P, totalJobs, tilesX, ownedRows);
+    else if (F) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_raytrace_wave_frames<S, X>), P, totalJobs, tilesX, ownedRows);
+    else if (T) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, k_raytrace_wave_tlas, P, totalJobs, tilesX, ownedRows);
     else RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_raytrace_wave<S, X, C>), P, totalJobs, tilesX, ownedRows);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     return cudaEventRecord(evB, stream);
@@ -526,6 +573,15 @@ inline cudaError_t wave_launch(const DevParams& P, int numSMs, cudaStream_t stre
 
     const size_t smemBytes = sizeof(WaveSmemHeader) + (size_t)P.smemPairs * sizeof(NodePair) + (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
     const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;   // extensions (peer stores, sphere accelerator, staged tree tops) compiled into their own instantiation
+    // a batch of frames (rtDispatchFrames, P.frames > 1, whole pixels): the FRAMES kernels, chosen like the single-frame ones
+    if (P.frames > 1)
+    {
+        if (P.countStats) return ext ? wave_launch_one<true, true, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
+                                     : wave_launch_one<true, false, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
+        if (P.tlas && P.modelSkip) return wave_launch_one<false, true, true, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
+        return ext ? wave_launch_one<false, true, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
+                   : wave_launch_one<false, false, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
+    }
     // sample chunks (P.chunks > 1, small tiles): the hand-off lives in instantiations of its own (the extension family and the TLAS kernel)
     if (P.chunks > 1 && !(P.tlas && P.modelSkip && !P.countStats))
         return P.countStats ? wave_launch_one<true, true, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)

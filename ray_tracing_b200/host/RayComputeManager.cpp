@@ -28,6 +28,7 @@ std::string RtApi::Load(const char* path)
     ReadbackWait = reinterpret_cast<decltype(ReadbackWait)>(dlsym(dl, "rtReadbackWait"));
     ReadbackPixelStats = reinterpret_cast<decltype(ReadbackPixelStats)>(dlsym(dl, "rtReadbackPixelStats"));
     DisplayPixelStats = reinterpret_cast<decltype(DisplayPixelStats)>(dlsym(dl, "rtDisplayPixelStats"));
+    DispatchFrames = reinterpret_cast<decltype(DispatchFrames)>(dlsym(dl, "rtDispatchFrames"));
     return "";
 }
 
@@ -90,6 +91,24 @@ int RayComputeManager::RenderFrame()
     if (rc != RT_OK) return rc;
     TRY(api.Dispatch(ctx, kernelRayTrace, (texWidth + 7) / 8, (texHeight + 7) / 8, 1));
     if (accumulate) numAccumulatedFrames++;
+    return RT_OK;
+}
+
+int RayComputeManager::RenderFrames(int n)
+{
+    if (!ctx) return RT_E_STATE;
+    if (n < 1) { lastError = "RenderFrames: n must be >= 1"; return RT_E_INVALID; }
+    if (!accumulate)                             // only the last frame would be observable: the frames one by one
+    {
+        for (int k = 0; k < n; k++) { const int rc = RenderFrame(); if (rc != RT_OK) return rc; }
+        return RT_OK;
+    }
+    if (!IsRendering()) return RT_OK;
+    if (!api.DispatchFrames) { lastError = "the library does not export rtDispatchFrames"; return RT_E_STATE; }
+    int rc = InitFrame();                        // Frame = numAccumulatedFrames, the batch's first frame
+    if (rc != RT_OK) return rc;
+    TRY(api.DispatchFrames(ctx, (texWidth + 7) / 8, (texHeight + 7) / 8, 1, n));
+    numAccumulatedFrames += n;
     return RT_OK;
 }
 

@@ -56,6 +56,7 @@ struct RtApi
     decltype(&rtReadbackAsync) ReadbackAsync = nullptr; decltype(&rtReadbackWait) ReadbackWait = nullptr;   // optional: pipelined readback
     decltype(&rtCreateMulti) CreateMulti = nullptr;   // optional: several GPUs behind one context (the all-gather of tiles inside rtDispatch)
     decltype(&rtReadbackPixelStats) ReadbackPixelStats = nullptr; decltype(&rtDisplayPixelStats) DisplayPixelStats = nullptr;   // optional: debug view
+    decltype(&rtDispatchFrames) DispatchFrames = nullptr;   // optional: several accumulated frames in one launch (RenderFrames)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -109,6 +110,9 @@ public:
     int ResetAccumulatedRender();                // :69-76
     int Update() { return RenderFrame(); }       // :78-82 (HandleInput is UI, out of scope)
     int RenderFrame();                           // :84-95
+    // not in the reference: n RenderFrame() calls of a still image in one batch (rtDispatchFrames) — InitFrame, one launch of frames
+    // numAccumulatedFrames .. + n - 1, numAccumulatedFrames += n.  With accumulate off, n RenderFrame() calls.
+    int RenderFrames(int n);
     int OnDestroy();                             // :238-247
     void InvalidateBVH() { hasBVH = false; }     // meshes changed: rebuild on the next frame
 

@@ -228,6 +228,7 @@ int rcmSetSpheres(void* hv, const RtSphere* spheres, int count)
 int rcmOnEnable(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->OnEnable(); } CATCH_ALL(h) }
 int rcmResetAccumulatedRender(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->ResetAccumulatedRender(); } CATCH_ALL(h) }
 int rcmRenderFrame(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFrame(); } CATCH_ALL(h) }
+int rcmRenderFrames(void* hv, int n) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFrames(n); } CATCH_ALL(h) }
 int rcmReadFrame(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadFrame(dst, bytes); }
 int rcmReadAccumulated(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadAccumulated(dst, bytes); }
 int rcmReadPixelStats(void* hv, RtPixelStats* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadPixelStats(dst, bytes); }

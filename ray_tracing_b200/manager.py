@@ -57,6 +57,7 @@ def host_lib() -> C.CDLL:
         L.rcmSetSpheres.argtypes = [vp, vp, ci]
         for n in ("rcmOnEnable", "rcmResetAccumulatedRender", "rcmRenderFrame"):
             getattr(L, n).argtypes = [vp]
+        L.rcmRenderFrames.argtypes = [vp, ci]
         L.rcmReadFrame.argtypes = [vp, vp, C.c_size_t]
         L.rcmReadAccumulated.argtypes = [vp, vp, C.c_size_t]
         L.rcmGetBVHStats.argtypes = [vp, vp, ci]
@@ -220,6 +221,11 @@ class RayComputeManager:
         self._ck(self._L.rcmRenderFrame(self._h))
 
     Update = RenderFrame
+
+    def RenderFrames(self, n: int):
+        """n RenderFrame() calls of a still image as one batch (rtDispatchFrames): the same images, numAccumulatedFrames += n.
+        With accumulate off it is n RenderFrame() calls."""
+        self._ck(self._L.rcmRenderFrames(self._h, int(n)))
 
     def OnDestroy(self):
         if self._h:

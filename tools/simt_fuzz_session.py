@@ -5,11 +5,14 @@ resizes, accumulation resets, settings and kernel options that change between fr
 manager against the oracle and against the kernels, compared bit for bit after every frame.  What it exercises is the host-side
 state of csrc/rt_api.cu: dirty flags, cached repacks, the regions the padded boxes were built for, kernel selection.
 
-    python tools/simt_fuzz_session.py [--cases 100] [--seed 1] [--steps 8] [--pixel-stats]
+    python tools/simt_fuzz_session.py [--cases 100] [--seed 1] [--steps 8] [--pixel-stats] [--frames]
 
 --pixel-stats: both sides count from the start ("countStats" = 1, and the script's countStats switches reach the oracle too), and after
 every frame the per-pixel counters (PixelStats rays, box and triangle tests) are compared as well: accumulation across frames, resizes,
 partial state changes.
+
+--frames: a step may render a batch of 2-6 frames as one call (RenderFrames: rtDispatchFrames) instead of one frame, on both sides.
+Where the kernels' side refuses the batch because "sampleChunks" is forced to 2 or more, it renders the frames one by one instead.
 """
 import argparse
 import os
@@ -36,8 +39,9 @@ def random_spheres(rng, n):
     return sph
 
 
-def make_script(rng, sc, steps):
-    """A list of (action, arguments) — applied to both managers; ('option', ...) only to the kernels' side."""
+def make_script(rng, sc, steps, frames=False):
+    """A list of (action, arguments) — applied to both managers; ('option', ...) only to the kernels' side.  frames: a step may end in
+    ('frames', (n,)), a batch of n frames, instead of ('frame', ())."""
     script = []
     nm = len(sc.models)
     for _ in range(steps):
@@ -69,7 +73,10 @@ def make_script(rng, sc, steps):
                 value = {"kernel": [0, 1, 2, -1], "tlas": [-1, 0, 1], "modelSkip": [0, 1], "poolSlots": [0, 32, 64, 96], "pairOrder": [0, 1, 3], "smemNodes": [0, 9, 200, -1],
                          "tailLanes": [0, 5, 16, 31], "sortRays": [0, 1], "gridFit": [0, 1], "extInstantiation": [0, 1], "countStats": [0, 1], "sampleChunks": [-1, 0, 2, 3]}[name]
                 script.append(("option", (name, int(rng.choice(value)))))
-        script.append(("frame", ()))
+        if frames and rng.rand() < 0.5:
+            script.append(("frames", (int(rng.randint(2, 7)),)))
+        else:
+            script.append(("frame", ()))
     return script
 
 
@@ -110,6 +117,7 @@ def main():
     ap.add_argument("--steps", type=int, default=8)
     ap.add_argument("--lib", default=None)
     ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters after every frame")
+    ap.add_argument("--frames", action="store_true", help="steps may render a batch of 2-6 frames in one call (RenderFrames)")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
     bad = 0
@@ -117,7 +125,7 @@ def main():
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
         sc = random_scene(rng, odd=0.0)
-        script = make_script(rng, sc, args.steps)
+        script = make_script(rng, sc, args.steps, args.frames)
         mgrs = []
         for backend in (ORACLE_LIB, lib):
             m = rt.RayComputeManager(backend)
@@ -126,19 +134,30 @@ def main():
                 m.context.set_option("countStats", 1)
             m.OnEnable()
             mgrs.append(m)
-        frame_no, failed, resized = 0, None, False
+        frame_no, failed, resized, chunks = 0, None, False, -1
         try:
             for action, a in script:
                 if action == "screen":
                     resized = True                      # the textures follow at the next RenderFrame (InitFrame): no raw dispatch in between
                 if action == "rawframe" and resized:
                     continue
-                if action == "frame":
+                if action in ("frame", "frames"):
                     resized = False
-                if action in ("frame", "rawframe"):
-                    for m in mgrs:
+                if action == "option" and a[0] == "sampleChunks":
+                    chunks = a[1]
+                if action in ("frame", "frames", "rawframe"):
+                    for i, m in enumerate(mgrs):
                         if action == "frame":
                             m.RenderFrame()
+                        elif action == "frames":
+                            try:
+                                m.RenderFrames(a[0])
+                            except rt.capi.RtError as e:
+                                # a batch runs whole pixels: refused on the kernels' side while sampleChunks is forced to 2 or more
+                                if not (i == 1 and chunks >= 2 and e.code == rt.capi.RT_E_STATE):
+                                    raise
+                                for _ in range(a[0]):
+                                    m.RenderFrame()
                         else:
                             m.context.set_int("modelCount", a[0]); m.context.set_int("Frame", a[1]); m.context.dispatch_full(0)
                     frame_no += 1
