@@ -52,6 +52,14 @@ public static class RtB200
     public struct PixelStats { public uint rays, boxTests, triTests, sphereTests, sphereBoxTests; }
     [DllImport(Lib)] public static extern int rtReadbackPixelStats(IntPtr ctx, [Out] PixelStats[] dst, UIntPtr bytes);
     [DllImport(Lib)] public static extern int rtDisplayPixelStats(IntPtr ctx, int visMode, float debugVisScale, byte[] rgba, UIntPtr bytes);
+    // closest-hit queries (CalculateRayCollision, RayCommon.hlsl:335-374): click to pick a Model, autofocus (focusDistance = hit.dst of the
+    // centre pixel's ray), line of sight.  kind: 0 nothing hit, 1 Spheres[index], 2 ModelInfo[index]; flags 1 = forceDontCullBack
+    [StructLayout(LayoutKind.Sequential)]
+    public struct Ray { public UnityEngine.Vector3 origin, dir; }
+    [StructLayout(LayoutKind.Sequential)]
+    public struct RayHit { public float dst; public UnityEngine.Vector3 pos, normal; public int isBackface, kind, index, pad0, pad1; }
+    [DllImport(Lib)] public static extern int rtTraceRays(IntPtr ctx, Ray[] rays, int n, [Out] RayHit[] hits, int flags);
+    [DllImport(Lib)] public static extern int rtTraceRaysDevice(IntPtr ctx, IntPtr dRays, IntPtr dHits, int n, int flags);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

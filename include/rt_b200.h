@@ -102,6 +102,35 @@ int rtDispatch(RtContext* ctx, int kernelIndex, int groupsX, int groupsY, int gr
 #define RT_MAX_BATCH_SAMPLES ((1 << 20) - 1)
 int rtDispatchFrames(RtContext* ctx, int groupsX, int groupsY, int groupsZ, int frameCount);
 
+/* Extension: closest-hit queries for caller-supplied rays (picking, autofocus, line of sight, visibility / occlusion baking).
+ * hits[i] = CalculateRayCollision(rays[i], forceDontCullBack = flags & RT_TRACE_NO_CULL) (HL:335-374, HL:356), with the sphere
+ * extension tested first as in rtDispatch: the same bits as the camera rays' intersection.  Ties keep the reference's order: spheres
+ * before models, the lower buffer index first, strict <.  RtRayHit (rt_types.h): dst = +inf, pos = normal = 0, isBackface = 0,
+ * kind = RT_HIT_NONE and index = -1 on a miss; kind / index name the winning Spheres or ModelInfo entry otherwise.
+ *   - Reads the current Spheres, ModelInfo, Nodes, Triangles and "modelCount" and no other uniform; needs no rtResize and no
+ *     earlier dispatch.  Leaves FrameRender, AccumulatedRender, "Frame", PixelStats, RtStats.dispatches and kernelMs alone and
+ *     does not change what later dispatches render.
+ *   - RtStats.rays grows by n.  With "countStats" = 1 the box / triangle / sphere / sphere-accelerator counters grow as a counting
+ *     dispatch's do (every model is walked, like the reference).
+ *   - Model skipping, the TLAS and the sphere accelerator are used only for rays whose origin lies inside the box their records were
+ *     padded for (the camera and all geometry, with room) and whose direction has 2^-20 <= dot(dir, dir) <= 2^20 (the range in which
+ *     the padding's error argument holds); any other ray (origin far away or NaN, direction very short, very long, zero or NaN) walks
+ *     every model and tests every sphere in buffer order.  Rays that may skip share the open grazing-ray defect of model skipping
+ *     (DESIGN.md section 5) with the camera rays; "modelSkip" = 0 avoids it.
+ *   - On a group context (rtCreateMulti) the rays are traced on devices[0], which holds the whole scene; call it on the context
+ *     rtCreateMulti returned.
+ * Refused: ctx NULL, n < 0, rays / hits NULL with n > 0, flags outside {0, RT_TRACE_NO_CULL}, a device dRays not 4-byte or dHits not
+ * 16-byte aligned -> RT_E_INVALID; a member context of a group other than the one rtCreateMulti returned (as rtDispatch) and the scene
+ * checks of rtDispatch (modelCount beyond ModelInfo, models without Nodes / Triangles, an offset out of range, a tree deeper than 63
+ * inner levels) -> RT_E_STATE.  n = 0 is RT_OK and launches nothing.
+ * rtTraceRays: host arrays, traced in batches of at most RT_TRACE_CHUNK_RAYS through two device buffers the context keeps for later
+ * calls (72 bytes per ray of the largest batch so far, at most 72 MiB; freed by rtDestroy); synchronises.  rtTraceRaysDevice: n RtRay /
+ * RtRayHit in device memory of the context's device, no allocation; asynchronous on the context's stream (rtSetStream). */
+#define RT_TRACE_NO_CULL 1
+#define RT_TRACE_CHUNK_RAYS (1 << 20)
+int rtTraceRays(RtContext* ctx, const RtRay* rays, int n, RtRayHit* hits, int flags);
+int rtTraceRaysDevice(RtContext* ctx, const void* dRays, void* dHits, int n, int flags);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),

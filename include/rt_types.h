@@ -73,11 +73,33 @@ typedef struct RtPixelStats {
     uint32_t rays, boxTests, triTests, sphereTests, sphereBoxTests;
 } RtPixelStats;
 
+/* A caller-supplied ray of rtTraceRays / rtTraceRaysDevice (include/rt_b200.h): world-space origin and direction.  The direction
+ * need not be unit length; dst is measured in multiples of it. */
+typedef struct RtRay {
+    float origin[3];
+    float dir[3];
+} RtRay;
+
+enum { RT_HIT_NONE = 0, RT_HIT_SPHERE = 1, RT_HIT_MODEL = 2 };
+
+/* The closest hit of one RtRay: CalculateRayCollision's HitInfo (RayCommon.hlsl:335-374) plus which object won. */
+typedef struct RtRayHit {
+    float   dst;          /* ray parameter of the closest hit (HL:366); +inf = nothing hit */
+    float   pos[3];       /* origin + dir * dst (HL:368); 0 on a miss */
+    float   normal[3];    /* world-space normal as HL:367 (models) / HL:320 (spheres) compute it; 0 on a miss */
+    int32_t isBackface;   /* 0 / 1 */
+    int32_t kind;         /* RT_HIT_NONE, RT_HIT_SPHERE or RT_HIT_MODEL */
+    int32_t index;        /* index of the winner in Spheres / ModelInfo; -1 on a miss */
+    int32_t pad[2];       /* 0 */
+} RtRayHit;
+
 #pragma pack(pop)
 
 #ifdef __cplusplus
 }
 static_assert(sizeof(RtPixelStats) == 20, "PixelStats record");
+static_assert(sizeof(RtRay) == 24, "RtRay record");
+static_assert(sizeof(RtRayHit) == 48, "RtRayHit record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

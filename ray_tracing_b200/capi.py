@@ -42,6 +42,31 @@ assert PIXEL_STATS_DTYPE.itemsize == 20
 # rtDisplayPixelStats visMode: what the heat map shows per pixel
 VIS_MODES = {1: "boxTests per ray", 2: "triTests per ray", 3: "sphere tests per ray", 4: "rays"}
 
+# rtTraceRays: a caller-supplied ray and its closest hit (RtRay / RtRayHit)
+RAY_DTYPE = np.dtype([("origin", "<f4", 3), ("dir", "<f4", 3)])
+RAY_HIT_DTYPE = np.dtype([("dst", "<f4"), ("pos", "<f4", 3), ("normal", "<f4", 3), ("isBackface", "<i4"), ("kind", "<i4"),
+                          ("index", "<i4"), ("pad", "<i4", 2)])
+assert RAY_DTYPE.itemsize == 24 and RAY_HIT_DTYPE.itemsize == 48
+RT_HIT_NONE, RT_HIT_SPHERE, RT_HIT_MODEL = 0, 1, 2
+RT_TRACE_CHUNK_RAYS = 1 << 20      # rtTraceRays: host arrays travel in batches of at most this many rays
+RT_TRACE_NO_CULL = 1      # forceDontCullBack (RayCommon.hlsl:356): back faces count for every model, not only glass
+
+
+def make_rays(origins, dirs=None) -> np.ndarray:
+    """A RAY_DTYPE array from a structured array (returned as it is) or from (n, 3) origins and (n, 3) directions."""
+    if dirs is None:
+        rays = np.asarray(origins)
+        if rays.dtype != RAY_DTYPE:
+            raise TypeError(f"rays must have dtype {RAY_DTYPE} (or pass origins and dirs)")
+        return np.ascontiguousarray(rays).reshape(-1)
+    o = np.asarray(origins, dtype=np.float32).reshape(-1, 3)
+    d = np.asarray(dirs, dtype=np.float32).reshape(-1, 3)
+    if o.shape != d.shape:
+        raise ValueError("origins and dirs must both be (n, 3)")
+    rays = np.empty(o.shape[0], dtype=RAY_DTYPE)
+    rays["origin"], rays["dir"] = o, d
+    return rays
+
 
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
@@ -104,11 +129,13 @@ class RtLib:
             "rtReadbackPixelStats": ([vp, vp, C.c_size_t], ci),
             "rtDisplayPixelStats": ([vp, ci, cf, vp, C.c_size_t], ci),
             "rtDispatchFrames": ([vp, ci, ci, ci, ci], ci),
+            "rtTraceRays": ([vp, vp, ci, vp, ci], ci),
+            "rtTraceRaysDevice": ([vp, vp, vp, ci, ci], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
-                            "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames"):      # absent from older experimental builds used in A/B runs
+                            "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -219,6 +246,21 @@ class RtContext:
         gx = (self.width + 7) // 8 if gx is None else gx
         gy = (self.height + 7) // 8 if gy is None else gy
         self._ck(self._L.rtDispatchFrames(self._h, int(gx), int(gy), int(gz), int(n)))
+
+    def trace_rays(self, rays, dirs=None, no_cull: bool = False) -> np.ndarray:
+        """rtTraceRays: the closest hit of every ray against the current scene, as the path tracer computes it.  rays: a RAY_DTYPE
+        array, or (n, 3) origins with (n, 3) directions in `dirs`.  Returns n RAY_HIT_DTYPE records (dst = inf, kind = RT_HIT_NONE,
+        index = -1 on a miss).  no_cull: back faces count for every model (forceDontCullBack)."""
+        r = make_rays(rays, dirs)
+        hits = np.empty(r.shape[0], dtype=RAY_HIT_DTYPE)
+        self._ck(self._L.rtTraceRays(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), hits.ctypes.data if hits.size else None,
+                                     RT_TRACE_NO_CULL if no_cull else 0))
+        return hits
+
+    def trace_rays_device(self, rays_ptr: int, hits_ptr: int, n: int, no_cull: bool = False):
+        """rtTraceRaysDevice: n RtRay at rays_ptr -> n RtRayHit at hits_ptr (16-byte aligned), both device memory of the context's GPU
+        (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
+        self._ck(self._L.rtTraceRaysDevice(self._h, C.c_void_p(rays_ptr), C.c_void_p(hits_ptr), int(n), RT_TRACE_NO_CULL if no_cull else 0))
 
     def readback(self, tex: str, out: Optional[np.ndarray] = None) -> np.ndarray:
         if out is None:

@@ -9,6 +9,7 @@
 #include "rt_kernel_mega.cuh"
 #include "rt_kernel_wave.cuh"
 #include "rt_kernel_pool.cuh"
+#include "rt_kernel_query.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -99,6 +100,7 @@ struct RtContext
     unsigned long long* dCounters = nullptr;   // 5
     unsigned int* dWork = nullptr;
     DevBuf<RtPixelStats> pixelStats;           // "PixelStats": W*H per-pixel counters of the counting launches (allocated by the first one)
+    DevBuf<RtRay> queryRays; DevBuf<RtRayHit> queryHits;     // rtTraceRays: device copies of one batch (<= RT_TRACE_CHUNK_RAYS) of the caller's host arrays
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -207,7 +209,7 @@ int rtDestroy(RtContext* c)
     c->buildArena.release(); c->handoff.release(); c->poolCold.release();
     for (int k = 0; k < 2; k++) { if (c->stageBuf[k]) cudaFreeHost(c->stageBuf[k]); if (c->stageEv[k]) cudaEventDestroy(c->stageEv[k]); }
     c->frame.release(); c->accum.release(); c->tileSend.release(); c->tileRecv.release(); c->display.release();
-    c->pixelStats.release();
+    c->pixelStats.release(); c->queryRays.release(); c->queryHits.release();
     c->repack.release();
     closePeers(c);
     for (auto& ev : c->pending) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
@@ -557,35 +559,76 @@ static void applyL2Persistence(RtContext* c)
 #endif
 }
 
-static int prepareScene(RtContext* c)
+// Scene preparation, shared by rtDispatch (prepareScene) and rtTraceRays (prepareQueryScene); `what` names the call in messages.
+// checkScene: the buffers and offsets a trace reads are there.
+static int checkScene(RtContext* c, const std::string& what)
 {
-    if (c->P.modelCount < 0 || (size_t)c->P.modelCount > c->models.count) return fail(c, RT_E_STATE, "rtDispatch: modelCount exceeds the ModelInfo buffer");
-    if (c->P.modelCount > 0 && (c->nodes.count == 0 || c->tris.count == 0)) return fail(c, RT_E_STATE, "rtDispatch: models without Nodes / Triangles buffers");
+    if (c->P.modelCount < 0 || (size_t)c->P.modelCount > c->models.count) return fail(c, RT_E_STATE, what + ": modelCount exceeds the ModelInfo buffer");
+    if (c->P.modelCount > 0 && (c->nodes.count == 0 || c->tris.count == 0)) return fail(c, RT_E_STATE, what + ": models without Nodes / Triangles buffers");
     for (int i = 0; i < c->P.modelCount; i++)
     {
         const RtModel& m = c->hModels[i];
         if (m.nodeOffset < 0 || (size_t)m.nodeOffset >= c->nodes.count || m.triOffset < 0 || (size_t)m.triOffset > c->tris.count)
-            return fail(c, RT_E_STATE, "rtDispatch: model nodeOffset / triOffset out of range");
+            return fail(c, RT_E_STATE, what + ": model nodeOffset / triOffset out of range");
     }
+    return RT_OK;
+}
+
+// The layout of the pair records a RayTrace dispatch asks for now: the tree-top budget, the record order and the treelet flag
+static void sceneLayout(const RtContext* c, int& budget, int& pairOrder, bool& treelets)
+{
     // shared-memory budget for the tree tops: what the selected kernel can afford next to its own shared state
     // automatic = 0: staging tree tops never beat leaving that shared memory to L1
-    int budget = c->optSmemPairs < 0 ? 0 : c->optSmemPairs;
+    budget = c->optSmemPairs < 0 ? 0 : c->optSmemPairs;
     const int kernelSel = effectiveKernel(c);
-    const bool treelets = c->optTreeletPrefetch && kernelSel != 0;      // two-level treelets with flagged roots; no shared-memory staging with it
-    const int pairOrder = treelets ? 2 : c->optPairOrder;
+    treelets = c->optTreeletPrefetch && kernelSel != 0;                 // two-level treelets with flagged roots; no shared-memory staging with it
+    pairOrder = treelets ? 2 : c->optPairOrder;
     if (treelets) budget = 0;
     if (budget > 3072) budget = 3072;                                   // planScene's own clamp (192 KB), so that budgetUsed compares equal
     if (kernelSel == 2) { const int mx = pool_max_smem_pairs(c->optPoolSlots ? c->optPoolSlots : 96, (int)c->spheres.count); if (budget > mx) budget = mx; }
     else if (kernelSel == 0) budget = 0;
+}
+
+// The pair records, mesh roots and triangle streams, when the scene's topology changed
+static int planSceneIfDirty(RtContext* c, const std::string& what, int budget, int pairOrder, bool treelets)
+{
+    if (!c->sceneDirty) return RT_OK;
+    std::string msg;
+    cudaError_t e = c->repack.buildScene(c->hNodes, c->hModels, c->P.modelCount, c->tris.p, c->tris.count, budget, c->stream, msg, pairOrder, treelets);
+    if (e != cudaSuccess) return failCuda(c, e, "repack scene");
+    if (!msg.empty()) return fail(c, RT_E_STATE, what + ": " + msg);
+    c->sceneDirty = false; c->modelsDirty = true;
+    return RT_OK;
+}
+
+static int fitOriginPadding(RtContext* c);
+
+static int prepareScene(RtContext* c)
+{
+    int rc = checkScene(c, "rtDispatch"); if (rc != RT_OK) return rc;
+    int budget, pairOrder; bool treelets;
+    sceneLayout(c, budget, pairOrder, treelets);
     if (budget != c->repack.budgetUsed || pairOrder != c->repack.orderUsed || treelets != c->repack.flagsUsed) c->sceneDirty = true;
-    if (c->sceneDirty)
-    {
-        std::string msg;
-        cudaError_t e = c->repack.buildScene(c->hNodes, c->hModels, c->P.modelCount, c->tris.p, c->tris.count, budget, c->stream, msg, pairOrder, treelets);
-        if (e != cudaSuccess) return failCuda(c, e, "repack scene");
-        if (!msg.empty()) return fail(c, RT_E_STATE, "rtDispatch: " + msg);
-        c->sceneDirty = false; c->modelsDirty = true;
-    }
+    if ((rc = planSceneIfDirty(c, "rtDispatch", budget, pairOrder, treelets)) != RT_OK) return rc;
+    return fitOriginPadding(c);
+}
+
+// rtTraceRays: what does not depend on the image or the kernel choice.  A layout that is already built is kept whatever its budget
+// (a query reads every record from global memory); a scene that must be planned anyway gets the layout the next dispatch would ask
+// for, so that with default options the query never makes that dispatch plan again.
+static int prepareQueryScene(RtContext* c)
+{
+    int rc = checkScene(c, "rtTraceRays"); if (rc != RT_OK) return rc;
+    int budget, pairOrder; bool treelets;
+    sceneLayout(c, budget, pairOrder, treelets);
+    if ((rc = planSceneIfDirty(c, "rtTraceRays", budget, pairOrder, treelets)) != RT_OK) return rc;
+    return fitOriginPadding(c);
+}
+
+// The model records (with the TLAS) and the sphere accelerator, rebuilt when they changed or when the box of possible camera-ray
+// origins outgrew the one their padding was computed for
+static int fitOriginPadding(RtContext* c)
+{
     {
         // box containing every possible ray origin: the camera (with its defocus disc) and all geometry; it sizes the padding of
         // the models' world boxes and of the sphere accelerator, which are rebuilt when the box outgrows the one they were built for
@@ -619,6 +662,21 @@ static int prepareScene(RtContext* c)
         }
     }
     return RT_OK;
+}
+
+// The scene's buffers, the counters and the scene options in a parameter block (what both the camera kernels and the queries read)
+static void bindScene(const RtContext* c, DevParams& P)
+{
+    P.sphereCount = (int)c->spheres.count;
+    P.Nodes = c->nodes.p; P.Triangles = c->tris.p; P.ModelInfo = c->models.p; P.Spheres = c->spheres.p;
+    P.pairs = c->repack.pairs.p; P.triGeom = c->repack.triGeom.p; P.triNormals = c->repack.triNormals.p;
+    P.models = c->repack.models.p; P.spheres = c->repack.spheres.p;
+    P.sphPairs = c->repack.sphPairs.p; P.sphLeaves = c->repack.sphLeaves.p; P.sphBvh = c->repack.sphBvh;
+    P.sphRootStart = c->repack.sphRootStart; P.sphRootCount = c->repack.sphRootCount;
+    P.counters = c->dCounters; P.workCounter = c->dWork;
+    P.forceExt = c->optForceExt; P.modelSkip = c->optModelSkip;
+    P.tlasPairs = c->repack.tlasPairs.p; P.tlasLeaves = c->repack.tlasLeaves.p; P.tlas = c->repack.tlas;
+    P.tlasRootStart = c->repack.tlasRootStart; P.tlasRootCount = c->repack.tlasRootCount;
 }
 
 // One GPU's share of a dispatch: the RayTrace kernel over this context's tile (the whole image without rtSetTile).
@@ -666,18 +724,11 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     DevParams P = c->P;
     P.limX = limX; P.limY = limY;
     P.tileRank = c->tileRank; P.tileWorld = c->tileWorld; P.bandRows = c->bandRows; P.countStats = c->optCountStats;
-    P.sphereCount = (int)c->spheres.count;
-    P.Nodes = c->nodes.p; P.Triangles = c->tris.p; P.ModelInfo = c->models.p; P.Spheres = c->spheres.p;
-    P.pairs = c->repack.pairs.p; P.triGeom = c->repack.triGeom.p; P.triNormals = c->repack.triNormals.p;
-    P.models = c->repack.models.p; P.spheres = c->repack.spheres.p;
-    P.sphPairs = c->repack.sphPairs.p; P.sphLeaves = c->repack.sphLeaves.p; P.sphBvh = c->repack.sphBvh;
-    P.sphRootStart = c->repack.sphRootStart; P.sphRootCount = c->repack.sphRootCount; P.smemPairs = c->repack.smemPairs; P.tailLanes = c->optTailLanes; P.sortRays = c->optSortRays; P.gridFit = c->optGridFit;
+    bindScene(c, P);
+    P.smemPairs = c->repack.smemPairs; P.tailLanes = c->optTailLanes; P.sortRays = c->optSortRays; P.gridFit = c->optGridFit;
     P.FrameRender = c->frame.p; P.AccumulatedRender = c->accum.p;
-    P.counters = c->dCounters; P.workCounter = c->dWork;
     P.pixelStats = c->optCountStats ? c->pixelStats.p : nullptr;
-    P.nPeers = c->nPeers; P.forceExt = c->optForceExt; P.modelSkip = c->optModelSkip;
-    P.tlasPairs = c->repack.tlasPairs.p; P.tlasLeaves = c->repack.tlasLeaves.p; P.tlas = c->repack.tlas;
-    P.tlasRootStart = c->repack.tlasRootStart; P.tlasRootCount = c->repack.tlasRootCount;
+    P.nPeers = c->nPeers;
     P.frames = frames;
     {
         // camOrigin = M * (0,0,0,1) as SetupPixel computes it (left to right, unfused): exact zero components and non-finite axes rule the shortcut out
@@ -986,6 +1037,70 @@ int rtDispatchFrames(RtContext* c, int gx, int gy, int gz, int frameCount)
     std::vector<RtContext*> all(1, c);                      // one exchange for the whole batch: it carries the last frame and the sum
     all.insert(all.end(), c->followers.begin(), c->followers.end());
     return exchangeTiles(all.data(), (int)all.size());
+}
+
+// ---- closest-hit queries (rtTraceRays, rt_kernel_query.cuh) -----------------------------------------------------------------------
+static int stagedH2D(RtContext* c, void* dst, const void* src, size_t bytes);
+static int stagedD2H(RtContext* c, void* dst, const void* src, size_t bytes);
+
+static int traceArgs(RtContext* c, const char* what, const void* rays, const void* hits, int n, int flags)
+{
+    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; trace on the context rtCreateMulti returned");
+    if (n < 0 || (n > 0 && (!rays || !hits))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or rays / hits NULL)");
+    if (flags != 0 && flags != RT_TRACE_NO_CULL) return fail(c, RT_E_INVALID, std::string(what) + ": flags must be 0 or RT_TRACE_NO_CULL");
+    return RT_OK;
+}
+
+// n rays in device memory of this context's GPU -> n hits; asynchronous on the context's stream.  RtStats.rays grows by n through the
+// kernel's counters; no timing events, so dispatches / kernelMs stay the camera kernels'.
+static int traceLocal(RtContext* c, const RtRay* dRays, RtRayHit* dHits, int n, int flags)
+{
+    int rc = prepareQueryScene(c); if (rc != RT_OK) return rc;
+    DevParams P = c->P;
+    bindScene(c, P);
+    P.countStats = c->optCountStats;
+    P.smemPairs = 0;                                 // no tree-top staging: every record from global memory
+    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    QueryParams Q;
+    Q.rays = dRays; Q.hits = dHits; Q.n = (unsigned int)n; Q.noCull = flags & RT_TRACE_NO_CULL;
+    for (int a = 0; a < 3; a++)
+    {
+        Q.modelLo[a] = c->repack.modelBoundLo[a]; Q.modelHi[a] = c->repack.modelBoundHi[a];
+        Q.sphLo[a] = c->repack.sphBoundLo[a]; Q.sphHi[a] = c->repack.sphBoundHi[a];
+    }
+    cudaError_t e = query_launch(P, Q, c->numSMs, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "rtTraceRays launch");
+    return RT_OK;
+}
+
+int rtTraceRays(RtContext* c, const RtRay* rays, int n, RtRayHit* hits, int flags)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = traceArgs(c, "rtTraceRays", rays, hits, n, flags); if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    // batches of at most RT_TRACE_CHUNK_RAYS through device buffers of that size, kept by the context (72 MB at most)
+    const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
+    if (c->queryRays.cap < (size_t)chunk) { CK(c->queryRays.ensure((size_t)chunk)); CK(c->queryHits.ensure((size_t)chunk)); }
+    for (int i0 = 0; i0 < n; i0 += chunk)
+    {
+        const int m = n - i0 < chunk ? n - i0 : chunk;
+        if ((rc = stagedH2D(c, c->queryRays.p, rays + i0, (size_t)m * sizeof(RtRay))) != RT_OK) return rc;
+        if ((rc = traceLocal(c, c->queryRays.p, c->queryHits.p, m, flags)) != RT_OK) return rc;
+        if ((rc = stagedD2H(c, hits + i0, c->queryHits.p, (size_t)m * sizeof(RtRayHit))) != RT_OK) return rc;
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rtTraceRaysDevice(RtContext* c, const void* dRays, void* dHits, int n, int flags)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = traceArgs(c, "rtTraceRaysDevice", dRays, dHits, n, flags); if (rc != RT_OK) return rc;
+    if (((uintptr_t)dRays & 3u) || ((uintptr_t)dHits & 15u)) return fail(c, RT_E_INVALID, "rtTraceRaysDevice: dRays must be 4-byte and dHits 16-byte aligned");
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    return traceLocal(c, (const RtRay*)dRays, (RtRayHit*)dHits, n, flags);
 }
 
 int rtExchangeTiles(RtContext* c)

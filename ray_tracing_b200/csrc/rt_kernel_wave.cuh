@@ -144,21 +144,32 @@ RT_DI void TraverseMesh(const DevParams& P, const float4* __restrict__ smemPairs
     }
 }
 
-// HL:335-374 (+ sphere extension) on the repacked streams
-template <bool STATS, bool EXT, bool TLAS>
+// A caller-supplied ray (rtTraceRays, rt_kernel_query.cuh).  In: whether its origin lies inside the box of origins the model records
+// (modelsExact) and the sphere accelerator (spheresExact) were padded for — only then may the ray skip models, walk the TLAS or use
+// the accelerator — and whether back faces count for every model (forceDontCullBack, HL:356).  Out: the winner's kind (RT_HIT_*) and
+// its index in Spheres / ModelInfo.
+struct QueryRay { bool modelsExact, spheresExact, noCull; int kind, index; };
+
+// HL:335-374 (+ sphere extension) on the repacked streams.  QUERY = rtTraceRays (q != nullptr); the camera kernels leave it false.
+template <bool STATS, bool EXT, bool TLAS, bool QUERY = false>
 RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, const DevSphere* __restrict__ smemSpheres,
-                    f3 rayPos, f3 rayDir, Counters& cnt)
+                    f3 rayPos, f3 rayDir, Counters& cnt, QueryRay* q = nullptr)
 {
     Hit result;
     result.dst = inf32(); result.isBackface = false; result.normal = splat3(0.0f); result.pos = splat3(0.0f); result.material = nullptr;
     cnt.rays++;
+    if constexpr (QUERY) { q->kind = RT_HIT_NONE; q->index = -1; }
 
     int bestSphere = -1; bool bestInside = false;
-    if (EXT && P.sphBvh)
+    if (EXT && P.sphBvh && (!QUERY || q->spheresExact))
     {
         int idx = 0x7fffffff, flag = 0;
         TraverseSpheres(P, rayPos, rayDir, result.dst, idx, bestInside, flag, cnt, STATS);
-        if (idx != 0x7fffffff) bestSphere = idx;
+        // (queries: the accelerator's tie rule also keeps a "hit" at dst = +inf, which the reference's strict < never takes; such a hit
+        // needs a direction so short or long that dot(dir, dir) leaves the float range — camera rays are unit length)
+        bool keep = idx != 0x7fffffff;
+        if constexpr (QUERY) keep = keep && result.dst < inf32();
+        if (keep) bestSphere = idx;
     }
     else
     for (int i = 0; i < P.sphereCount; i++)
@@ -183,13 +194,17 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
         result.pos = rayPos + rayDir * result.dst;
         result.normal = normalize3(result.pos - centre) * (bestInside ? -1.0f : 1.0f);
         result.material = &P.Spheres[bestSphere].material;
+        if constexpr (QUERY) { q->kind = RT_HIT_SPHERE; q->index = bestSphere; }
     }
 
     const f3 rayInv = rcp3(rayDir);
+    // model skipping (the TLAS and the per-model box test) is exact only for origins inside the box the model records were padded for
+    bool skipExact = true;
+    if constexpr (QUERY) skipExact = q->modelsExact;
     // many-model scenes (<TLAS> kernels only): one walk of the TLAS marks the models this ray can reach at all; the loop below
     // then jumps from marked model to marked model, still in buffer order and still re-testing each against the running result
     unsigned int tlasMask[TLAS ? RT_TLAS_WORDS : 1];
-    const bool useTlas = TLAS && !STATS && P.modelSkip && P.tlas;
+    const bool useTlas = TLAS && !STATS && P.modelSkip && P.tlas && skipExact;
     if (useTlas) TlasCollect(P, rayPos, rayInv, result.dst, tlasMask);
     for (int i = 0; i < P.modelCount; i++)
     {
@@ -198,7 +213,7 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
         const float4* mr = reinterpret_cast<const float4*>(m);
         // the instrumented build walks every model like the reference (identical test counts); otherwise models the ray cannot
         // reach before its current best hit are skipped — they could not have changed the result
-        if (!STATS && P.modelSkip && ModelOutOfReach(mr, rayPos, rayInv, result.dst)) continue;
+        if (!STATS && P.modelSkip && skipExact && ModelOutOfReach(mr, rayPos, rayInv, result.dst)) continue;
         float w2l[12];
         {
             const float4 r0 = __ldg(mr), r1 = __ldg(mr + 1), r2 = __ldg(mr + 2);
@@ -211,8 +226,10 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
         const f3 localDir = mul_rm(w2l, rayDir, 0.0f);
         const f3 invDir = rcp3(localDir);
         NodeRef root; root.start = meta.x; root.count = meta.y;
+        bool cullBackface = meta.z != 0;
+        if constexpr (QUERY) cullBackface = cullBackface && !q->noCull;
         float dst, u, v, det; int tri;
-        TraverseMesh<STATS, EXT>(P, smemPairs, localPos, localDir, invDir, result.dst, root, meta.z != 0, dst, tri, u, v, det, cnt);
+        TraverseMesh<STATS, EXT>(P, smemPairs, localPos, localDir, invDir, result.dst, root, cullBackface, dst, tri, u, v, det, cnt);
         if (dst < result.dst)
         {
             const float4* nq = reinterpret_cast<const float4*>(P.triNormals + tri);
@@ -230,6 +247,7 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
             result.normal = normalize3(mul_rm(l2w, n, 0.0f));
             result.pos = rayPos + rayDir * dst;
             result.material = &P.ModelInfo[meta.w].material;
+            if constexpr (QUERY) { q->kind = RT_HIT_MODEL; q->index = meta.w; }
         }
     }
     return result;

@@ -29,6 +29,7 @@ std::string RtApi::Load(const char* path)
     ReadbackPixelStats = reinterpret_cast<decltype(ReadbackPixelStats)>(dlsym(dl, "rtReadbackPixelStats"));
     DisplayPixelStats = reinterpret_cast<decltype(DisplayPixelStats)>(dlsym(dl, "rtDisplayPixelStats"));
     DispatchFrames = reinterpret_cast<decltype(DispatchFrames)>(dlsym(dl, "rtDispatchFrames"));
+    TraceRays = reinterpret_cast<decltype(TraceRays)>(dlsym(dl, "rtTraceRays"));
     return "";
 }
 
@@ -289,6 +290,43 @@ int RayComputeManager::DisplayDebugView(int visMode, float debugVisScale, uint8_
     if (!api.DisplayPixelStats) { lastError = "the library does not export rtDisplayPixelStats"; return RT_E_STATE; }
     TRY(api.DisplayPixelStats(ctx, visMode, debugVisScale, dst, bytes));
     return RT_OK;
+}
+
+int RayComputeManager::TraceRays(const RtRay* rays, int n, RtRayHit* hits, int flags)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.TraceRays) { lastError = "the library does not export rtTraceRays"; return RT_E_STATE; }
+    int rc;
+    if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
+    TRY(api.TraceRays(ctx, rays, n, hits, flags));
+    return RT_OK;
+}
+
+void RayComputeManager::PickRay(float x, float y, RtRay* ray) const
+{
+    // ViewParams as UpdateCameraParams computes them; uv, origin and focus point as SetupPixel does (HL:547-558), left to right, unfused
+    const float Deg2Rad = 0.0174532924f;
+    const float planeHeight = focusDistance * (float)std::tan((double)(mainCamera.fieldOfView * 0.5f * Deg2Rad)) * 2;
+    const float planeWidth = planeHeight * mainCamera.aspect;
+    const float* M = mainCamera.transform.localToWorldMatrix.m;            // column-major
+    const float u = x / ((float)Screen.width - 1.0f), v = y / ((float)Screen.height - 1.0f);
+    const float local[3] = {(u - 0.5f) * planeWidth, (v - 0.5f) * planeHeight, 1.0f * focusDistance};
+    float o[3], d[3];
+    for (int a = 0; a < 3; a++)
+    {
+        o[a] = ((M[a] * 0.0f + M[4 + a] * 0.0f) + M[8 + a] * 0.0f) + M[12 + a] * 1.0f;
+        const float f = ((M[a] * local[0] + M[4 + a] * local[1]) + M[8 + a] * local[2]) + M[12 + a] * 1.0f;
+        d[a] = f - o[a];
+    }
+    const float inv = 1.0f / std::sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]);
+    for (int a = 0; a < 3; a++) { ray->origin[a] = o[a]; ray->dir[a] = d[a] * inv; }
+}
+
+int RayComputeManager::Pick(float x, float y, RtRayHit* hit)
+{
+    RtRay ray;
+    PickRay(x, y, &ray);
+    return TraceRays(&ray, 1, hit, 0);
 }
 
 int RayComputeManager::WaitReadback()

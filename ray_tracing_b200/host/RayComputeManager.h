@@ -57,6 +57,7 @@ struct RtApi
     decltype(&rtCreateMulti) CreateMulti = nullptr;   // optional: several GPUs behind one context (the all-gather of tiles inside rtDispatch)
     decltype(&rtReadbackPixelStats) ReadbackPixelStats = nullptr; decltype(&rtDisplayPixelStats) DisplayPixelStats = nullptr;   // optional: debug view
     decltype(&rtDispatchFrames) DispatchFrames = nullptr;   // optional: several accumulated frames in one launch (RenderFrames)
+    decltype(&rtTraceRays) TraceRays = nullptr;             // optional: closest-hit queries (TraceRays / Pick)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -125,6 +126,13 @@ public:
     // their heat map (visMode 1 box tests / ray, 2 triangle tests / ray, 3 sphere tests / ray, 4 rays; debugVisScale = full white)
     int ReadPixelStats(RtPixelStats* dst, size_t bytes);
     int DisplayDebugView(int visMode, float debugVisScale, uint8_t* dst, size_t bytes);
+    // not in the reference: the closest hit of caller-supplied rays against the current scene (rtTraceRays; flags RT_TRACE_NO_CULL).
+    // The scene is uploaded first as a frame would upload it; the render textures are not touched.
+    int TraceRays(const RtRay* rays, int n, RtRayHit* hits, int flags = 0);
+    // picking / autofocus: the un-jittered camera ray through pixel (x, y) of the screen — SetupPixel's operations (HL:547-558) on the
+    // manager's own camera fields — and its closest hit
+    void PickRay(float x, float y, RtRay* ray) const;
+    int Pick(float x, float y, RtRayHit* hit);
     RtContext* Context() const { return ctx; }
     const RtApi& Api() const { return api; }
 

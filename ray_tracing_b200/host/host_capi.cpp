@@ -234,6 +234,16 @@ int rcmReadAccumulated(void* hv, float* dst, size_t bytes) { Handle* h = (Handle
 int rcmReadPixelStats(void* hv, RtPixelStats* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadPixelStats(dst, bytes); }
 int rcmDisplayDebugView(void* hv, int visMode, float debugVisScale, uint8_t* dst, size_t bytes)
 { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->DisplayDebugView(visMode, debugVisScale, dst, bytes); }
+int rcmTraceRays(void* hv, const RtRay* rays, int n, RtRayHit* hits, int flags)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TraceRays(rays, n, hits, flags); } CATCH_ALL(h) }
+/* the pick ray through pixel (x, y) into *ray (may be NULL) and its closest hit into *hit (may be NULL: the ray alone) */
+int rcmPick(void* hv, float x, float y, RtRay* ray, RtRayHit* hit)
+{
+    Handle* h = (Handle*)hv; GUARD(h);
+    if (ray) h->mgr->PickRay(x, y, ray);
+    if (!hit) return RT_OK;
+    try { return h->mgr->Pick(x, y, hit); } CATCH_ALL(h)
+}
 
 /* BVH statistics of the last build: writes up to cap entries of 9 ints each (see rthBuildBVH); returns the mesh count */
 int rcmGetBVHStats(void* hv, int* out, int cap)

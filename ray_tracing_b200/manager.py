@@ -63,6 +63,8 @@ def host_lib() -> C.CDLL:
         L.rcmGetBVHStats.argtypes = [vp, vp, ci]
         L.rcmReadPixelStats.argtypes = [vp, vp, C.c_size_t]
         L.rcmDisplayDebugView.argtypes = [vp, ci, cf, vp, C.c_size_t]
+        L.rcmTraceRays.argtypes = [vp, vp, ci, vp, ci]
+        L.rcmPick.argtypes = [vp, cf, cf, vp, vp]
         _host = L
     return _host
 
@@ -273,6 +275,29 @@ class RayComputeManager:
         out = np.empty((h, w, 4), dtype=np.uint8)
         self._ck(self._L.rcmDisplayDebugView(self._h, int(visMode), float(debugVisScale), out.ctypes.data, out.nbytes))
         return out
+
+    # -- closest-hit queries against the current scene (rtTraceRays): picking, autofocus, line of sight
+    def trace_rays(self, rays, dirs=None, no_cull: bool = False) -> np.ndarray:
+        """The closest hit of every ray (capi.RAY_DTYPE array, or (n, 3) origins with (n, 3) dirs) as n capi.RAY_HIT_DTYPE records.
+        The scene is uploaded as a frame would upload it; the render textures are not touched."""
+        r = capi.make_rays(rays, dirs)
+        hits = np.empty(r.shape[0], dtype=capi.RAY_HIT_DTYPE)
+        self._ck(self._L.rcmTraceRays(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), hits.ctypes.data if hits.size else None,
+                                      capi.RT_TRACE_NO_CULL if no_cull else 0))
+        return hits
+
+    def pick_ray(self, x: float, y: float) -> np.ndarray:
+        """The un-jittered camera ray through pixel (x, y) (row 0 = bottom), as one capi.RAY_DTYPE record."""
+        ray = np.zeros(1, dtype=capi.RAY_DTYPE)
+        self._ck(self._L.rcmPick(self._h, float(x), float(y), ray.ctypes.data, None))
+        return ray[0]
+
+    def pick(self, x: float, y: float) -> np.ndarray:
+        """What lies under pixel (x, y): the closest hit of pick_ray(x, y), one capi.RAY_HIT_DTYPE record (kind / index name the
+        Spheres or ModelInfo entry; dst is the distance along the unit-length ray, e.g. for focusDistance)."""
+        hit = np.zeros(1, dtype=capi.RAY_HIT_DTYPE)
+        self._ck(self._L.rcmPick(self._h, float(x), float(y), None, hit.ctypes.data))
+        return hit[0]
 
     def bvh_stats(self) -> list[dict]:
         buf = np.zeros(9 * 64, dtype=np.int32)

@@ -4,10 +4,14 @@ emissive materials, sky, defocus, near / far / inside cameras, extreme scales) r
 interpreter build (tests/simt) with random options, compared bit for bit with the oracle.  Found the distant-camera defect of the
 model skipping in round 1 by hand-made cases; this keeps looking.  Every failure prints the seed that reproduces it.
 
-    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats]
+    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats] [--queries]
 
 --pixel-stats: wherever the traversal totals are compared (counting launches of whole images), also compare the per-pixel counters
 (PixelStats: rays, box and triangle tests everywhere; sphere tests too when the Spheres buffer is below the accelerator's threshold).
+
+--queries: every scene also traces a random batch of rays (rtTraceRays, tests/test_gpu_trace_rays.py ray_sets: pick rays, origins in the
+scene, inside its meshes and spheres, 1e3 - 1e5 units out, special directions and NaN / inf) with either flag, compared bit for bit
+with the oracle (a NaN must be a NaN on both sides), and with "countStats" the counters the batch added.
 """
 import argparse
 import os
@@ -24,6 +28,7 @@ import build as simt_build                      # noqa: E402
 from conftest import ORACLE_LIB, render        # noqa: E402
 import ray_tracing_b200 as rt                   # noqa: E402
 from ray_tracing_b200 import scenes             # noqa: E402
+from test_gpu_trace_rays import assert_hits_equal, ray_sets      # noqa: E402  (the query batch of the rtTraceRays tests)
 
 
 def render_pixel_stats(lib, sc, frames, options, tile=None):
@@ -40,6 +45,21 @@ def render_pixel_stats(lib, sc, frames, options, tile=None):
     for _ in range(frames):
         mgr.RenderFrame()
     out = (mgr.raytraceFrameTex, mgr.accumulatedResult, ctx.stats(), mgr.pixel_stats() if (options or {}).get("countStats") else None)
+    mgr.OnDestroy()
+    return out
+
+
+def trace_batch(lib, sc, options, rays, no_cull):
+    """rtTraceRays of `rays` on a fresh context of the scene (after OnEnable), with the RtStats counters the batch added."""
+    mgr = rt.RayComputeManager(lib)
+    scenes.apply(sc, mgr)
+    ctx = mgr.context
+    for k, v in (options or {}).items():
+        ctx.set_option(k, v)
+    mgr.OnEnable()
+    ctx.reset_stats()
+    hits = ctx.trace_rays(rays, no_cull=no_cull)
+    out = (hits, ctx.stats())
     mgr.OnDestroy()
     return out
 
@@ -192,9 +212,11 @@ def main():
     ap.add_argument("--spheres", type=float, default=0.05, help="share of cases of the large-Spheres-buffer class")
     ap.add_argument("--far", type=float, default=0.05, help="share of cases of the many-small-models-from-afar class")
     ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters wherever the totals are compared")
+    ap.add_argument("--queries", action="store_true", help="also trace a random batch of rays through every scene (rtTraceRays) against the oracle")
+    ap.add_argument("--query-rays", type=int, default=32, help="rays per kind in a --queries batch")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
-    bad, pix_cases, t0 = 0, 0, time.time()
+    bad, pix_cases, query_cases, t0 = 0, 0, 0, time.time()
     for case in range(args.cases):
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
@@ -227,9 +249,27 @@ def main():
             bad += 1
             print(f"case seed {seed}: {int(diff.sum())} values differ, counters {'ok' if counters_ok else 'DIFFER'}, PixelStats {pix_bad or 'ok'}; {len(sc.models)} models, {len(sc.spheres)} spheres, "
                   f"{sc.width}x{sc.height}, frames {frames}, options {opts}, tile {tile}, settings {sc.settings}", flush=True)
+        if args.queries:
+            # pick rays, origins inside the scene and inside its meshes / spheres, 1e3 - 1e5 units out, axis-aligned / zero / NaN / inf
+            sets = ray_sets(sc, seed=seed, n=args.query_rays)
+            batch = np.concatenate(list(sets.values()))
+            batch = batch[rng.permutation(len(batch))]
+            no_cull = bool(rng.rand() < 0.5)
+            q_opts = {k: v for k, v in opts.items() if k in ("tlas", "modelSkip", "extInstantiation", "countStats", "smemNodes", "pairOrder")}
+            try:
+                want, so = trace_batch(ORACLE_LIB, sc, {}, batch, no_cull)
+                got, sg = trace_batch(lib, sc, q_opts, batch, no_cull)
+                assert_hits_equal(got, want, "rtTraceRays")
+                keys = ("rays", "boxTests", "triTests") + (("sphereTests",) if len(sc.spheres) <= 64 else ())
+                assert not q_opts.get("countStats") or all(sg[k] == so[k] for k in keys), f"counters {sg} vs {so}"
+                query_cases += 1
+            except Exception as e:
+                bad += 1
+                print(f"case seed {seed}: queries: {type(e).__name__}: {e}   options {q_opts}, no_cull {no_cull}, {len(sc.models)} models, {len(sc.spheres)} spheres", flush=True)
         if (case + 1) % 25 == 0:
             print(f"  {case + 1} cases, {bad} findings, {time.time() - t0:.0f} s", flush=True)
-    print(f"{args.cases} cases, {bad} findings" + (f"; PixelStats compared in {pix_cases} cases" if args.pixel_stats else ""))
+    print(f"{args.cases} cases, {bad} findings" + (f"; PixelStats compared in {pix_cases} cases" if args.pixel_stats else "")
+          + (f"; query batches equal in {query_cases} cases" if args.queries else ""))
     return 1 if bad else 0
 
 
