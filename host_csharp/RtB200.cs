@@ -60,6 +60,12 @@ public static class RtB200
     public struct RayHit { public float dst; public UnityEngine.Vector3 pos, normal; public int isBackface, kind, index, pad0, pad1; }
     [DllImport(Lib)] public static extern int rtTraceRays(IntPtr ctx, Ray[] rays, int n, [Out] RayHit[] hits, int flags);
     [DllImport(Lib)] public static extern int rtTraceRaysDevice(IntPtr ctx, IntPtr dRays, IntPtr dHits, int n, int flags);
+    // occlusion queries: is anything on origin + t * dir, 0 <= t < tMax?  Shadow rays (tMax just below 1 with dir = light point - origin),
+    // ambient occlusion, line of sight.  occluded[i] = 1 or 0; stops at the first hit, so cheaper than rtTraceRays for yes / no questions
+    [StructLayout(LayoutKind.Sequential)]
+    public struct RaySegment { public UnityEngine.Vector3 origin, dir; public float tMax; }
+    [DllImport(Lib)] public static extern int rtTraceOcclusion(IntPtr ctx, RaySegment[] segs, int n, [Out] byte[] occluded, int flags);
+    [DllImport(Lib)] public static extern int rtTraceOcclusionDevice(IntPtr ctx, IntPtr dSegs, IntPtr dOccluded, int n, int flags);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

@@ -131,6 +131,28 @@ int rtDispatchFrames(RtContext* ctx, int groupsX, int groupsY, int groupsZ, int 
 int rtTraceRays(RtContext* ctx, const RtRay* rays, int n, RtRayHit* hits, int flags);
 int rtTraceRaysDevice(RtContext* ctx, const void* dRays, void* dHits, int n, int flags);
 
+/* Extension: occlusion queries for caller-supplied segments (shadow and ambient-occlusion rays, line of sight, visibility baking).
+ * occluded[i] = 1 if and only if CalculateRayCollision(ray, forceDontCullBack = flags & RT_TRACE_NO_CULL) (HL:335-374, sphere
+ * extension first) finds a hit when its result.dst starts at segs[i].tMax instead of +inf; 0 otherwise.  Every < stays strict, as in
+ * the reference: TMax as DXR / OptiX define it, in the reference's own arithmetic.  The walk stops at its first hit.  That is exact
+ * whatever order the primitives are visited in: before the first hit the running bound is the constant tMax, so a box is entered when
+ * its entry is < tMax and a primitive counts when its dst < tMax, whatever was visited before.
+ *   - This is NOT always rtTraceRays(ray).dst < tMax: a box whose float entry is >= tMax can hold a triangle whose float hit is < tMax;
+ *     the reference from +inf enters that box, a walk bounded by tMax does not.  occluded = 1 implies rtTraceRays(ray).dst < tMax, and
+ *     with tMax = +inf the two are equal (occluded == (kind != RT_HIT_NONE)).
+ *   - tMax needs no validation: NaN, 0, -0 and negative values are never occluded (every comparison with them fails); +inf is any hit.
+ *   - With "countStats" = 1 the box / triangle / sphere counters count the walk in the reference's order (spheres in buffer order,
+ *     then every model in buffer order, each BVH near child first) up to and including the test that produced the first hit; with
+ *     the sphere accelerator the sphere counters are the accelerator's, as in rtTraceRays.
+ *   - Everything else is rtTraceRays': what it reads and leaves alone, RtStats.rays growing by n, the conditions under which model
+ *     skipping, the TLAS and the sphere accelerator are used, the grazing-ray defect, devices[0] on a group context, the refusals (with
+ *     dSegs 4-byte aligned, dOccluded unaligned) and n = 0.
+ * rtTraceOcclusion: host arrays, in batches of at most RT_TRACE_CHUNK_RAYS through the two device buffers rtTraceRays keeps (29 of their
+ * 72 bytes per segment); synchronises.  rtTraceOcclusionDevice: n RtRaySegment / bytes in device memory of the context's device, no
+ * allocation; asynchronous on the context's stream (rtSetStream). */
+int rtTraceOcclusion(RtContext* ctx, const RtRaySegment* segs, int n, uint8_t* occluded, int flags);
+int rtTraceOcclusionDevice(RtContext* ctx, const void* dSegs, void* dOccluded, int n, int flags);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),

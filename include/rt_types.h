@@ -93,6 +93,14 @@ typedef struct RtRayHit {
     int32_t pad[2];       /* 0 */
 } RtRayHit;
 
+/* A caller-supplied segment of rtTraceOcclusion / rtTraceOcclusionDevice (include/rt_b200.h): the points origin + t * dir with
+ * 0 <= t < tMax, t in multiples of dir as RtRayHit.dst is. */
+typedef struct RtRaySegment {
+    float origin[3];
+    float dir[3];
+    float tMax;
+} RtRaySegment;
+
 #pragma pack(pop)
 
 #ifdef __cplusplus
@@ -100,6 +108,7 @@ typedef struct RtRayHit {
 static_assert(sizeof(RtPixelStats) == 20, "PixelStats record");
 static_assert(sizeof(RtRay) == 24, "RtRay record");
 static_assert(sizeof(RtRayHit) == 48, "RtRayHit record");
+static_assert(sizeof(RtRaySegment) == 28, "RtRaySegment record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

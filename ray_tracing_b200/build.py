@@ -91,10 +91,11 @@ def build_oracle(force: bool = False) -> str:
     # the oracle (oracle/rt_oracle.cpp) with its per-pixel counters (PixelStats) around it: the extension includes the oracle's
     # source unchanged and wraps the entry points that reach the counters (tests/oracle_ext/rt_oracle_pixel_stats.cpp); rtDispatchFrames
     # is the loop over single-frame dispatches around that (tests/oracle_ext/rt_oracle_frames.cpp); rtTraceRays is CalculateRayCollision
-    # per ray around that in turn (tests/oracle_ext/rt_oracle_trace_rays.cpp, the translation unit built here)
+    # per ray around that in turn (tests/oracle_ext/rt_oracle_trace_rays.cpp); rtTraceOcclusion is its tMax-bounded early-exit walk
+    # around that (tests/oracle_ext/rt_oracle_occlusion.cpp, the translation unit built here)
     srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(ORACLE_EXT, (".cpp",)) + _glob(INCLUDE, (".h",))
     if force or _newer(LIB_ORACLE, srcs):
-        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_trace_rays.cpp")])
+        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_occlusion.cpp")])
     return LIB_ORACLE
 
 

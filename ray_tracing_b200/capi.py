@@ -68,6 +68,31 @@ def make_rays(origins, dirs=None) -> np.ndarray:
     return rays
 
 
+# rtTraceOcclusion: a caller-supplied segment, origin + t * dir for 0 <= t < tMax (RtRaySegment)
+SEGMENT_DTYPE = np.dtype([("origin", "<f4", 3), ("dir", "<f4", 3), ("tMax", "<f4")])
+assert SEGMENT_DTYPE.itemsize == 28
+
+
+def make_segments(origins, dirs=None, t_max=None) -> np.ndarray:
+    """A SEGMENT_DTYPE array from a structured array (returned as it is) or from (n, 3) origins, (n, 3) directions and n tMax values
+    (a scalar applies to every segment)."""
+    if dirs is None:
+        segs = np.asarray(origins)
+        if segs.dtype != SEGMENT_DTYPE:
+            raise TypeError(f"segments must have dtype {SEGMENT_DTYPE} (or pass origins, dirs and t_max)")
+        return np.ascontiguousarray(segs).reshape(-1)
+    if t_max is None:
+        raise ValueError("t_max is required with origins and dirs")
+    o = np.asarray(origins, dtype=np.float32).reshape(-1, 3)
+    d = np.asarray(dirs, dtype=np.float32).reshape(-1, 3)
+    if o.shape != d.shape:
+        raise ValueError("origins and dirs must both be (n, 3)")
+    segs = np.empty(o.shape[0], dtype=SEGMENT_DTYPE)
+    segs["origin"], segs["dir"] = o, d
+    segs["tMax"] = np.broadcast_to(np.asarray(t_max, dtype=np.float32).reshape(-1), (o.shape[0],))
+    return segs
+
+
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
                 ("dispatches", C.c_uint64), ("kernelMs", C.c_double), ("sphereBoxTests", C.c_uint64), ("exchangeMs", C.c_double)]
@@ -131,11 +156,14 @@ class RtLib:
             "rtDispatchFrames": ([vp, ci, ci, ci, ci], ci),
             "rtTraceRays": ([vp, vp, ci, vp, ci], ci),
             "rtTraceRaysDevice": ([vp, vp, vp, ci, ci], ci),
+            "rtTraceOcclusion": ([vp, vp, ci, vp, ci], ci),
+            "rtTraceOcclusionDevice": ([vp, vp, vp, ci, ci], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
-                            "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice"):      # absent from older experimental builds used in A/B runs
+                            "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
+                            "rtTraceOcclusion", "rtTraceOcclusionDevice"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -261,6 +289,20 @@ class RtContext:
         """rtTraceRaysDevice: n RtRay at rays_ptr -> n RtRayHit at hits_ptr (16-byte aligned), both device memory of the context's GPU
         (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtTraceRaysDevice(self._h, C.c_void_p(rays_ptr), C.c_void_p(hits_ptr), int(n), RT_TRACE_NO_CULL if no_cull else 0))
+
+    def trace_occlusion(self, segs, no_cull: bool = False) -> np.ndarray:
+        """rtTraceOcclusion: for every segment (a SEGMENT_DTYPE array, see make_segments), whether anything lies on it — a hit with
+        dst < tMax as the path tracer computes it.  Returns n bools.  no_cull: back faces count for every model (forceDontCullBack)."""
+        s = make_segments(segs)
+        occ = np.empty(s.shape[0], dtype=np.uint8)
+        self._ck(self._L.rtTraceOcclusion(self._h, s.ctypes.data if s.size else None, int(s.shape[0]), occ.ctypes.data if occ.size else None,
+                                          RT_TRACE_NO_CULL if no_cull else 0))
+        return occ.view(np.bool_)
+
+    def trace_occlusion_device(self, segs_ptr: int, occluded_ptr: int, n: int, no_cull: bool = False):
+        """rtTraceOcclusionDevice: n RtRaySegment at segs_ptr (4-byte aligned) -> n bytes (1 = occluded) at occluded_ptr, both device
+        memory of the context's GPU (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
+        self._ck(self._L.rtTraceOcclusionDevice(self._h, C.c_void_p(segs_ptr), C.c_void_p(occluded_ptr), int(n), RT_TRACE_NO_CULL if no_cull else 0))
 
     def readback(self, tex: str, out: Optional[np.ndarray] = None) -> np.ndarray:
         if out is None:

@@ -101,6 +101,7 @@ struct RtContext
     unsigned int* dWork = nullptr;
     DevBuf<RtPixelStats> pixelStats;           // "PixelStats": W*H per-pixel counters of the counting launches (allocated by the first one)
     DevBuf<RtRay> queryRays; DevBuf<RtRayHit> queryHits;     // rtTraceRays: device copies of one batch (<= RT_TRACE_CHUNK_RAYS) of the caller's host arrays
+                                                             // (rtTraceOcclusion: its segments in queryHits, its bytes in queryRays)
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -613,15 +614,15 @@ static int prepareScene(RtContext* c)
     return fitOriginPadding(c);
 }
 
-// rtTraceRays: what does not depend on the image or the kernel choice.  A layout that is already built is kept whatever its budget
-// (a query reads every record from global memory); a scene that must be planned anyway gets the layout the next dispatch would ask
-// for, so that with default options the query never makes that dispatch plan again.
-static int prepareQueryScene(RtContext* c)
+// rtTraceRays / rtTraceOcclusion: what does not depend on the image or the kernel choice.  A layout that is already built is kept
+// whatever its budget (a query reads every record from global memory); a scene that must be planned anyway gets the layout the next
+// dispatch would ask for, so that with default options the query never makes that dispatch plan again.
+static int prepareQueryScene(RtContext* c, const char* what)
 {
-    int rc = checkScene(c, "rtTraceRays"); if (rc != RT_OK) return rc;
+    int rc = checkScene(c, what); if (rc != RT_OK) return rc;
     int budget, pairOrder; bool treelets;
     sceneLayout(c, budget, pairOrder, treelets);
-    if ((rc = planSceneIfDirty(c, "rtTraceRays", budget, pairOrder, treelets)) != RT_OK) return rc;
+    if ((rc = planSceneIfDirty(c, what, budget, pairOrder, treelets)) != RT_OK) return rc;
     return fitOriginPadding(c);
 }
 
@@ -1039,7 +1040,7 @@ int rtDispatchFrames(RtContext* c, int gx, int gy, int gz, int frameCount)
     return exchangeTiles(all.data(), (int)all.size());
 }
 
-// ---- closest-hit queries (rtTraceRays, rt_kernel_query.cuh) -----------------------------------------------------------------------
+// ---- closest-hit and occlusion queries (rtTraceRays, rtTraceOcclusion, rt_kernel_query.cuh) -----------------------------------------
 static int stagedH2D(RtContext* c, void* dst, const void* src, size_t bytes);
 static int stagedD2H(RtContext* c, void* dst, const void* src, size_t bytes);
 
@@ -1051,25 +1052,46 @@ static int traceArgs(RtContext* c, const char* what, const void* rays, const voi
     return RT_OK;
 }
 
-// n rays in device memory of this context's GPU -> n hits; asynchronous on the context's stream.  RtStats.rays grows by n through the
-// kernel's counters; no timing events, so dispatches / kernelMs stay the camera kernels'.
-static int traceLocal(RtContext* c, const RtRay* dRays, RtRayHit* dHits, int n, int flags)
+// n rays (Q.rays -> Q.hits) or, with `occlusion`, n segments (Q.segs -> Q.occluded) in device memory of this context's GPU;
+// asynchronous on the context's stream.  RtStats.rays grows by n through the kernel's counters; no timing events, so dispatches /
+// kernelMs stay the camera kernels'.
+static int queryLocal(RtContext* c, const char* what, QueryParams& Q, int n, int flags, bool occlusion)
 {
-    int rc = prepareQueryScene(c); if (rc != RT_OK) return rc;
+    int rc = prepareQueryScene(c, what); if (rc != RT_OK) return rc;
     DevParams P = c->P;
     bindScene(c, P);
     P.countStats = c->optCountStats;
     P.smemPairs = 0;                                 // no tree-top staging: every record from global memory
     P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
-    QueryParams Q;
-    Q.rays = dRays; Q.hits = dHits; Q.n = (unsigned int)n; Q.noCull = flags & RT_TRACE_NO_CULL;
+    Q.n = (unsigned int)n; Q.noCull = flags & RT_TRACE_NO_CULL;
     for (int a = 0; a < 3; a++)
     {
         Q.modelLo[a] = c->repack.modelBoundLo[a]; Q.modelHi[a] = c->repack.modelBoundHi[a];
         Q.sphLo[a] = c->repack.sphBoundLo[a]; Q.sphHi[a] = c->repack.sphBoundHi[a];
     }
-    cudaError_t e = query_launch(P, Q, c->numSMs, c->stream);
-    if (e != cudaSuccess) return failCuda(c, e, "rtTraceRays launch");
+    cudaError_t e = occlusion ? query_launch<true>(P, Q, c->numSMs, c->stream) : query_launch<false>(P, Q, c->numSMs, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, occlusion ? "rtTraceOcclusion launch" : "rtTraceRays launch");
+    return RT_OK;
+}
+
+static int traceLocal(RtContext* c, const RtRay* dRays, RtRayHit* dHits, int n, int flags)
+{
+    QueryParams Q = {};
+    Q.rays = dRays; Q.hits = dHits;
+    return queryLocal(c, "rtTraceRays", Q, n, flags, false);
+}
+
+static int occlusionLocal(RtContext* c, const RtRaySegment* dSegs, unsigned char* dOccluded, int n, int flags)
+{
+    QueryParams Q = {};
+    Q.segs = dSegs; Q.occluded = dOccluded;
+    return queryLocal(c, "rtTraceOcclusion", Q, n, flags, true);
+}
+
+// The device buffers of the host forms: one batch of at most RT_TRACE_CHUNK_RAYS records, 72 bytes each (72 MiB at most)
+static int queryBuffers(RtContext* c, int chunk)
+{
+    if (c->queryRays.cap < (size_t)chunk) { CK(c->queryRays.ensure((size_t)chunk)); CK(c->queryHits.ensure((size_t)chunk)); }
     return RT_OK;
 }
 
@@ -1081,7 +1103,7 @@ int rtTraceRays(RtContext* c, const RtRay* rays, int n, RtRayHit* hits, int flag
     CK(cudaSetDevice(c->device));
     // batches of at most RT_TRACE_CHUNK_RAYS through device buffers of that size, kept by the context (72 MB at most)
     const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
-    if (c->queryRays.cap < (size_t)chunk) { CK(c->queryRays.ensure((size_t)chunk)); CK(c->queryHits.ensure((size_t)chunk)); }
+    if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
     for (int i0 = 0; i0 < n; i0 += chunk)
     {
         const int m = n - i0 < chunk ? n - i0 : chunk;
@@ -1101,6 +1123,39 @@ int rtTraceRaysDevice(RtContext* c, const void* dRays, void* dHits, int n, int f
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     return traceLocal(c, (const RtRay*)dRays, (RtRayHit*)dHits, n, flags);
+}
+
+// The segments travel in queryHits (28 of its 48 bytes per record) and the answers in queryRays (1 of 24), so an occlusion batch needs
+// no memory beyond what a closest-hit batch of the same size keeps.
+int rtTraceOcclusion(RtContext* c, const RtRaySegment* segs, int n, uint8_t* occluded, int flags)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = traceArgs(c, "rtTraceOcclusion", segs, occluded, n, flags); if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
+    if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
+    RtRaySegment* dSegs = reinterpret_cast<RtRaySegment*>(c->queryHits.p);
+    unsigned char* dOccluded = reinterpret_cast<unsigned char*>(c->queryRays.p);
+    for (int i0 = 0; i0 < n; i0 += chunk)
+    {
+        const int m = n - i0 < chunk ? n - i0 : chunk;
+        if ((rc = stagedH2D(c, dSegs, segs + i0, (size_t)m * sizeof(RtRaySegment))) != RT_OK) return rc;
+        if ((rc = occlusionLocal(c, dSegs, dOccluded, m, flags)) != RT_OK) return rc;
+        if ((rc = stagedD2H(c, occluded + i0, dOccluded, (size_t)m)) != RT_OK) return rc;
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rtTraceOcclusionDevice(RtContext* c, const void* dSegs, void* dOccluded, int n, int flags)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = traceArgs(c, "rtTraceOcclusionDevice", dSegs, dOccluded, n, flags); if (rc != RT_OK) return rc;
+    if ((uintptr_t)dSegs & 3u) return fail(c, RT_E_INVALID, "rtTraceOcclusionDevice: dSegs must be 4-byte aligned");
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    return occlusionLocal(c, (const RtRaySegment*)dSegs, (unsigned char*)dOccluded, n, flags);
 }
 
 int rtExchangeTiles(RtContext* c)

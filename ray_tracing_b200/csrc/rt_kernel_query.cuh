@@ -1,9 +1,11 @@
-// rt_kernel_query.cuh — rtTraceRays: the closest hit of caller-supplied rays (picking, autofocus, line of sight, visibility baking).
+// rt_kernel_query.cuh — rtTraceRays: the closest hit of caller-supplied rays (picking, autofocus, line of sight, visibility baking);
+// rtTraceOcclusion: whether anything lies on caller-supplied segments (shadow and ambient-occlusion rays, line of sight).
 //
 // Each lane traces one ray through the camera kernels' own Intersect (rt_kernel_wave.cuh), so a query returns the bits the path tracer
 // computes for the same ray.  Shape: a persistent grid (a multiple of the SM count); every warp reserves 32 consecutive rays with one
 // atomicAdd, each lane traces one of them and writes its 48-byte RtRayHit as three 16-byte stores.  Spheres are staged in shared
-// memory as in wave_body; tree tops are not (smemPairs = 0).
+// memory as in wave_body; tree tops are not (smemPairs = 0).  k_trace_occlusion has the same shape: each lane walks its segment through
+// Intersect<..., ANY = true> (from tMax, ended by the first hit) and stores one byte.
 //
 // Model skipping, the TLAS and the sphere accelerator are exact only for origins inside the box their records were padded for (the
 // camera with its defocus disc and all geometry, RepackState::buildModels / buildSpheres).  Camera rays are inside by construction;
@@ -29,6 +31,8 @@ struct QueryParams
     int noCull;                                  // RT_TRACE_NO_CULL: forceDontCullBack (HL:356)
     float modelLo[3], modelHi[3];                // origins the model records (world boxes, TLAS) were padded for
     float sphLo[3], sphHi[3];                    // origins the sphere accelerator was padded for
+    const RtRaySegment* segs;                    // rtTraceOcclusion: the segments and their answers (rays / hits unused)
+    unsigned char* occluded;
 };
 
 constexpr float QUERY_DIR2_MIN = 9.5367431640625e-07f;      // 2^-20: |dir| >= 2^-10
@@ -45,8 +49,9 @@ RT_DI bool DirectionInRange(f3 d)
     return dd >= QUERY_DIR2_MIN && dd <= QUERY_DIR2_MAX;
 }
 
-template <bool STATS, bool EXT, bool TLAS>
-__global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_rays(const __grid_constant__ DevParams P, const __grid_constant__ QueryParams Q)
+// One persistent grid over Q.n rays (ANY = false: RtRay -> RtRayHit) or segments (ANY = true: RtRaySegment -> one byte, 1 = occluded)
+template <bool STATS, bool EXT, bool TLAS, bool ANY>
+RT_DI void query_body(const DevParams& P, const QueryParams& Q)
 {
     RT_DYNAMIC_SMEM(smemRaw);
     DevSphere* smemSpheres = reinterpret_cast<DevSphere*>(smemRaw);
@@ -67,7 +72,7 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_rays(
         const unsigned int i = base + lane;
         if (i < Q.n)
         {
-            const float* r = reinterpret_cast<const float*>(Q.rays + i);
+            const float* r = ANY ? reinterpret_cast<const float*>(Q.segs + i) : reinterpret_cast<const float*>(Q.rays + i);
             const f3 o = make_f3(__ldg(r), __ldg(r + 1), __ldg(r + 2));
             const f3 d = make_f3(__ldg(r + 3), __ldg(r + 4), __ldg(r + 5));
             QueryRay q;
@@ -75,11 +80,20 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_rays(
             q.modelsExact = dirOk && OriginInside(o, Q.modelLo, Q.modelHi);
             q.spheresExact = dirOk && OriginInside(o, Q.sphLo, Q.sphHi);
             q.noCull = Q.noCull != 0;
-            const Hit h = Intersect<STATS, EXT, TLAS, true>(P, nullptr, smemSpheres, o, d, cnt, &q);
-            float4* out = reinterpret_cast<float4*>(Q.hits + i);
-            out[0] = make_float4(h.dst, h.pos.x, h.pos.y, h.pos.z);
-            out[1] = make_float4(h.normal.x, h.normal.y, h.normal.z, __int_as_float(h.isBackface ? 1 : 0));
-            out[2] = make_float4(__int_as_float(q.kind), __int_as_float(q.index), 0.0f, 0.0f);
+            if constexpr (ANY)
+            {
+                q.tMax = __ldg(r + 6);
+                Intersect<STATS, EXT, TLAS, true, true>(P, nullptr, smemSpheres, o, d, cnt, &q);
+                Q.occluded[i] = q.kind != RT_HIT_NONE ? 1 : 0;
+            }
+            else
+            {
+                const Hit h = Intersect<STATS, EXT, TLAS, true>(P, nullptr, smemSpheres, o, d, cnt, &q);
+                float4* out = reinterpret_cast<float4*>(Q.hits + i);
+                out[0] = make_float4(h.dst, h.pos.x, h.pos.y, h.pos.z);
+                out[1] = make_float4(h.normal.x, h.normal.y, h.normal.z, __int_as_float(h.isBackface ? 1 : 0));
+                out[2] = make_float4(__int_as_float(q.kind), __int_as_float(q.index), 0.0f, 0.0f);
+            }
         }
     }
 
@@ -92,11 +106,24 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_rays(
     }
 }
 
-template <bool S, bool X, bool T> inline cudaError_t query_launch_one(const DevParams& P, const QueryParams& Q, int numSMs, cudaStream_t stream)
+template <bool STATS, bool EXT, bool TLAS>
+__global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_rays(const __grid_constant__ DevParams P, const __grid_constant__ QueryParams Q)
 {
+    query_body<STATS, EXT, TLAS, false>(P, Q);
+}
+
+template <bool STATS, bool EXT, bool TLAS>
+__global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_occlusion(const __grid_constant__ DevParams P, const __grid_constant__ QueryParams Q)
+{
+    query_body<STATS, EXT, TLAS, true>(P, Q);
+}
+
+template <bool S, bool X, bool T, bool ANY> inline cudaError_t query_launch_one(const DevParams& P, const QueryParams& Q, int numSMs, cudaStream_t stream)
+{
+    auto kernel = ANY ? k_trace_occlusion<S, X, T> : k_trace_rays<S, X, T>;
     const size_t smemBytes = (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
     int ctasPerSM = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_trace_rays<S, X, T>, WAVE_THREADS, smemBytes);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
     if (e != cudaSuccess) return e;
     if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
     unsigned int grid = (unsigned int)(numSMs * ctasPerSM);                  // persistent: a multiple of the SM count
@@ -104,18 +131,20 @@ template <bool S, bool X, bool T> inline cudaError_t query_launch_one(const DevP
     const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
     if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
     if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_trace_rays<S, X, T>), P, Q);
+    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, Q);
     return cudaGetLastError();
 }
 
 // The instantiation follows the scene the way wave_launch chooses a camera kernel: the counting build walks every model; the TLAS
 // kernel when the scene has a TLAS and skipping is on; the extension family with the sphere accelerator (or "extInstantiation").
+// ANY: the occlusion kernels, chosen by the same rules.
+template <bool ANY = false>
 inline cudaError_t query_launch(const DevParams& P, const QueryParams& Q, int numSMs, cudaStream_t stream)
 {
     const bool ext = P.sphBvh != 0 || P.forceExt != 0;
-    if (P.countStats) return ext ? query_launch_one<true, true, false>(P, Q, numSMs, stream) : query_launch_one<true, false, false>(P, Q, numSMs, stream);
-    if (P.tlas && P.modelSkip) return query_launch_one<false, true, true>(P, Q, numSMs, stream);
-    return ext ? query_launch_one<false, true, false>(P, Q, numSMs, stream) : query_launch_one<false, false, false>(P, Q, numSMs, stream);
+    if (P.countStats) return ext ? query_launch_one<true, true, false, ANY>(P, Q, numSMs, stream) : query_launch_one<true, false, false, ANY>(P, Q, numSMs, stream);
+    if (P.tlas && P.modelSkip) return query_launch_one<false, true, true, ANY>(P, Q, numSMs, stream);
+    return ext ? query_launch_one<false, true, false, ANY>(P, Q, numSMs, stream) : query_launch_one<false, false, false, ANY>(P, Q, numSMs, stream);
 }
 
 } // namespace rtd

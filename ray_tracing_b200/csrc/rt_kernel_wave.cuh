@@ -93,8 +93,9 @@ RT_DI void LoadPair(const DevParams& P, const float4* __restrict__ smemPairs, in
     }
 }
 
-// HL:234-287 on the repacked streams.  Same visiting order and culling as the reference.
-template <bool STATS, bool STAGED>
+// HL:234-287 on the repacked streams.  Same visiting order and culling as the reference.  ANY (occlusion queries, rtTraceOcclusion):
+// return right after the first triangle that hits closer than rayLength; bestDst < rayLength then says that there was one.
+template <bool STATS, bool STAGED, bool ANY = false>
 RT_DI void TraverseMesh(const DevParams& P, const float4* __restrict__ smemPairs, f3 pos, f3 dir, f3 invDir, float rayLength,
                         NodeRef root, bool cullBackface,
                         float& bestDst, int& bestTri, float& bestU, float& bestV, float& bestDet, Counters& cnt)
@@ -116,7 +117,11 @@ RT_DI void TraverseMesh(const DevParams& P, const float4* __restrict__ smemPairs
                 const bool didHit = RayTriangleCore(pos, dir, make_f3(g0.x, g0.y, g0.z), make_f3(g0.w, g1.x, g1.y), make_f3(g1.z, g1.w, g2.x),
                                                     make_f3(g2.y, g2.z, g2.w), cullBackface, dst, u, v, det);
                 if (STATS) cnt.tri++;
-                if (didHit && dst < bestDst) { bestDst = dst; bestTri = cur.start + i; bestU = u; bestV = v; bestDet = det; }
+                if (didHit && dst < bestDst)
+                {
+                    bestDst = dst; bestTri = cur.start + i; bestU = u; bestV = v; bestDet = det;
+                    if (ANY) return;
+                }
             }
             if (stackCount == 0) return;
             cur = stack[--stackCount];
@@ -147,16 +152,22 @@ RT_DI void TraverseMesh(const DevParams& P, const float4* __restrict__ smemPairs
 // A caller-supplied ray (rtTraceRays, rt_kernel_query.cuh).  In: whether its origin lies inside the box of origins the model records
 // (modelsExact) and the sphere accelerator (spheresExact) were padded for — only then may the ray skip models, walk the TLAS or use
 // the accelerator — and whether back faces count for every model (forceDontCullBack, HL:356).  Out: the winner's kind (RT_HIT_*) and
-// its index in Spheres / ModelInfo.
-struct QueryRay { bool modelsExact, spheresExact, noCull; int kind, index; };
+// its index in Spheres / ModelInfo.  Occlusion queries (ANY) also bring the segment's end, tMax, and get kind != RT_HIT_NONE back when
+// something lies closer than it (kind then names the stage that found it; index stays -1).
+struct QueryRay { bool modelsExact, spheresExact, noCull; int kind, index; float tMax; };
 
 // HL:335-374 (+ sphere extension) on the repacked streams.  QUERY = rtTraceRays (q != nullptr); the camera kernels leave it false.
-template <bool STATS, bool EXT, bool TLAS, bool QUERY = false>
+// ANY (with QUERY) = rtTraceOcclusion: the same walk with result.dst starting at q->tMax instead of +inf, ended by the first hit.  Before
+// that hit the running bound is the constant tMax, so which boxes are entered and which primitives count does not depend on what was
+// visited before: the first hit exists exactly when the full walk from tMax finds one.  No position, normal or winner is computed.
+template <bool STATS, bool EXT, bool TLAS, bool QUERY = false, bool ANY = false>
 RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, const DevSphere* __restrict__ smemSpheres,
                     f3 rayPos, f3 rayDir, Counters& cnt, QueryRay* q = nullptr)
 {
+    static_assert(QUERY || !ANY, "occlusion queries are queries");
     Hit result;
     result.dst = inf32(); result.isBackface = false; result.normal = splat3(0.0f); result.pos = splat3(0.0f); result.material = nullptr;
+    if constexpr (ANY) result.dst = q->tMax;
     cnt.rays++;
     if constexpr (QUERY) { q->kind = RT_HIT_NONE; q->index = -1; }
 
@@ -166,9 +177,10 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
         int idx = 0x7fffffff, flag = 0;
         TraverseSpheres(P, rayPos, rayDir, result.dst, idx, bestInside, flag, cnt, STATS);
         // (queries: the accelerator's tie rule also keeps a "hit" at dst = +inf, which the reference's strict < never takes; such a hit
-        // needs a direction so short or long that dot(dir, dir) leaves the float range — camera rays are unit length)
+        // needs a direction so short or long that dot(dir, dir) leaves the float range — camera rays are unit length.  Occlusion
+        // queries start from tMax, so the same rule keeps a sphere at exactly dst = tMax: it counts only below tMax.)
         bool keep = idx != 0x7fffffff;
-        if constexpr (QUERY) keep = keep && result.dst < inf32();
+        if constexpr (QUERY) keep = keep && result.dst < (ANY ? q->tMax : inf32());
         if (keep) bestSphere = idx;
     }
     else
@@ -182,8 +194,11 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
         if (RaySphereCore(rayPos, rayDir, make_f3(cx, cy, cz), r2, dst, inside) && dst < result.dst)
         {
             result.dst = dst; bestSphere = i; bestInside = inside;
+            if (ANY) break;
         }
     }
+    if constexpr (ANY)
+        if (bestSphere >= 0) { q->kind = RT_HIT_SPHERE; return result; }
     if (bestSphere >= 0)
     {
         // HL:319-320 for the winner only (position / normal of a sphere hit depend on nothing but the winner)
@@ -229,7 +244,9 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
         bool cullBackface = meta.z != 0;
         if constexpr (QUERY) cullBackface = cullBackface && !q->noCull;
         float dst, u, v, det; int tri;
-        TraverseMesh<STATS, EXT>(P, smemPairs, localPos, localDir, invDir, result.dst, root, cullBackface, dst, tri, u, v, det, cnt);
+        TraverseMesh<STATS, EXT, ANY>(P, smemPairs, localPos, localDir, invDir, result.dst, root, cullBackface, dst, tri, u, v, det, cnt);
+        if constexpr (ANY)
+            if (dst < result.dst) { q->kind = RT_HIT_MODEL; return result; }
         if (dst < result.dst)
         {
             const float4* nq = reinterpret_cast<const float4*>(P.triNormals + tri);

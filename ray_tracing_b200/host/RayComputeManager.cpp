@@ -30,6 +30,7 @@ std::string RtApi::Load(const char* path)
     DisplayPixelStats = reinterpret_cast<decltype(DisplayPixelStats)>(dlsym(dl, "rtDisplayPixelStats"));
     DispatchFrames = reinterpret_cast<decltype(DispatchFrames)>(dlsym(dl, "rtDispatchFrames"));
     TraceRays = reinterpret_cast<decltype(TraceRays)>(dlsym(dl, "rtTraceRays"));
+    TraceOcclusion = reinterpret_cast<decltype(TraceOcclusion)>(dlsym(dl, "rtTraceOcclusion"));
     return "";
 }
 
@@ -299,6 +300,16 @@ int RayComputeManager::TraceRays(const RtRay* rays, int n, RtRayHit* hits, int f
     int rc;
     if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
     TRY(api.TraceRays(ctx, rays, n, hits, flags));
+    return RT_OK;
+}
+
+int RayComputeManager::TraceOcclusion(const RtRaySegment* segs, int n, uint8_t* occluded, int flags)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.TraceOcclusion) { lastError = "the library does not export rtTraceOcclusion"; return RT_E_STATE; }
+    int rc;
+    if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
+    TRY(api.TraceOcclusion(ctx, segs, n, occluded, flags));
     return RT_OK;
 }
 

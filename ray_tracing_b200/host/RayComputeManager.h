@@ -58,6 +58,7 @@ struct RtApi
     decltype(&rtReadbackPixelStats) ReadbackPixelStats = nullptr; decltype(&rtDisplayPixelStats) DisplayPixelStats = nullptr;   // optional: debug view
     decltype(&rtDispatchFrames) DispatchFrames = nullptr;   // optional: several accumulated frames in one launch (RenderFrames)
     decltype(&rtTraceRays) TraceRays = nullptr;             // optional: closest-hit queries (TraceRays / Pick)
+    decltype(&rtTraceOcclusion) TraceOcclusion = nullptr;   // optional: occlusion queries (TraceOcclusion)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -129,6 +130,9 @@ public:
     // not in the reference: the closest hit of caller-supplied rays against the current scene (rtTraceRays; flags RT_TRACE_NO_CULL).
     // The scene is uploaded first as a frame would upload it; the render textures are not touched.
     int TraceRays(const RtRay* rays, int n, RtRayHit* hits, int flags = 0);
+    // not in the reference: whether anything lies on caller-supplied segments (rtTraceOcclusion; occluded[i] = 1 or 0) — shadow rays,
+    // ambient occlusion, line of sight.  The scene is uploaded first as for TraceRays.
+    int TraceOcclusion(const RtRaySegment* segs, int n, uint8_t* occluded, int flags = 0);
     // picking / autofocus: the un-jittered camera ray through pixel (x, y) of the screen — SetupPixel's operations (HL:547-558) on the
     // manager's own camera fields — and its closest hit
     void PickRay(float x, float y, RtRay* ray) const;

@@ -236,6 +236,9 @@ int rcmDisplayDebugView(void* hv, int visMode, float debugVisScale, uint8_t* dst
 { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->DisplayDebugView(visMode, debugVisScale, dst, bytes); }
 int rcmTraceRays(void* hv, const RtRay* rays, int n, RtRayHit* hits, int flags)
 { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TraceRays(rays, n, hits, flags); } CATCH_ALL(h) }
+
+int rcmTraceOcclusion(void* hv, const RtRaySegment* segs, int n, uint8_t* occluded, int flags)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TraceOcclusion(segs, n, occluded, flags); } CATCH_ALL(h) }
 /* the pick ray through pixel (x, y) into *ray (may be NULL) and its closest hit into *hit (may be NULL: the ray alone) */
 int rcmPick(void* hv, float x, float y, RtRay* ray, RtRayHit* hit)
 {

@@ -64,6 +64,7 @@ def host_lib() -> C.CDLL:
         L.rcmReadPixelStats.argtypes = [vp, vp, C.c_size_t]
         L.rcmDisplayDebugView.argtypes = [vp, ci, cf, vp, C.c_size_t]
         L.rcmTraceRays.argtypes = [vp, vp, ci, vp, ci]
+        L.rcmTraceOcclusion.argtypes = [vp, vp, ci, vp, ci]
         L.rcmPick.argtypes = [vp, cf, cf, vp, vp]
         _host = L
     return _host
@@ -285,6 +286,16 @@ class RayComputeManager:
         self._ck(self._L.rcmTraceRays(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), hits.ctypes.data if hits.size else None,
                                       capi.RT_TRACE_NO_CULL if no_cull else 0))
         return hits
+
+    # -- occlusion queries (rtTraceOcclusion): shadow and ambient-occlusion rays, line of sight
+    def trace_occlusion(self, segs, no_cull: bool = False) -> np.ndarray:
+        """Whether anything lies on each segment (a capi.SEGMENT_DTYPE array, see capi.make_segments) as n bools.  The scene is
+        uploaded as a frame would upload it; the render textures are not touched."""
+        s = capi.make_segments(segs)
+        occ = np.empty(s.shape[0], dtype=np.uint8)
+        self._ck(self._L.rcmTraceOcclusion(self._h, s.ctypes.data if s.size else None, int(s.shape[0]), occ.ctypes.data if occ.size else None,
+                                           capi.RT_TRACE_NO_CULL if no_cull else 0))
+        return occ.view(np.bool_)
 
     def pick_ray(self, x: float, y: float) -> np.ndarray:
         """The un-jittered camera ray through pixel (x, y) (row 0 = bottom), as one capi.RAY_DTYPE record."""

@@ -4,7 +4,7 @@ emissive materials, sky, defocus, near / far / inside cameras, extreme scales) r
 interpreter build (tests/simt) with random options, compared bit for bit with the oracle.  Found the distant-camera defect of the
 model skipping in round 1 by hand-made cases; this keeps looking.  Every failure prints the seed that reproduces it.
 
-    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats] [--queries]
+    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats] [--queries] [--occlusion]
 
 --pixel-stats: wherever the traversal totals are compared (counting launches of whole images), also compare the per-pixel counters
 (PixelStats: rays, box and triangle tests everywhere; sphere tests too when the Spheres buffer is below the accelerator's threshold).
@@ -12,6 +12,10 @@ model skipping in round 1 by hand-made cases; this keeps looking.  Every failure
 --queries: every scene also traces a random batch of rays (rtTraceRays, tests/test_gpu_trace_rays.py ray_sets: pick rays, origins in the
 scene, inside its meshes and spheres, 1e3 - 1e5 units out, special directions and NaN / inf) with either flag, compared bit for bit
 with the oracle (a NaN must be a NaN on both sides), and with "countStats" the counters the batch added.
+
+--occlusion: every scene also traces a random batch of segments (rtTraceOcclusion): the rays of --queries with tMax at, one ulp below
+and one ulp above the oracle's closest hit, fractions of it, +inf and special values (tests/test_gpu_occlusion.py tmax_sets), with
+either flag, compared with the oracle's answers, and with "countStats" the early-exit counters the batch added.
 """
 import argparse
 import os
@@ -29,6 +33,7 @@ from conftest import ORACLE_LIB, render        # noqa: E402
 import ray_tracing_b200 as rt                   # noqa: E402
 from ray_tracing_b200 import scenes             # noqa: E402
 from test_gpu_trace_rays import assert_hits_equal, ray_sets      # noqa: E402  (the query batch of the rtTraceRays tests)
+from test_gpu_occlusion import assert_occlusion_equal, tmax_sets  # noqa: E402  (the segment lengths of the rtTraceOcclusion tests)
 
 
 def render_pixel_stats(lib, sc, frames, options, tile=None):
@@ -49,8 +54,9 @@ def render_pixel_stats(lib, sc, frames, options, tile=None):
     return out
 
 
-def trace_batch(lib, sc, options, rays, no_cull):
-    """rtTraceRays of `rays` on a fresh context of the scene (after OnEnable), with the RtStats counters the batch added."""
+def trace_batch(lib, sc, options, rays, no_cull, occlusion=False):
+    """rtTraceRays of `rays` (occlusion: rtTraceOcclusion of segments) on a fresh context of the scene (after OnEnable), with the
+    RtStats counters the batch added."""
     mgr = rt.RayComputeManager(lib)
     scenes.apply(sc, mgr)
     ctx = mgr.context
@@ -58,7 +64,7 @@ def trace_batch(lib, sc, options, rays, no_cull):
         ctx.set_option(k, v)
     mgr.OnEnable()
     ctx.reset_stats()
-    hits = ctx.trace_rays(rays, no_cull=no_cull)
+    hits = ctx.trace_occlusion(rays, no_cull=no_cull) if occlusion else ctx.trace_rays(rays, no_cull=no_cull)
     out = (hits, ctx.stats())
     mgr.OnDestroy()
     return out
@@ -214,9 +220,10 @@ def main():
     ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters wherever the totals are compared")
     ap.add_argument("--queries", action="store_true", help="also trace a random batch of rays through every scene (rtTraceRays) against the oracle")
     ap.add_argument("--query-rays", type=int, default=32, help="rays per kind in a --queries batch")
+    ap.add_argument("--occlusion", action="store_true", help="also trace a random batch of segments through every scene (rtTraceOcclusion) against the oracle")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
-    bad, pix_cases, query_cases, t0 = 0, 0, 0, time.time()
+    bad, pix_cases, query_cases, occlusion_cases, t0 = 0, 0, 0, 0, time.time()
     for case in range(args.cases):
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
@@ -266,10 +273,29 @@ def main():
             except Exception as e:
                 bad += 1
                 print(f"case seed {seed}: queries: {type(e).__name__}: {e}   options {q_opts}, no_cull {no_cull}, {len(sc.models)} models, {len(sc.spheres)} spheres", flush=True)
+        if args.occlusion:
+            orng = np.random.RandomState(seed + 7)
+            rays = np.concatenate(list(ray_sets(sc, seed=seed + 7, n=args.query_rays).values()))
+            no_cull = bool(orng.rand() < 0.5)
+            o_opts = {k: v for k, v in opts.items() if k in ("tlas", "modelSkip", "extInstantiation", "countStats", "smemNodes", "pairOrder")}
+            try:
+                closest, _ = trace_batch(ORACLE_LIB, sc, {}, rays, no_cull)
+                segs = np.concatenate(list(tmax_sets(rays, closest, seed=seed).values()))
+                segs = segs[orng.permutation(len(segs))]
+                want, so = trace_batch(ORACLE_LIB, sc, {}, segs, no_cull, occlusion=True)
+                got, sg = trace_batch(lib, sc, o_opts, segs, no_cull, occlusion=True)
+                assert_occlusion_equal(got, want, "rtTraceOcclusion", segs)
+                keys = ("rays", "boxTests", "triTests") + (("sphereTests",) if len(sc.spheres) <= 64 else ())
+                assert not o_opts.get("countStats") or all(sg[k] == so[k] for k in keys), f"counters {sg} vs {so}"
+                occlusion_cases += 1
+            except Exception as e:
+                bad += 1
+                print(f"case seed {seed}: occlusion: {type(e).__name__}: {e}   options {o_opts}, no_cull {no_cull}, {len(sc.models)} models, {len(sc.spheres)} spheres", flush=True)
         if (case + 1) % 25 == 0:
             print(f"  {case + 1} cases, {bad} findings, {time.time() - t0:.0f} s", flush=True)
     print(f"{args.cases} cases, {bad} findings" + (f"; PixelStats compared in {pix_cases} cases" if args.pixel_stats else "")
-          + (f"; query batches equal in {query_cases} cases" if args.queries else ""))
+          + (f"; query batches equal in {query_cases} cases" if args.queries else "")
+          + (f"; occlusion batches equal in {occlusion_cases} cases" if args.occlusion else ""))
     return 1 if bad else 0
 
 
