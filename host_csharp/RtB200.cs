@@ -66,6 +66,15 @@ public static class RtB200
     public struct RaySegment { public UnityEngine.Vector3 origin, dir; public float tMax; }
     [DllImport(Lib)] public static extern int rtTraceOcclusion(IntPtr ctx, RaySegment[] segs, int n, [Out] byte[] occluded, int flags);
     [DllImport(Lib)] public static extern int rtTraceOcclusionDevice(IntPtr ctx, IntPtr dSegs, IntPtr dOccluded, int n, int flags);
+    // radiance along caller rays: the path tracer's Trace (glass / diffuse / specular / emissive, sky, Russian roulette) from origin along
+    // dir (used as given), `samples` paths on the RNG chain that starts at rngState; out[i].rgb = their mean, out[i].rngState = the state
+    // after the last one.  Custom cameras (360 panoramas, cube maps, fisheye, stereo), light / reflection probe baking
+    [StructLayout(LayoutKind.Sequential)]
+    public struct PathRay { public UnityEngine.Vector3 origin, dir; public uint rngState; }
+    [StructLayout(LayoutKind.Sequential)]
+    public struct PathRadiance { public UnityEngine.Vector3 rgb; public uint rngState; }
+    [DllImport(Lib)] public static extern int rtTracePaths(IntPtr ctx, PathRay[] rays, int n, int samples, [Out] PathRadiance[] output);
+    [DllImport(Lib)] public static extern int rtTracePathsDevice(IntPtr ctx, IntPtr dRays, IntPtr dOut, int n, int samples);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

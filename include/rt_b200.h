@@ -153,6 +153,41 @@ int rtTraceRaysDevice(RtContext* ctx, const void* dRays, void* dHits, int n, int
 int rtTraceOcclusion(RtContext* ctx, const RtRaySegment* segs, int n, uint8_t* occluded, int flags);
 int rtTraceOcclusionDevice(RtContext* ctx, const void* dSegs, void* dOccluded, int n, int flags);
 
+/* Extension: the path tracer's radiance along caller-supplied rays (custom cameras: equirectangular, cube map, fisheye, stereo,
+ * orthographic; light-probe and irradiance-volume baking; reflection probes; what one path or direction contributes).  The reference's
+ * per-pixel sample loop (HL:560-581) with the caller's ray in place of the jittered camera ray, and no camera draws:
+ *     state = rays[i].rngState; total = (0, 0, 0)
+ *     for k in 0 .. samples - 1: total += Trace(CreateRay(origin, dir, transmittance 1, bounce 0), state)      (HL:578, in order)
+ *     out[i].rgb = total / (float)samples; out[i].rngState = state                                            (HL:581)
+ * Trace is HL:479-542 with its glass / diffuse / specular / emissive shading, the sky and Russian roulette; dir is used as given.
+ *   - Exactness: the oracle's bits.  A NaN appears exactly where the oracle has one (its payload is free).  forceDontCullBack is false,
+ *     as at HL:487, so the call takes no flags; material culling is the reference's.  With a camera ray and the state after its four
+ *     jitter draws (HL:565-572), samples = 1 returns that camera sample's Trace bit for bit: a pixel of rtDispatch is the float sum of
+ *     its R samples' results, in order, over (float)R.
+ *   - Reads the scene buffers, "modelCount", "MaxBounceCount", "UseSky", "SunFocus", "SunIntensity", "SunColour" and "dirToSun".  Reads
+ *     no camera, "Frame", "renderSeed", "NumRaysPerPixel" or "Resolution", and needs no rtResize.
+ *   - Leaves FrameRender, AccumulatedRender, PixelStats, "Frame", RtStats.dispatches and kernelMs alone and does not change what later
+ *     dispatches render.
+ *   - RtStats.rays grows by the number of CalculateRayCollision calls: one per path segment, as for the camera kernels (not by n).  With
+ *     "countStats" = 1 the box / triangle / sphere counters grow as a counting dispatch's do, walking every model.
+ *   - Model skipping, the TLAS and the sphere accelerator are used per SEGMENT under rtTraceRays' conditions: the segment's origin inside
+ *     the padded box and 2^-20 <= dot(dir, dir) <= 2^20.  The test applies to every bounce, not only the first: a bounce starts at a hit
+ *     point, and a first segment from a far origin or with an extreme direction length puts that point where the padding argument was
+ *     not made.  Any other segment walks every model and tests every sphere in buffer order.  Segments that may skip share the open
+ *     grazing-ray defect (DESIGN.md section 5) with the camera rays.
+ *   - On a group context (rtCreateMulti) the paths are traced on devices[0]; call it on the context rtCreateMulti returned.
+ *   - Throughput: one lane traces one ray's samples (one RNG chain), so a batch fills the GPU from about as many rays as the persistent
+ *     grid has lanes (132 SMs x 6 CTAs x 128 threads, about 101k on an H100 SXM); smaller batches leave it partly idle.
+ * Refused: ctx NULL, n < 0, rays / out NULL with n > 0, samples < 1 or > RT_MAX_BATCH_SAMPLES (the per-launch sample budget of a batch
+ * of frames), a device dRays not 4-byte or dOut not 16-byte aligned -> RT_E_INVALID; a member context of a group other than the one
+ * rtCreateMulti returned, the scene checks of rtDispatch, and "MaxBounceCount" outside 0 .. 200 (as rtDispatch) -> RT_E_STATE.  n = 0 is
+ * RT_OK and launches nothing.
+ * rtTracePaths: host arrays, in batches of at most RT_TRACE_CHUNK_RAYS through the two device buffers rtTraceRays keeps (rays in the
+ * hit buffer, 28 of its 48 bytes; results in the ray buffer, 16 of its 24); synchronises.  rtTracePathsDevice: n RtPathRay /
+ * RtPathRadiance in device memory of the context's device, no allocation; asynchronous on the context's stream (rtSetStream). */
+int rtTracePaths(RtContext* ctx, const RtPathRay* rays, int n, int samples, RtPathRadiance* out);
+int rtTracePathsDevice(RtContext* ctx, const void* dRays, void* dOut, int n, int samples);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),

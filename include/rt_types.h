@@ -101,6 +101,20 @@ typedef struct RtRaySegment {
     float tMax;
 } RtRaySegment;
 
+/* A caller-supplied path of rtTracePaths / rtTracePathsDevice (include/rt_b200.h): the first segment's world-space origin and
+ * direction, and the RNG state the path starts from. */
+typedef struct RtPathRay {
+    float    origin[3];
+    float    dir[3];       /* not normalised by the call: Trace uses it as given, as HL:479 does */
+    uint32_t rngState;     /* the RNG state the path starts from (HL:127-138) */
+} RtPathRay;
+
+/* The radiance along one RtPathRay: the mean of its samples, and the RNG state after the last one (16 bytes: one float4 store). */
+typedef struct RtPathRadiance {
+    float    rgb[3];
+    uint32_t rngState;     /* the state after the last sample: a caller continues the chain with it */
+} RtPathRadiance;
+
 #pragma pack(pop)
 
 #ifdef __cplusplus
@@ -109,6 +123,8 @@ static_assert(sizeof(RtPixelStats) == 20, "PixelStats record");
 static_assert(sizeof(RtRay) == 24, "RtRay record");
 static_assert(sizeof(RtRayHit) == 48, "RtRayHit record");
 static_assert(sizeof(RtRaySegment) == 28, "RtRaySegment record");
+static_assert(sizeof(RtPathRay) == 28, "RtPathRay record");
+static_assert(sizeof(RtPathRadiance) == 16, "RtPathRadiance record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

@@ -92,10 +92,11 @@ def build_oracle(force: bool = False) -> str:
     # source unchanged and wraps the entry points that reach the counters (tests/oracle_ext/rt_oracle_pixel_stats.cpp); rtDispatchFrames
     # is the loop over single-frame dispatches around that (tests/oracle_ext/rt_oracle_frames.cpp); rtTraceRays is CalculateRayCollision
     # per ray around that in turn (tests/oracle_ext/rt_oracle_trace_rays.cpp); rtTraceOcclusion is its tMax-bounded early-exit walk
-    # around that (tests/oracle_ext/rt_oracle_occlusion.cpp, the translation unit built here)
+    # around that (tests/oracle_ext/rt_oracle_occlusion.cpp); rtTracePaths is Shader::Trace per sample of a caller ray around that
+    # (tests/oracle_ext/rt_oracle_paths.cpp, the translation unit built here)
     srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(ORACLE_EXT, (".cpp",)) + _glob(INCLUDE, (".h",))
     if force or _newer(LIB_ORACLE, srcs):
-        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_occlusion.cpp")])
+        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_paths.cpp")])
     return LIB_ORACLE
 
 

@@ -93,6 +93,32 @@ def make_segments(origins, dirs=None, t_max=None) -> np.ndarray:
     return segs
 
 
+# rtTracePaths: a caller-supplied path start (RtPathRay) and the radiance along it (RtPathRadiance)
+PATH_RAY_DTYPE = np.dtype([("origin", "<f4", 3), ("dir", "<f4", 3), ("rngState", "<u4")])
+PATH_RADIANCE_DTYPE = np.dtype([("rgb", "<f4", 3), ("rngState", "<u4")])
+assert PATH_RAY_DTYPE.itemsize == 28 and PATH_RADIANCE_DTYPE.itemsize == 16
+
+
+def make_path_rays(origins, dirs=None, rng_state=None) -> np.ndarray:
+    """A PATH_RAY_DTYPE array from a structured array (returned as it is) or from (n, 3) origins, (n, 3) directions (used as given,
+    not normalised) and n uint32 RNG states (a scalar applies to every ray)."""
+    if dirs is None:
+        rays = np.asarray(origins)
+        if rays.dtype != PATH_RAY_DTYPE:
+            raise TypeError(f"path rays must have dtype {PATH_RAY_DTYPE} (or pass origins, dirs and rng_state)")
+        return np.ascontiguousarray(rays).reshape(-1)
+    if rng_state is None:
+        raise ValueError("rng_state is required with origins and dirs")
+    o = np.asarray(origins, dtype=np.float32).reshape(-1, 3)
+    d = np.asarray(dirs, dtype=np.float32).reshape(-1, 3)
+    if o.shape != d.shape:
+        raise ValueError("origins and dirs must both be (n, 3)")
+    rays = np.empty(o.shape[0], dtype=PATH_RAY_DTYPE)
+    rays["origin"], rays["dir"] = o, d
+    rays["rngState"] = np.broadcast_to(np.asarray(rng_state, dtype=np.uint64).astype(np.uint32).reshape(-1), (o.shape[0],))
+    return rays
+
+
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
                 ("dispatches", C.c_uint64), ("kernelMs", C.c_double), ("sphereBoxTests", C.c_uint64), ("exchangeMs", C.c_double)]
@@ -158,12 +184,14 @@ class RtLib:
             "rtTraceRaysDevice": ([vp, vp, vp, ci, ci], ci),
             "rtTraceOcclusion": ([vp, vp, ci, vp, ci], ci),
             "rtTraceOcclusionDevice": ([vp, vp, vp, ci, ci], ci),
+            "rtTracePaths": ([vp, vp, ci, ci, vp], ci),
+            "rtTracePathsDevice": ([vp, vp, vp, ci, ci], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
-                            "rtTraceOcclusion", "rtTraceOcclusionDevice"):      # absent from older experimental builds used in A/B runs
+                            "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -303,6 +331,19 @@ class RtContext:
         """rtTraceOcclusionDevice: n RtRaySegment at segs_ptr (4-byte aligned) -> n bytes (1 = occluded) at occluded_ptr, both device
         memory of the context's GPU (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtTraceOcclusionDevice(self._h, C.c_void_p(segs_ptr), C.c_void_p(occluded_ptr), int(n), RT_TRACE_NO_CULL if no_cull else 0))
+
+    def trace_paths(self, rays, samples: int = 1) -> np.ndarray:
+        """rtTracePaths: the path tracer's radiance along every ray (a PATH_RAY_DTYPE array, see make_path_rays), the mean of `samples`
+        paths on the ray's RNG chain.  Returns n PATH_RADIANCE_DTYPE records: rgb and the RNG state after the last sample."""
+        r = make_path_rays(rays)
+        out = np.empty(r.shape[0], dtype=PATH_RADIANCE_DTYPE)
+        self._ck(self._L.rtTracePaths(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), int(samples), out.ctypes.data if out.size else None))
+        return out
+
+    def trace_paths_device(self, rays_ptr: int, out_ptr: int, n: int, samples: int = 1):
+        """rtTracePathsDevice: n RtPathRay at rays_ptr (4-byte aligned) -> n RtPathRadiance at out_ptr (16-byte aligned), both device
+        memory of the context's GPU (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
+        self._ck(self._L.rtTracePathsDevice(self._h, C.c_void_p(rays_ptr), C.c_void_p(out_ptr), int(n), int(samples)))
 
     def readback(self, tex: str, out: Optional[np.ndarray] = None) -> np.ndarray:
         if out is None:

@@ -101,7 +101,8 @@ struct RtContext
     unsigned int* dWork = nullptr;
     DevBuf<RtPixelStats> pixelStats;           // "PixelStats": W*H per-pixel counters of the counting launches (allocated by the first one)
     DevBuf<RtRay> queryRays; DevBuf<RtRayHit> queryHits;     // rtTraceRays: device copies of one batch (<= RT_TRACE_CHUNK_RAYS) of the caller's host arrays
-                                                             // (rtTraceOcclusion: its segments in queryHits, its bytes in queryRays)
+                                                             // (rtTraceOcclusion: its segments in queryHits, its bytes in queryRays;
+                                                             //  rtTracePaths: its RtPathRay in queryHits, its RtPathRadiance in queryRays)
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -1156,6 +1157,72 @@ int rtTraceOcclusionDevice(RtContext* c, const void* dSegs, void* dOccluded, int
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     return occlusionLocal(c, (const RtRaySegment*)dSegs, (unsigned char*)dOccluded, n, flags);
+}
+
+// ---- radiance along caller-supplied rays (rtTracePaths, k_trace_paths in rt_kernel_query.cuh) ------------------------------------------
+static int pathArgs(RtContext* c, const char* what, const void* rays, const void* out, int n, int samples)
+{
+    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; trace on the context rtCreateMulti returned");
+    if (n < 0 || (n > 0 && (!rays || !out))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or rays / out NULL)");
+    if (samples < 1 || samples > RT_MAX_BATCH_SAMPLES) return fail(c, RT_E_INVALID, std::string(what) + ": samples must be 1 .. RT_MAX_BATCH_SAMPLES");
+    return RT_OK;
+}
+
+// n rays in device memory of this context's GPU -> n radiances; asynchronous on the context's stream.  RtStats.rays grows by the
+// segments traced, through the kernel's counters; no timing events, so dispatches / kernelMs stay the camera kernels'.
+static int pathsLocal(RtContext* c, const RtPathRay* dRays, RtPathRadiance* dOut, int n, int samples)
+{
+    // a kernel-1-style loop traces one segment even with a negative bound, where the reference's loop (HL:484) traces none
+    if (c->P.MaxBounceCount < 0 || c->P.MaxBounceCount > 200) return fail(c, RT_E_STATE, "rtTracePaths: MaxBounceCount must be 0 .. 200 (as rtDispatch)");
+    int rc = prepareQueryScene(c, "rtTracePaths"); if (rc != RT_OK) return rc;
+    DevParams P = c->P;
+    bindScene(c, P);
+    P.countStats = c->optCountStats;
+    P.smemPairs = 0;                                 // no tree-top staging: every record from global memory
+    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    PathParams Q = {};
+    Q.rays = dRays; Q.out = dOut; Q.n = (unsigned int)n; Q.samples = samples;
+    for (int a = 0; a < 3; a++)
+    {
+        Q.modelLo[a] = c->repack.modelBoundLo[a]; Q.modelHi[a] = c->repack.modelBoundHi[a];
+        Q.sphLo[a] = c->repack.sphBoundLo[a]; Q.sphHi[a] = c->repack.sphBoundHi[a];
+    }
+    cudaError_t e = paths_launch(P, Q, c->numSMs, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "rtTracePaths launch");
+    return RT_OK;
+}
+
+// The rays travel in queryHits (28 of its 48 bytes per record) and the results in queryRays (16 of 24), so a path batch needs no
+// memory beyond what a closest-hit batch of the same size keeps.
+int rtTracePaths(RtContext* c, const RtPathRay* rays, int n, int samples, RtPathRadiance* out)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = pathArgs(c, "rtTracePaths", rays, out, n, samples); if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
+    if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
+    RtPathRay* dRays = reinterpret_cast<RtPathRay*>(c->queryHits.p);
+    RtPathRadiance* dOut = reinterpret_cast<RtPathRadiance*>(c->queryRays.p);
+    for (int i0 = 0; i0 < n; i0 += chunk)
+    {
+        const int m = n - i0 < chunk ? n - i0 : chunk;
+        if ((rc = stagedH2D(c, dRays, rays + i0, (size_t)m * sizeof(RtPathRay))) != RT_OK) return rc;
+        if ((rc = pathsLocal(c, dRays, dOut, m, samples)) != RT_OK) return rc;
+        if ((rc = stagedD2H(c, out + i0, dOut, (size_t)m * sizeof(RtPathRadiance))) != RT_OK) return rc;
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rtTracePathsDevice(RtContext* c, const void* dRays, void* dOut, int n, int samples)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = pathArgs(c, "rtTracePathsDevice", dRays, dOut, n, samples); if (rc != RT_OK) return rc;
+    if (((uintptr_t)dRays & 3u) || ((uintptr_t)dOut & 15u)) return fail(c, RT_E_INVALID, "rtTracePathsDevice: dRays must be 4-byte and dOut 16-byte aligned");
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    return pathsLocal(c, (const RtPathRay*)dRays, (RtPathRadiance*)dOut, n, samples);
 }
 
 int rtExchangeTiles(RtContext* c)

@@ -31,6 +31,7 @@ std::string RtApi::Load(const char* path)
     DispatchFrames = reinterpret_cast<decltype(DispatchFrames)>(dlsym(dl, "rtDispatchFrames"));
     TraceRays = reinterpret_cast<decltype(TraceRays)>(dlsym(dl, "rtTraceRays"));
     TraceOcclusion = reinterpret_cast<decltype(TraceOcclusion)>(dlsym(dl, "rtTraceOcclusion"));
+    TracePaths = reinterpret_cast<decltype(TracePaths)>(dlsym(dl, "rtTracePaths"));
     return "";
 }
 
@@ -310,6 +311,16 @@ int RayComputeManager::TraceOcclusion(const RtRaySegment* segs, int n, uint8_t* 
     int rc;
     if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
     TRY(api.TraceOcclusion(ctx, segs, n, occluded, flags));
+    return RT_OK;
+}
+
+int RayComputeManager::TracePaths(const RtPathRay* rays, int n, int samples, RtPathRadiance* out)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.TracePaths) { lastError = "the library does not export rtTracePaths"; return RT_E_STATE; }
+    int rc;
+    if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
+    TRY(api.TracePaths(ctx, rays, n, samples, out));
     return RT_OK;
 }
 

@@ -59,6 +59,7 @@ struct RtApi
     decltype(&rtDispatchFrames) DispatchFrames = nullptr;   // optional: several accumulated frames in one launch (RenderFrames)
     decltype(&rtTraceRays) TraceRays = nullptr;             // optional: closest-hit queries (TraceRays / Pick)
     decltype(&rtTraceOcclusion) TraceOcclusion = nullptr;   // optional: occlusion queries (TraceOcclusion)
+    decltype(&rtTracePaths) TracePaths = nullptr;           // optional: radiance along caller rays (TracePaths)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -133,6 +134,9 @@ public:
     // not in the reference: whether anything lies on caller-supplied segments (rtTraceOcclusion; occluded[i] = 1 or 0) — shadow rays,
     // ambient occlusion, line of sight.  The scene is uploaded first as for TraceRays.
     int TraceOcclusion(const RtRaySegment* segs, int n, uint8_t* occluded, int flags = 0);
+    // not in the reference: the path tracer's radiance along caller-supplied rays, the mean of `samples` paths on each ray's RNG chain
+    // (rtTracePaths) — custom cameras, probe baking.  The scene is uploaded first as for TraceRays.
+    int TracePaths(const RtPathRay* rays, int n, int samples, RtPathRadiance* out);
     // picking / autofocus: the un-jittered camera ray through pixel (x, y) of the screen — SetupPixel's operations (HL:547-558) on the
     // manager's own camera fields — and its closest hit
     void PickRay(float x, float y, RtRay* ray) const;

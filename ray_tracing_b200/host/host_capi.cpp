@@ -239,6 +239,9 @@ int rcmTraceRays(void* hv, const RtRay* rays, int n, RtRayHit* hits, int flags)
 
 int rcmTraceOcclusion(void* hv, const RtRaySegment* segs, int n, uint8_t* occluded, int flags)
 { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TraceOcclusion(segs, n, occluded, flags); } CATCH_ALL(h) }
+
+int rcmTracePaths(void* hv, const RtPathRay* rays, int n, int samples, RtPathRadiance* out)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TracePaths(rays, n, samples, out); } CATCH_ALL(h) }
 /* the pick ray through pixel (x, y) into *ray (may be NULL) and its closest hit into *hit (may be NULL: the ray alone) */
 int rcmPick(void* hv, float x, float y, RtRay* ray, RtRayHit* hit)
 {

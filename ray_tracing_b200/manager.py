@@ -65,6 +65,7 @@ def host_lib() -> C.CDLL:
         L.rcmDisplayDebugView.argtypes = [vp, ci, cf, vp, C.c_size_t]
         L.rcmTraceRays.argtypes = [vp, vp, ci, vp, ci]
         L.rcmTraceOcclusion.argtypes = [vp, vp, ci, vp, ci]
+        L.rcmTracePaths.argtypes = [vp, vp, ci, ci, vp]
         L.rcmPick.argtypes = [vp, cf, cf, vp, vp]
         _host = L
     return _host
@@ -296,6 +297,16 @@ class RayComputeManager:
         self._ck(self._L.rcmTraceOcclusion(self._h, s.ctypes.data if s.size else None, int(s.shape[0]), occ.ctypes.data if occ.size else None,
                                            capi.RT_TRACE_NO_CULL if no_cull else 0))
         return occ.view(np.bool_)
+
+    # -- radiance along caller rays (rtTracePaths): custom cameras, probe baking
+    def trace_paths(self, rays, samples: int = 1) -> np.ndarray:
+        """The path tracer's radiance along each ray (a capi.PATH_RAY_DTYPE array, see capi.make_path_rays), the mean of `samples`
+        paths, as n capi.PATH_RADIANCE_DTYPE records.  The scene is uploaded as a frame would upload it; the render textures are not
+        touched."""
+        r = capi.make_path_rays(rays)
+        out = np.empty(r.shape[0], dtype=capi.PATH_RADIANCE_DTYPE)
+        self._ck(self._L.rcmTracePaths(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), int(samples), out.ctypes.data if out.size else None))
+        return out
 
     def pick_ray(self, x: float, y: float) -> np.ndarray:
         """The un-jittered camera ray through pixel (x, y) (row 0 = bottom), as one capi.RAY_DTYPE record."""

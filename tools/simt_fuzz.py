@@ -4,7 +4,7 @@ emissive materials, sky, defocus, near / far / inside cameras, extreme scales) r
 interpreter build (tests/simt) with random options, compared bit for bit with the oracle.  Found the distant-camera defect of the
 model skipping in round 1 by hand-made cases; this keeps looking.  Every failure prints the seed that reproduces it.
 
-    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats] [--queries] [--occlusion]
+    python tools/simt_fuzz.py [--cases 200] [--seed 1] [--lib path/to/another/build.so] [--pixel-stats] [--queries] [--occlusion] [--paths]
 
 --pixel-stats: wherever the traversal totals are compared (counting launches of whole images), also compare the per-pixel counters
 (PixelStats: rays, box and triangle tests everywhere; sphere tests too when the Spheres buffer is below the accelerator's threshold).
@@ -16,6 +16,10 @@ with the oracle (a NaN must be a NaN on both sides), and with "countStats" the c
 --occlusion: every scene also traces a random batch of segments (rtTraceOcclusion): the rays of --queries with tMax at, one ulp below
 and one ulp above the oracle's closest hit, fractions of it, +inf and special values (tests/test_gpu_occlusion.py tmax_sets), with
 either flag, compared with the oracle's answers, and with "countStats" the early-exit counters the batch added.
+
+--paths: every scene also traces a random batch of path rays (rtTracePaths): the rays of --queries with random RNG states
+(tests/test_gpu_trace_paths.py path_rays) and a random sample count, under the scene's random MaxBounceCount / UseSky / sun, compared
+bit for bit with the oracle in rgb and final state, and the segments (RtStats.rays) and, with "countStats", the counters the batch added.
 """
 import argparse
 import os
@@ -34,6 +38,7 @@ import ray_tracing_b200 as rt                   # noqa: E402
 from ray_tracing_b200 import scenes             # noqa: E402
 from test_gpu_trace_rays import assert_hits_equal, ray_sets      # noqa: E402  (the query batch of the rtTraceRays tests)
 from test_gpu_occlusion import assert_occlusion_equal, tmax_sets  # noqa: E402  (the segment lengths of the rtTraceOcclusion tests)
+from test_gpu_trace_paths import assert_radiance_equal, path_rays  # noqa: E402  (the path rays of the rtTracePaths tests)
 
 
 def render_pixel_stats(lib, sc, frames, options, tile=None):
@@ -54,7 +59,7 @@ def render_pixel_stats(lib, sc, frames, options, tile=None):
     return out
 
 
-def trace_batch(lib, sc, options, rays, no_cull, occlusion=False):
+def trace_batch(lib, sc, options, rays, no_cull, occlusion=False, samples=0):
     """rtTraceRays of `rays` (occlusion: rtTraceOcclusion of segments) on a fresh context of the scene (after OnEnable), with the
     RtStats counters the batch added."""
     mgr = rt.RayComputeManager(lib)
@@ -64,7 +69,10 @@ def trace_batch(lib, sc, options, rays, no_cull, occlusion=False):
         ctx.set_option(k, v)
     mgr.OnEnable()
     ctx.reset_stats()
-    hits = ctx.trace_occlusion(rays, no_cull=no_cull) if occlusion else ctx.trace_rays(rays, no_cull=no_cull)
+    if samples:                                  # rtTracePaths of path rays
+        hits = ctx.trace_paths(rays, samples)
+    else:
+        hits = ctx.trace_occlusion(rays, no_cull=no_cull) if occlusion else ctx.trace_rays(rays, no_cull=no_cull)
     out = (hits, ctx.stats())
     mgr.OnDestroy()
     return out
@@ -221,9 +229,10 @@ def main():
     ap.add_argument("--queries", action="store_true", help="also trace a random batch of rays through every scene (rtTraceRays) against the oracle")
     ap.add_argument("--query-rays", type=int, default=32, help="rays per kind in a --queries batch")
     ap.add_argument("--occlusion", action="store_true", help="also trace a random batch of segments through every scene (rtTraceOcclusion) against the oracle")
+    ap.add_argument("--paths", action="store_true", help="also trace a random batch of path rays through every scene (rtTracePaths) against the oracle")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
-    bad, pix_cases, query_cases, occlusion_cases, t0 = 0, 0, 0, 0, time.time()
+    bad, pix_cases, query_cases, occlusion_cases, path_cases, t0 = 0, 0, 0, 0, 0, time.time()
     for case in range(args.cases):
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
@@ -291,11 +300,27 @@ def main():
             except Exception as e:
                 bad += 1
                 print(f"case seed {seed}: occlusion: {type(e).__name__}: {e}   options {o_opts}, no_cull {no_cull}, {len(sc.models)} models, {len(sc.spheres)} spheres", flush=True)
+        if args.paths:
+            prng = np.random.RandomState(seed + 11)
+            rays = path_rays(sc, seed=seed + 11, n=args.query_rays)
+            samples = int(prng.choice([1, 2, 3, 7]))
+            p_opts = {k: v for k, v in opts.items() if k in ("tlas", "modelSkip", "extInstantiation", "countStats", "smemNodes", "pairOrder")}
+            try:
+                want, so = trace_batch(ORACLE_LIB, sc, {}, rays, False, samples=samples)
+                got, sg = trace_batch(lib, sc, p_opts, rays, False, samples=samples)
+                assert_radiance_equal(got, want, "rtTracePaths")
+                keys = ("rays",) + (("boxTests", "triTests") + (("sphereTests",) if len(sc.spheres) <= 64 else ()) if p_opts.get("countStats") else ())
+                assert all(sg[k] == so[k] for k in keys), f"counters {sg} vs {so}"
+                path_cases += 1
+            except Exception as e:
+                bad += 1
+                print(f"case seed {seed}: paths: {type(e).__name__}: {e}   options {p_opts}, samples {samples}, {len(sc.models)} models, {len(sc.spheres)} spheres", flush=True)
         if (case + 1) % 25 == 0:
             print(f"  {case + 1} cases, {bad} findings, {time.time() - t0:.0f} s", flush=True)
     print(f"{args.cases} cases, {bad} findings" + (f"; PixelStats compared in {pix_cases} cases" if args.pixel_stats else "")
           + (f"; query batches equal in {query_cases} cases" if args.queries else "")
-          + (f"; occlusion batches equal in {occlusion_cases} cases" if args.occlusion else ""))
+          + (f"; occlusion batches equal in {occlusion_cases} cases" if args.occlusion else "")
+          + (f"; path batches equal in {path_cases} cases" if args.paths else ""))
     return 1 if bad else 0
 
 
