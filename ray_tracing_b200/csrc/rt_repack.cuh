@@ -440,6 +440,11 @@ struct RepackState
 
     // Host only (no CUDA call).  A model with a singular worldToLocal carries an infinite box (buildModels); it
     // makes every TLAS box above it infinite, so it is always marked — conservative, like the linear test.
+    // A TLAS box must reject a ray only where WorldBoxOutOfReach also rejects each model box below it.  Two kinds of box break the
+    // plain union (buildModels never makes either, its padding is positive and finite): a flat box, whose slab WorldBoxOutOfReach
+    // ignores for a ray lying in its plane (both slab distances 0 x inf = NaN), and a NaN bound, which leaves that slab to the other
+    // bound alone or, for a ray in that bound's plane, ignores it.  The tree sees a flat box one ulp wider on each side and an axis with
+    // a NaN bound as unbounded.
     static void planTlas(const std::vector<DevModel>& dm, int modelCount, std::vector<NodePair>& pairsOut, std::vector<int>& order, int& rootStart, int& rootCount)
     {
         const size_t n = (size_t)modelCount;
@@ -449,7 +454,10 @@ struct RepackState
             const float bmin[3] = {dm[i].wmin[0], dm[i].wmin[1], dm[i].wmin[2]}, bmax[3] = {dm[i].wmaxx, dm[i].wmaxy, dm[i].wmaxz};
             for (int a = 0; a < 3; a++)
             {
-                lo[3 * i + a] = bmin[a]; hi[3 * i + a] = bmax[a];
+                float l = bmin[a], h = bmax[a];
+                if (std::isnan(l) || std::isnan(h)) { l = -INFINITY; h = INFINITY; }
+                else if (l == h && std::isfinite(l)) { l = std::nextafterf(l, -INFINITY); h = std::nextafterf(h, INFINITY); }
+                lo[3 * i + a] = l; hi[3 * i + a] = h;
                 const float c = 0.5f * bmin[a] + 0.5f * bmax[a];
                 cen[3 * i + a] = std::isfinite(c) ? c : 0.0f;
             }

@@ -50,6 +50,16 @@ class Lib:
                                         C.c_void_p(padded.ctypes.data), C.c_size_t(len(w)))
         return exact, padded, placed
 
+    def tlas_check(self, boxes, rays):
+        """TlasCollect over the TLAS planTlas builds for the (n, 6) model boxes, for (m, 7) rays (pos, dir, bestDst): (m, 3) int32 rows
+        (models WorldBoxOutOfReach keeps on their own box, how many of those the TLAS mask lacks, the first of them or -1)."""
+        b, r = np.ascontiguousarray(boxes, dtype=np.float32), np.ascontiguousarray(rays, dtype=np.float32)
+        out = np.empty((len(r), 3), dtype=np.int32)
+        self.lib.rtpTlasCheck.restype = C.c_int
+        rc = self.lib.rtpTlasCheck(C.c_void_p(b.ctypes.data), C.c_int(len(b)), C.c_void_p(r.ctypes.data), C.c_size_t(len(r)), C.c_void_p(out.ctypes.data))
+        assert rc == 0, f"rtpTlasCheck returned {rc}"
+        return out
+
     def run(self, name, cases=None, n=None, base=0, stride=1, partner=0, arrays=True):
         """cases: (n, nin) uint32, or None for index mode over n cases.  Returns (outputs (n, nout) uint32 or None, digest (nout,))."""
         code, nin, nout, fmask = FN[name]
@@ -315,6 +325,108 @@ def sphere_cases(rng, n):
     return rec.view(np.uint32), cls
 
 
+def sphere_gate_cases(rng, n, lengths=None):
+    """sphere_cases over the query gate's domain: pos, dir, centre, radius and an origin box (n, 6) that holds the ray origin and the
+    sphere.  Classes: 0 aimed at a point inside the sphere from up to 8 units away; 1 near-tangent, as sphere_cases; 2 from the surface
+    (up to rounding) in any direction, as a bounce leaves it; 3 from anywhere in a box that holds the sphere and a point up to 1e5
+    away, aimed at a point inside the sphere.  Direction lengths log-uniform over the gate's [2^-10, 2^10] with both bounds
+    (gate_lengths), or `lengths` (n,)."""
+    cen = rng.standard_normal((n, 3)) * 4.0
+    r = np.abs(rng.standard_normal(n)) + 0.05
+    pos = rng.standard_normal((n, 3)) * 8.0
+    aim = cen + _unit(rng, n) * (r * rng.random(n))[:, None]
+    cls = rng.integers(0, 4, n)
+    far = cen + _unit(rng, n) * (10.0 ** rng.uniform(0, 5, n))[:, None]
+    lo, hi = np.minimum(far, cen - r[:, None]), np.maximum(far, cen + r[:, None])
+    s = np.flatnonzero(cls == 3)
+    pos[s] = lo[s] + rng.random((len(s), 3)) * (hi[s] - lo[s])
+    d = aim - pos
+    s = np.flatnonzero(cls == 1)                                   # tangent: offset perpendicular to dir by r (1 + {0, +-1e-7, 1e-6})
+    u = _unit(rng, len(s)).astype(np.float64)
+    perp = np.cross(u, _unit(rng, len(s)))
+    perp /= np.linalg.norm(perp, axis=1, keepdims=True)
+    pos[s] = cen[s] + perp * (r[s] * (1.0 + rng.choice(np.array([0.0, 1e-7, -1e-7, 1e-6]), len(s))))[:, None] - u * 3.0
+    d[s] = u
+    s = np.flatnonzero(cls == 2)                                   # on the surface, any direction
+    pos[s] = cen[s] + _unit(rng, len(s)) * r[s][:, None]
+    d[s] = rng.standard_normal((len(s), 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    d *= (gate_lengths(rng, n) if lengths is None else np.asarray(lengths, dtype=np.float64))[:, None]
+    pos32, c32, r32 = pos.astype(np.float32), cen.astype(np.float32), r.astype(np.float32)
+    origin = np.concatenate([np.minimum(np.minimum(lo, pos32), c32 - r32[:, None]), np.maximum(np.maximum(hi, pos32), c32 + r32[:, None])], axis=1)
+    rec = np.concatenate([pos32, d.astype(np.float32), c32, r32[:, None]], axis=1)
+    return rec.view(np.uint32), cls, origin.astype(np.float32)
+
+
+TLAS_SIZES = (1, 2, 4, 5, 17, 129, 4096)
+
+
+def tlas_boxes(rng, n):
+    """n padded model boxes (n, 6: min xyz, max xyz) as planTlas receives them.  Classes: generic boxes scattered over 10 .. 1e4
+    units; cells of a grid, which share faces exactly; flat boxes (min = max on an axis); bounds at +-0; a NaN bound; the infinite
+    box of a model worldBoxOfModel cannot place."""
+    spread = 10.0 ** rng.uniform(1, 4)
+    c = rng.uniform(-1, 1, (n, 3)) * spread
+    h = np.exp(rng.uniform(np.log(1e-4), np.log(0.3), (n, 3))) * spread
+    lo, hi = c - h, c + h
+    cls = rng.integers(0, 6, n)
+    s = np.flatnonzero(cls == 1)                                    # grid cells: neighbours share a face
+    cell = spread / 8
+    g = rng.integers(-4, 4, (len(s), 3)).astype(np.float64)
+    lo[s], hi[s] = g * cell, (g + rng.integers(1, 3, (len(s), 3))) * cell
+    s = np.flatnonzero(cls == 2)                                    # flat on one axis
+    ax = rng.integers(0, 3, len(s))
+    hi[s, ax] = lo[s, ax]
+    s = np.flatnonzero(cls == 3)                                    # a bound at +-0
+    ax = rng.integers(0, 3, len(s))
+    lo[s, ax] = np.minimum(lo[s, ax], -1.0)
+    hi[s, ax] = np.where(rng.random(len(s)) < 0.5, 0.0, -0.0)
+    flip = rng.random(len(s)) < 0.5
+    lo[s[flip], ax[flip]] = np.where(rng.random(int(flip.sum())) < 0.5, 0.0, -0.0)
+    hi[s[flip], ax[flip]] = np.abs(hi[s[flip], ax[flip]]) + 1.0
+    box = np.concatenate([lo, hi], axis=1).astype(np.float32)
+    s = np.flatnonzero(cls == 4)                                    # a NaN bound
+    box[s, rng.integers(0, 6, len(s))] = np.nan
+    s = np.flatnonzero((cls == 5) & (rng.random(n) < 0.1))          # the infinite box of a singular model (rare: it marks every ray)
+    box[s, :3], box[s, 3:] = -np.inf, np.inf
+    return box
+
+
+def tlas_rays(rng, boxes, m):
+    """(m, 7) rays pos, dir, bestDst against `boxes`.  Directions: generic, axis-aligned (+-0 components, invDir = +-inf), lengths over
+    the query gate's range.  Origins: anywhere around the boxes, on a slab plane of some box (with the direction parallel to it: 0 x inf),
+    at a box corner.  bestDst: +inf, the distance to some box's corner, 0, -0, a tiny or huge value, NaN."""
+    fin = np.where(np.isfinite(boxes), boxes, 0.0).astype(np.float64)
+    span = max(float(np.abs(fin).max()), 1.0)
+    pos = rng.uniform(-1.2, 1.2, (m, 3)) * span
+    d = rng.standard_normal((m, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    d *= gate_lengths(rng, m)[:, None]
+    d = d.astype(np.float32)
+    cls = rng.integers(0, 4, m)
+    pick = rng.integers(0, len(boxes), m)
+    s = np.flatnonzero(cls == 1)
+    d[s] = _axis_aligned(rng, d[s])
+    s = np.flatnonzero(cls == 2)                                    # on a slab plane of a box or one ulp inside it, parallel to it
+    ax = rng.integers(0, 3, len(s))
+    side = rng.integers(0, 2, len(s))
+    face = fin[pick[s], ax + 3 * side].astype(np.float32)
+    inward = np.where(side == 0, np.float32(np.inf), np.float32(-np.inf))
+    pos[s, ax] = np.where(rng.random(len(s)) < 0.5, face, np.nextafter(face, inward))
+    d[s, ax] = np.where(rng.random(len(s)) < 0.5, np.float32(0.0), np.float32(-0.0))
+    s = np.flatnonzero(cls == 3)                                    # at a corner, axis-aligned half of the time
+    pos[s] = np.where(rng.random((len(s), 3)) < 0.5, fin[pick[s], :3], fin[pick[s], 3:])
+    half = s[rng.random(len(s)) < 0.5]
+    d[half] = _axis_aligned(rng, d[half])
+    corner = np.where(rng.random((m, 3)) < 0.5, fin[pick, :3], fin[pick, 3:])
+    best = (np.linalg.norm(corner - pos, axis=1) / np.maximum(np.linalg.norm(d.astype(np.float64), axis=1), 1e-30)).astype(np.float32)
+    kind = rng.random(m)
+    best = np.where(kind < 0.3, np.float32(np.inf), best)
+    special = np.array([0.0, -0.0, 1e-30, 1e-6, 3.4028235e38, np.nan], dtype=np.float32)
+    best = np.where(kind > 0.85, rng.choice(special, m), best).astype(np.float32)
+    return np.concatenate([pos.astype(np.float32), d, best[:, None]], axis=1)
+
+
 def shading_cases(rng, n):
     """inDir, normal, iorA, iorB.  Classes: generic glass (one ior 1, the other in [1, 2.5]); total internal reflection at sinSqr == 1
     exactly (grazing incidence with equal iors) and around it; ior in {0, 1, negative}; special values anywhere."""
@@ -387,15 +499,50 @@ def model_cases(rng, n):
     the triangle's interior, at its edges and vertices (weights 0 or +-1e-7) and just outside (weight -1e-5).
     Returns (worldToLocal column-major (n, 16) float32, triangle (n, 9) local A B C, geometry box (n, 6), ray pos (n, 3), dir (n, 3),
     origin box (n, 6), cull (n,))."""
-    def rot(k):
-        q = rng.standard_normal((k, 4))
-        q /= np.linalg.norm(q, axis=1, keepdims=True)
-        w, x, y, z = q.T
-        return np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                         2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                         2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], axis=1).reshape(k, 3, 3)
     scale = rng.uniform(0.3, 3.0, (n, 3)) * np.where(rng.random((n, 3)) < 0.1, -1.0, 1.0)
-    A = rot(n) @ (scale[:, :, None] * rot(n))                      # x_local = A x_world + t
+    A = _rotations(rng, n) @ (scale[:, :, None] * _rotations(rng, n))         # x_local = A x_world + t
+    return _model_records(rng, n, A)
+
+
+def _rotations(rng, k):
+    q = rng.standard_normal((k, 4))
+    q /= np.linalg.norm(q, axis=1, keepdims=True)
+    w, x, y, z = q.T
+    return np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                     2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                     2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], axis=1).reshape(k, 3, 3)
+
+
+# the query gate of rt_kernel_query.cuh: model skipping, the TLAS and the sphere accelerator are used for 2^-20 <= dot(dir, dir) <= 2^20
+GATE_LEN_MIN, GATE_LEN_MAX = 2.0 ** -10, 2.0 ** 10
+
+
+def gate_lengths(rng, n, lo=GATE_LEN_MIN, hi=GATE_LEN_MAX):
+    """Direction lengths log-uniform over [lo, hi], the bounds themselves in a tenth of the cases."""
+    L = np.exp(rng.uniform(np.log(lo), np.log(hi), n))
+    edge = rng.random(n)
+    return np.where(edge < 0.05, lo, np.where(edge < 0.1, hi, L))
+
+
+def model_gate_cases(rng, n, lengths=None):
+    """model_cases over the query gate's domain.  worldToLocal: rotation x scale x rotation with singular values log-uniform in
+    1e-3 .. 1e3 (class bit 0 clear), or the product of two rotation x scale pairs (a rotated child of a non-uniformly scaled parent:
+    sheared, singular values spread over about the same range; bit 0 set).  Rays (class >> 1): 0 from up to 1e5 away aimed at the
+    triangle, as model_cases; 1 from anywhere in an origin box that holds the geometry and a point up to 1e5 away, aimed at the
+    triangle; 2 from a point of the triangle itself in any direction, as a bounce leaves a surface.  Direction lengths log-uniform
+    over the gate's [2^-10, 2^10] with both bounds (gate_lengths), or `lengths` (n,).  Returns model_cases' tuple and the class."""
+    shear = rng.random(n) < 0.5
+    s1 = np.exp(rng.uniform(np.log(1e-3), np.log(1e3), (n, 3))) * np.where(rng.random((n, 3)) < 0.1, -1.0, 1.0)
+    A = _rotations(rng, n) @ (s1[:, :, None] * _rotations(rng, n))
+    s2 = np.exp(rng.uniform(np.log(10 ** -1.5), np.log(10 ** 1.5), (n, 2, 3)))
+    B = (s2[:, 0, :, None] * _rotations(rng, n)) @ (s2[:, 1, :, None] * _rotations(rng, n))
+    A[shear] = B[shear]
+    origin_cls = rng.integers(0, 3, n)
+    L = gate_lengths(rng, n) if lengths is None else np.asarray(lengths, dtype=np.float64)
+    return _model_records(rng, n, A, origin_cls, L) + (shear.astype(int) + 2 * origin_cls,)
+
+
+def _model_records(rng, n, A, origin_cls=None, L=None):
     size = 10.0 ** rng.uniform(-3, 2, n)
     centre_local = rng.standard_normal((n, 3)) * size[:, None] * rng.uniform(0, 3, (n, 1))
     tri = centre_local[:, None, :] + rng.standard_normal((n, 3, 3)) * size[:, None, None]
@@ -420,11 +567,23 @@ def model_cases(rng, n):
     d /= np.linalg.norm(d, axis=1, keepdims=True)
     dist = 10.0 ** rng.uniform(-1, 5, n)
     pos = (target - d * dist[:, None]).astype(np.float32)
-    d = d.astype(np.float32)
-    geo = np.concatenate([tri.min(axis=1), tri.max(axis=1)], axis=1).astype(np.float32)
     world_tri = np.linalg.solve(A32[:, None], (tri - t32[:, None, :])[..., None])[..., 0]        # the vertices in world space
     lo = np.minimum(pos.astype(np.float64), world_tri.min(axis=1))                               # origin box: camera and geometry
     hi = np.maximum(pos.astype(np.float64), world_tri.max(axis=1))
+    if origin_cls is not None:
+        s = np.flatnonzero(origin_cls == 1)                         # anywhere in the origin box, aimed at the target
+        p = lo[s] + rng.random((len(s), 3)) * (hi[s] - lo[s])
+        pos[s] = p.astype(np.float32)
+        d[s] = target[s] - pos[s]
+        s = np.flatnonzero(origin_cls == 2)                         # on the triangle, any direction
+        w = rng.dirichlet((1.0, 1.0, 1.0), len(s))
+        pos[s] = np.einsum("nk,nkj->nj", w, world_tri[s]).astype(np.float32)
+        d[s] = rng.standard_normal((len(s), 3))
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+        d *= L[:, None]
+        lo, hi = np.minimum(lo, pos.astype(np.float64)), np.maximum(hi, pos.astype(np.float64))
+    d = d.astype(np.float32)
+    geo = np.concatenate([tri.min(axis=1), tri.max(axis=1)], axis=1).astype(np.float32)
     origin = np.concatenate([lo, hi], axis=1).astype(np.float32)
     cull = (rng.random(n) < 0.5).astype(np.uint32)
     return w2l.transpose(0, 2, 1).reshape(n, 16), tri.reshape(n, 9).astype(np.float32), geo, pos, d, origin, cull

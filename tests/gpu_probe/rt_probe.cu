@@ -182,6 +182,29 @@ __global__ void k_probe(int fn, int nin, int nout, const uint32_t* __restrict__ 
     if (digest) for (int j = 0; j < nout; j++) atomicAdd(digest + j, h[j]);
 }
 
+// One ray per thread against the TLAS in P (planned over `boxes`): TlasCollect as the kernels call it (rayInv = rcp3(dir)), then
+// WorldBoxOutOfReach on every model's own box at the same bestDst.  out[3i .. 3i + 2]: the models their own box keeps, how many of
+// those the TLAS mask lacks, the first of them (-1 when none).
+__global__ void k_tlas_check(DevParams P, const float* __restrict__ boxes, const float* __restrict__ rays, size_t n, int* __restrict__ out)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    {
+        const float* r = rays + 7 * i;
+        const f3 pos = make_f3(r[0], r[1], r[2]), inv = rcp3(make_f3(r[3], r[4], r[5]));
+        unsigned int mask[RT_TLAS_WORDS];
+        TlasCollect(P, pos, inv, r[6], mask);
+        int kept = 0, lost = 0, first = -1;
+        for (int m = 0; m < P.modelCount; m++)
+        {
+            const float* b = boxes + 6 * m;
+            if (WorldBoxOutOfReach(make_f3(b[0], b[1], b[2]), make_f3(b[3], b[4], b[5]), pos, inv, r[6])) continue;
+            kept++;
+            if (!((mask[m >> 5] >> (m & 31)) & 1u)) { lost++; if (first < 0) first = m; }
+        }
+        out[3 * i] = kept; out[3 * i + 1] = lost; out[3 * i + 2] = first;
+    }
+}
+
 template <class T> struct DevBuf
 {
     T* p = nullptr;
@@ -283,6 +306,44 @@ int rtpModelBoxes(const float* worldToLocal, const float* geo, const float* orig
         placedCount += placed ? 1 : 0;
     }
     return placedCount;
+}
+
+// The TLAS over n model world boxes (boxes[6m..6m+5]: min xyz, max xyz, as DevModel holds them), planned by the host's
+// RepackState::planTlas (the tree rtxPlanTlas exposes), walked on the device by TlasCollect for each of the nrays rays (rays[7i..]:
+// pos, dir, bestDst); see k_tlas_check for out.  Returns 0, 1 for n outside 1 .. RT_TLAS_MAX_MODELS, 2 for a CUDA error (printed).
+int rtpTlasCheck(const float* boxes, int n, const float* rays, size_t nrays, int* out)
+{
+    if (n < 1 || n > RT_TLAS_MAX_MODELS) return 1;
+    std::vector<DevModel> dm((size_t)n);
+    for (int i = 0; i < n; i++)
+    {
+        memset(&dm[i], 0, sizeof(DevModel));
+        const float* b = boxes + 6 * i;
+        dm[i].wmin[0] = b[0]; dm[i].wmin[1] = b[1]; dm[i].wmin[2] = b[2]; dm[i].wmaxx = b[3]; dm[i].wmaxy = b[4]; dm[i].wmaxz = b[5];
+    }
+    std::vector<NodePair> pairs; std::vector<int> order;
+    DevParams P;
+    memset(&P, 0, sizeof(P));
+    P.modelCount = n;
+    RepackState::planTlas(dm, n, pairs, order, P.tlasRootStart, P.tlasRootCount);
+    DevBuf<NodePair> dPairs; DevBuf<int> dLeaves, dOut; DevBuf<float> dBoxes, dRays;
+    if (report(dPairs.alloc(pairs.size()), "cudaMalloc") || report(dLeaves.alloc(order.size()), "cudaMalloc") || report(dOut.alloc(3 * nrays), "cudaMalloc") ||
+        report(dBoxes.alloc(6 * (size_t)n), "cudaMalloc") || report(dRays.alloc(7 * nrays), "cudaMalloc")) return 2;
+    if ((!pairs.empty() && report(cudaMemcpy(dPairs.p, pairs.data(), pairs.size() * sizeof(NodePair), cudaMemcpyHostToDevice), "cudaMemcpy")) ||
+        report(cudaMemcpy(dLeaves.p, order.data(), order.size() * sizeof(int), cudaMemcpyHostToDevice), "cudaMemcpy") ||
+        report(cudaMemcpy(dBoxes.p, boxes, 6 * (size_t)n * 4, cudaMemcpyHostToDevice), "cudaMemcpy") ||
+        (nrays && report(cudaMemcpy(dRays.p, rays, 7 * nrays * 4, cudaMemcpyHostToDevice), "cudaMemcpy"))) return 2;
+    P.tlasPairs = dPairs.p; P.tlasLeaves = dLeaves.p; P.tlas = 1;
+    if (!nrays) return 0;
+#ifdef RT_SIMT_EMU
+    const unsigned grid = (unsigned)std::min<size_t>((nrays + 255) / 256, 16);
+#else
+    const unsigned grid = (unsigned)std::min<size_t>((nrays + 255) / 256, 8192);
+#endif
+    RT_LAUNCH(grid, 256, 0, (cudaStream_t)0, k_tlas_check, P, dBoxes.p, dRays.p, nrays, dOut.p);
+    if (report(cudaGetLastError(), "launch")) return 2;
+    if (report(cudaMemcpy(out, dOut.p, 3 * nrays * 4, cudaMemcpyDeviceToHost), "cudaMemcpy")) return 2;
+    return report(cudaStreamSynchronize((cudaStream_t)0), "cudaStreamSynchronize");
 }
 
 } // extern "C"

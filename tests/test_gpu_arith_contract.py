@@ -393,21 +393,79 @@ def test_ray_sphere_and_the_sphere_padding_bound(libs, scale):
         g = np.isin(cls, (0, 1, 2, 5)) & ((got[:, 0] & 1) == 1)
         pos32, c32, r32 = rec[g, 0:3].view(np.float32), rec[g, 6:9].view(np.float32), rec[g, 9].view(np.float32)
         origin = np.concatenate([np.minimum(pos32, c32 - r32[:, None]), np.maximum(pos32, c32 + r32[:, None])], axis=1)
-        blo, bhi = dev.sphere_boxes(np.concatenate([c32, r32[:, None]], axis=1), origin)
-        pos, d, c = _f64(rec[g], 0, 3), _f64(rec[g], 3, 6), _f64(rec[g], 6, 9)
-        r = np.abs(r32.astype(np.float64))
-        p = pos + d * got[g, 1].view(np.float32).astype(np.float64)[:, None]
-        inside = np.all((p >= blo) & (p <= bhi), axis=1)
+        inside, off_pad, off_claim = _sphere_hit_in_padded_box(dev, rec[g], got[g], origin)
         assert np.all(inside), f"{np.count_nonzero(~inside)} sphere hit points outside the padded box of their sphere"
-        off = np.abs(np.linalg.norm(p - c, axis=1) - r)
-        pad = np.minimum((c - r[:, None]) - blo, bhi - (c + r[:, None])).min(axis=1)
-        D2 = ((pos - c) ** 2).sum(axis=1)
-        worst_pad = max(worst_pad, float((off / pad).max(initial=0)))
-        worst_claim = max(worst_claim, float((off / (2.5e-7 * (D2 + r * r) / r)).max(initial=0)))
+        worst_pad = max(worst_pad, float(off_pad.max(initial=0)))
+        worst_claim = max(worst_claim, float(off_claim.max(initial=0)))
         counted += int(np.count_nonzero(g))
     _report("RaySphereCore", total, f"{counted:,} hit points inside the product's padded sphere boxes; distance off the sphere: worst "
             f"{worst_pad:.3f} of the padding ({worst_claim:.3f} of the 2.5e-7 (D^2+r^2)/r estimate)")
     assert counted > 0 and worst_pad < 0.5
+
+
+def _sphere_hit_in_padded_box(dev, rec, got, origin):
+    """For ray_sphere hits (rec, got rows) and origin boxes (n, 6): whether the float64 hit point pos + dir * dst lies in the box
+    paddedSphereBox gives the sphere, its distance off the exact sphere over the padding of that box, and over the 2.5e-7 (D^2 + r^2)
+    / r estimate the padding was derived from."""
+    c32, r32 = rec[:, 6:9].view(np.float32), rec[:, 9].view(np.float32)
+    blo, bhi = dev.sphere_boxes(np.concatenate([c32, r32[:, None]], axis=1), origin)
+    pos, d, c = _f64(rec, 0, 3), _f64(rec, 3, 6), _f64(rec, 6, 9)
+    r = np.abs(r32.astype(np.float64))
+    p = pos + d * got[:, 1].view(np.float32).astype(np.float64)[:, None]
+    inside = np.all((p >= blo) & (p <= bhi), axis=1)
+    off = np.abs(np.linalg.norm(p - c, axis=1) - r)
+    pad = np.minimum((c - r[:, None]) - blo, bhi - (c + r[:, None])).min(axis=1)
+    D2 = ((pos - c) ** 2).sum(axis=1)
+    return inside, off / pad, off / (2.5e-7 * (D2 + r * r) / r)
+
+
+SPHERE_GATE_CLASSES = ("aimed inside", "near-tangent", "from the surface", "from inside the origin box")
+
+
+def test_sphere_padding_over_the_query_gates_domain(libs, scale):
+    """The padding bound above over the domain in which the queries use the sphere accelerator: direction lengths log-uniform over
+    the gate's 2^-10 .. 2^10 with both bounds, ray origins aimed from up to 8 units, near-tangent, on the surface (a bounce), and
+    anywhere in an origin box reaching 1e5 units out.  RaySphereCore bitwise against the oracle; per class, every hit point inside
+    the product's padded box and at most 0.5 of the padding off the sphere."""
+    dev, orc = libs
+    n_cls = len(SPHERE_GATE_CLASSES)
+    worst, counted, total = np.zeros(n_cls), np.zeros(n_cls, int), 0
+    for rng, m in _batches(scale, 10):
+        rec, cls, origin = P.sphere_gate_cases(rng, m)
+        got = P.compare_cases(dev, orc, "ray_sphere", rec)
+        g = (got[:, 0] & 1) == 1
+        inside, off_pad, _ = _sphere_hit_in_padded_box(dev, rec[g], got[g], origin[g])
+        assert np.all(inside), f"{np.count_nonzero(~inside)} sphere hit points outside the padded box, classes {sorted(set(cls[g][~inside].tolist()))}"
+        for c in range(n_cls):
+            s = cls[g] == c
+            worst[c] = max(worst[c], float(off_pad[s].max(initial=0)))
+            counted[c] += int(np.count_nonzero(s))
+        total += m
+    _report("RaySphereCore over the query gate's domain", total,
+            "; ".join(f"{name}: {counted[c]:,} hits, worst {worst[c]:.3f} of the padding" for c, name in enumerate(SPHERE_GATE_CLASSES)))
+    assert counted.min() > 0 and worst.max() < 0.5, f"worst margins {dict(zip(SPHERE_GATE_CLASSES, worst.round(3)))}"
+
+
+# Found by sphere_gate_cases with |dir| = 1e-21 (below the gate): a sphere of radius 0.19, 11.9 units from the ray origin.
+# dot(dir, dir) ~ 1e-42 is subnormal, the discriminant is mostly rounding, and the reference reports a hit at dst = 1.16e22, 0.20
+# units off the sphere (128 times the padding) and outside the box paddedSphereBox gives it: the accelerator would prune a hit the
+# reference draws.
+BELOW_GATE_SPHERE_CASE = [0xc0c6fcb7, 0xc08321d5, 0xc11e5cff, 0x1c54e618, 0x1bc1efc9, 0x1c3f59c8, 0x400daa36, 0xbe813338, 0xc016e4f8, 0x3e4486f3]
+BELOW_GATE_SPHERE_ORIGIN_BOX = [-6.218348979949951, -4.097879886627197, -9.897704124450684, 8.591245651245117, 2.244865655899048, -2.165803909301758]
+
+
+def test_sphere_hit_below_the_gate_lies_outside_its_padded_box(libs):
+    """Why the queries use the sphere accelerator only for 2^-20 <= dot(dir, dir) <= 2^20: below that the padding bound does not hold.
+    The pinned case: the device and the oracle agree bit for bit on a hit whose point lies outside the sphere's padded box."""
+    dev, orc = libs
+    rec = np.array([BELOW_GATE_SPHERE_CASE], dtype=np.uint32)
+    got = P.compare_cases(dev, orc, "ray_sphere", rec)
+    d = rec[0, 3:6].view(np.float32)
+    assert np.float32(np.float32(d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]) < np.float32(2.0 ** -20), "the case lies inside the gate"
+    assert got[0, 0] & 1, "the reference's arithmetic no longer reports the hit"
+    inside, off_pad, _ = _sphere_hit_in_padded_box(dev, rec, got, np.array([BELOW_GATE_SPHERE_ORIGIN_BOX], dtype=np.float32))
+    assert not inside[0], f"the hit point lies inside the padded box ({off_pad[0]:.3g} of the padding off the sphere)"
+    _report("RaySphereCore below the gate (|dir| = 1e-21)", 1, f"hit {off_pad[0]:.3g} x the padding off the sphere, outside its padded box")
 
 
 def test_model_skipping_keeps_every_hit_the_reference_finds(libs, scale):
@@ -427,40 +485,123 @@ def test_model_skipping_keeps_every_hit_the_reference_finds(libs, scale):
     dev, _ = libs
     worst, counted, outside_box, total, grazing, grazing_skipped = 0.0, 0, 0, 0, 0, 0
     for rng, m in _batches(scale, 7):
-        w2l, tri, geo, pos, d, origin, cull = P.model_cases(rng, m)
-        exact, padded, placed = dev.model_boxes(w2l, geo, origin)
-        assert placed == m
-        rows = w2l.reshape(m, 4, 4).transpose(0, 2, 1)[:, :3, :].reshape(m, 12)
-        rec = np.concatenate([P.f32bits(pos), P.f32bits(d), P.f32bits(tri), np.zeros((m, 9), np.uint32), P.f32bits(rows), P.f32bits(geo),
-                              padded.view(np.uint32), cull[:, None]], axis=1)
-        out, _ = dev.run("model_hit", rec)
-        f = out[:, 0]
-        A = rows.reshape(m, 3, 4)[:, :, :3].astype(np.float64)
-        ld = np.einsum("nij,nj->ni", A, d.astype(np.float64))
-        t3 = tri.reshape(m, 3, 3).astype(np.float64)
-        N = np.cross(t3[:, 1] - t3[:, 0], t3[:, 2] - t3[:, 0])
-        cos = np.abs((ld * N).sum(axis=1)) / (np.linalg.norm(ld, axis=1) * np.linalg.norm(N, axis=1))
-        hit = (f & 1) == 1
-        skipped = (f & 4) == 4
-        graze = cos < GRAZING_COS
-        grazing += int(np.count_nonzero(hit & graze))
-        grazing_skipped += int(np.count_nonzero(hit & graze & skipped))
-        hit &= ~graze
-        assert not np.any(hit & skipped), f"{np.count_nonzero(hit & skipped)} model hits skipped by WorldBoxOutOfReach"
-        g = hit & ((f & 2) == 2)
-        outside_box += int(np.count_nonzero(hit & ~g))
-        p = pos[g].astype(np.float64) + d[g].astype(np.float64) * out[g, 1].view(np.float32).astype(np.float64)[:, None]
-        lo, hi = exact[g, :3], exact[g, 3:]
-        need = np.maximum(np.maximum(lo - p, p - hi), 0.0)
-        pad = np.minimum(lo - padded[g, :3], padded[g, 3:] - hi)
-        worst = max(worst, float((need / pad).max(initial=0)))
-        counted += int(np.count_nonzero(g))
+        case = P.model_cases(rng, m)
+        r = _model_hit(dev, *case)
+        assert r["placed"].all()
+        grazing += int(np.count_nonzero(r["hit"] & r["graze"]))
+        grazing_skipped += int(np.count_nonzero(r["hit"] & r["graze"] & r["skipped"]))
+        hit = r["hit"] & ~r["graze"]
+        assert not np.any(hit & r["skipped"]), f"{np.count_nonzero(hit & r['skipped'])} model hits skipped by WorldBoxOutOfReach"
+        outside_box += int(np.count_nonzero(hit & ~r["in_box"]))
+        worst = max(worst, float(r["margin"].max(initial=0)))
+        counted += int(np.count_nonzero(hit & r["in_box"]))
         total += m
     _report("model skipping (mul_rm + RayTriangleCore + WorldBoxOutOfReach)", total,
             f"{counted:,} hits the reference finds, none skipped; worst distance outside the exact world box {worst:.3f} of the padding; "
             f"{outside_box:,} hits outside the geometry box, none skipped; {grazing:,} grazing hits (|cos| < {GRAZING_COS}), "
             f"{grazing_skipped} of them skipped (known defect)", vs_oracle=False)
     assert counted > 0 and worst < 0.5
+
+
+def _model_hit(dev, w2l, tri, geo, pos, d, origin, cull):
+    """model_hit on the product's padded world boxes of a batch of model_cases: per case `placed` (worldBoxOfModel accepted the
+    matrix; otherwise the box is infinite), `hit` (the reference finds it), `skipped` (WorldBoxOutOfReach skips the model), `graze`
+    (|cos| < GRAZING_COS), `in_box` (the local ray reaches the geometry box) and `margin`: for a non-grazing hit inside the geometry
+    box of a placed model, the largest distance of the world hit point outside the exact world box over that axis's padding (else 0)."""
+    m = len(pos)
+    exact, padded, _ = dev.model_boxes(w2l, geo, origin)
+    rows = w2l.reshape(m, 4, 4).transpose(0, 2, 1)[:, :3, :].reshape(m, 12)
+    rec = np.concatenate([P.f32bits(pos), P.f32bits(d), P.f32bits(tri), np.zeros((m, 9), np.uint32), P.f32bits(rows), P.f32bits(geo),
+                          padded.view(np.uint32), cull[:, None]], axis=1)
+    out, _ = dev.run("model_hit", rec)
+    f = out[:, 0]
+    A = rows.reshape(m, 3, 4)[:, :, :3].astype(np.float64)
+    ld = np.einsum("nij,nj->ni", A, d.astype(np.float64))
+    t3 = tri.reshape(m, 3, 3).astype(np.float64)
+    N = np.cross(t3[:, 1] - t3[:, 0], t3[:, 2] - t3[:, 0])
+    with np.errstate(all="ignore"):
+        cos = np.abs((ld * N).sum(axis=1)) / (np.linalg.norm(ld, axis=1) * np.linalg.norm(N, axis=1))
+    r = dict(placed=np.isfinite(padded).all(axis=1), hit=(f & 1) == 1, skipped=(f & 4) == 4, graze=cos < GRAZING_COS, in_box=(f & 2) == 2)
+    g = r["hit"] & ~r["graze"] & r["in_box"] & r["placed"]
+    p = pos[g].astype(np.float64) + d[g].astype(np.float64) * out[g, 1].view(np.float32).astype(np.float64)[:, None]
+    lo, hi = exact[g, :3], exact[g, 3:]
+    need = np.maximum(np.maximum(lo - p, p - hi), 0.0)
+    pad = np.minimum(lo - padded[g, :3], padded[g, 3:] - hi)
+    r["margin"] = np.zeros(m)
+    r["margin"][g] = (need / pad).max(axis=1, initial=0)
+    return r
+
+
+MODEL_GATE_CLASSES = ("R S R, from afar", "sheared, from afar", "R S R, from inside the origin box", "sheared, from inside the origin box",
+                      "R S R, from the triangle", "sheared, from the triangle")
+
+
+def test_model_skipping_over_the_query_gates_domain(libs, scale):
+    """The check above over the whole domain in which the queries (rtTraceRays, rtTraceOcclusion, every bounce of rtTracePaths) use
+    model skipping and the TLAS: worldToLocal with singular values 1e-3 .. 1e3, rotation x scale x rotation and sheared products of
+    two of them (a rotated child of a non-uniformly scaled parent); direction lengths log-uniform over the gate's 2^-10 .. 2^10 with
+    both bounds; ray origins from afar, anywhere in the origin box, and on the triangle itself (a bounce).  Per class: no non-grazing
+    hit skipped, worst distance outside the exact world box below 0.5 of the padding.  Matrices worldBoxOfModel refuses get an
+    infinite box (never skipped) and are counted.  Also reported, not asserted: skipped hits with |dir| below the gate (1e-23 ..
+    2^-10), where the queries take the linear loop."""
+    dev, _ = libs
+    n_cls = len(MODEL_GATE_CLASSES)
+    worst, counted, refused, grazing, total = np.zeros(n_cls), np.zeros(n_cls, int), 0, 0, 0
+    for rng, m in _batches(scale, 8):
+        *case, cls = P.model_gate_cases(rng, m)
+        r = _model_hit(dev, *case)
+        hit = r["hit"] & ~r["graze"]
+        bad = hit & r["skipped"]
+        assert not bad.any(), f"{np.count_nonzero(bad)} model hits skipped by WorldBoxOutOfReach, classes {sorted(set(cls[bad].tolist()))}"
+        for c in range(n_cls):
+            s = cls == c
+            worst[c] = max(worst[c], float(r["margin"][s].max(initial=0)))
+            counted[c] += int(np.count_nonzero(hit[s] & r["placed"][s]))
+        refused += int(np.count_nonzero(~r["placed"]))
+        grazing += int(np.count_nonzero(r["hit"] & r["graze"]))
+        total += m
+    below, below_hits, below_skipped = 0, 0, 0
+    for rng, m in _batches(dict(scale, cases=scale["cases"] // 10), 9):
+        *case, _ = P.model_gate_cases(rng, m, lengths=np.exp(rng.uniform(np.log(1e-23), np.log(P.GATE_LEN_MIN), m)))
+        r = _model_hit(dev, *case)
+        hit = r["hit"] & ~r["graze"]
+        below_hits += int(np.count_nonzero(hit))
+        below_skipped += int(np.count_nonzero(hit & r["skipped"]))
+        below += m
+    _report("model skipping over the query gate's domain", total,
+            "; ".join(f"{name}: {counted[c]:,} hits, worst {worst[c]:.3f} of the padding" for c, name in enumerate(MODEL_GATE_CLASSES)) +
+            f"; {refused:,} matrices refused by worldBoxOfModel (infinite box); {grazing:,} grazing hits left out.  Below the gate "
+            f"(|dir| 1e-23 .. 2^-10): {below:,} cases, {below_hits:,} hits, {below_skipped} skipped", vs_oracle=False)
+    assert counted.min() > 0 and worst.max() < 0.5, f"worst margins {dict(zip(MODEL_GATE_CLASSES, worst.round(3)))}"
+
+
+def test_tlas_marks_every_model_its_own_box_keeps(libs, scale):
+    """TlasCollect (rt_device.cuh) on the tree the host's planTlas builds: a model is left out of the mask only if WorldBoxOutOfReach
+    rejects a TLAS box that encloses its box, and that must imply the same test rejects the model's own box, at the same bestDst.
+    Trees of 1 .. 4,096 boxes (generic, grid cells sharing faces, flat, bounds at +-0, NaN bounds, the infinite box of a singular
+    model); rays generic, axis-aligned (invDir = +-inf), on a slab plane or one ulp inside it and parallel to it (0 x inf = NaN), from
+    box corners, direction lengths over the query gate's range; bestDst +inf, a box corner's distance, +-0, tiny, huge, NaN.  Every
+    model whose own box test keeps it must be marked.  Device only: the reference has no TLAS."""
+    dev, _ = libs
+    trees = 40
+    per_tree = max(scale["cases"] // trees, 1)
+    rng = np.random.default_rng(12)
+    kept, rays, models = 0, 0, 0
+    for t in range(trees):
+        n = P.TLAS_SIZES[t] if t < len(P.TLAS_SIZES) else int(np.exp(rng.uniform(0, np.log(4096))))
+        boxes = P.tlas_boxes(rng, n)
+        for done in range(0, per_tree, scale["batch"]):
+            r = P.tlas_rays(rng, boxes, min(scale["batch"], per_tree - done))
+            out = dev.tlas_check(boxes, r)
+            bad = np.flatnonzero(out[:, 1])
+            assert len(bad) == 0, (f"{len(bad)} rays:TlasCollect leaves out a model its own box keeps; first: {n} models, "
+                                   f"ray {r[bad[0]].tolist()}, model {out[bad[0], 2]} box {boxes[out[bad[0], 2]].tolist()}")
+            kept += int(out[:, 0].sum())
+            rays += len(r)
+        models += n
+    _report("TlasCollect on planTlas trees", rays, f"{trees} trees, {models:,} model boxes; {kept:,} (ray, model) pairs kept by the "
+            "model's own box, every one marked", vs_oracle=False)
+    assert kept > 0
 
 
 GRAZING_COS = 1e-2

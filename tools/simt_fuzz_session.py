@@ -13,6 +13,14 @@ partial state changes.
 
 --frames: a step may render a batch of 2-6 frames as one call (RenderFrames: rtDispatchFrames) instead of one frame, on both sides.
 Where the kernels' side refuses the batch because "sampleChunks" is forced to 2 or more, it renders the frames one by one instead.
+
+--queries: query steps anywhere in the script — before OnEnable, between a scene change and the next frame, right after a raw
+dispatch, between frames: rtTraceRays, rtTraceOcclusion or rtTracePaths of 0, 1, 31, 32, 33 or a few hundred rays (the ray sets of
+tests/test_gpu_trace_rays.py; for occlusion tMax at, one ulp below and above the oracle's closest hit and special values; for paths
+random RNG states, 1-3 samples and the session's MaxBounceCount), through the manager, the context's host form or, on the kernels'
+side, the context's device form (the oracle answers through the same host form).  The answers are compared bit for bit, then
+RtStats.rays the batch added and, while the kernels' side counts, its traversal counters; dispatches and kernelMs must not move.  The
+frames that follow compare the images as before, so a query that changed what a frame shows is found there.
 """
 import argparse
 import os
@@ -28,8 +36,109 @@ sys.path.insert(0, os.path.join(REPO, "tools"))
 import build as simt_build                      # noqa: E402
 from conftest import ORACLE_LIB                 # noqa: E402
 import ray_tracing_b200 as rt                   # noqa: E402
-from ray_tracing_b200 import scenes             # noqa: E402
+from ray_tracing_b200 import capi, scenes       # noqa: E402
 from simt_fuzz import random_material, random_scene   # noqa: E402
+from test_gpu_trace_rays import assert_hits_equal, ray_sets      # noqa: E402
+from test_gpu_occlusion import assert_occlusion_equal, tmax_sets  # noqa: E402
+from test_gpu_trace_paths import assert_radiance_equal           # noqa: E402
+
+QUERY_KINDS = ("trace_rays", "trace_occlusion", "trace_paths")
+QUERY_FORMS = ("manager", "context", "device")
+
+
+def random_query(rng):
+    """('query', (kind, form, batch size, seed, no_cull, samples))"""
+    n = int(rng.choice([0, 1, 31, 32, 33, int(rng.randint(100, 400))]))
+    return ("query", (str(rng.choice(QUERY_KINDS)), str(rng.choice(QUERY_FORMS)), n, int(rng.randint(0, 2 ** 31 - 1)), bool(rng.rand() < 0.5),
+                      int(rng.randint(1, 4))))
+
+
+class DeviceMemory:
+    """Buffers for the context's *_device forms: torch CUDA tensors for a CUDA build; for a build of tests/simt, whose device memory
+    is host memory, numpy arrays."""
+
+    def __init__(self, lib):
+        self.torch = None
+        if os.path.dirname(os.path.abspath(lib)) != os.path.abspath(simt_build.OUT_DIR):
+            import torch
+            self.torch = torch
+
+    def call(self, ctx, fn, src, out_dtype, *extra):
+        n = len(src)
+        out = np.zeros(n, dtype=out_dtype)
+        if self.torch is None:
+            src = np.ascontiguousarray(src)
+            getattr(ctx, fn)(src.ctypes.data, out.ctypes.data, n, *extra)
+            ctx.synchronize()
+            return out
+        t = self.torch
+        d_src = t.from_numpy(np.concatenate([src.view(np.uint8).ravel(), np.zeros(16, np.uint8)])).cuda()
+        d_out = t.zeros(out.nbytes + 16, dtype=t.uint8, device="cuda")
+        getattr(ctx, fn)(d_src.data_ptr(), d_out.data_ptr(), n, *extra)
+        ctx.synchronize()
+        return d_out.cpu().numpy()[:out.nbytes].view(out_dtype)
+
+
+def query_batch(oracle, q, pool):
+    """The rays, segments or path rays of query step q, drawn from the case's ray pool.  Segments take tMax from the oracle's closest
+    hits in the scene as it stands, through the step's form (before either side reads its counters)."""
+    kind, form, n, seed, no_cull, _ = q
+    rng = np.random.RandomState(seed)
+    rays = pool[rng.randint(0, len(pool), n)]
+    if kind == "trace_occlusion":
+        try:
+            closest = (oracle if form == "manager" else oracle.context).trace_rays(rays, no_cull=no_cull)
+        except rt.capi.RtError:                  # the query itself will be refused the same way: any tMax will do
+            closest = np.zeros(n, dtype=capi.RAY_HIT_DTYPE)
+            closest["dst"] = np.inf
+        segs = np.concatenate(list(tmax_sets(rays, closest, seed=seed).values()))
+        return segs[rng.permutation(len(segs))[:n]]
+    if kind == "trace_paths":
+        return capi.make_path_rays(rays["origin"], rays["dir"], rng.randint(0, 2 ** 32, size=n, dtype=np.uint64).astype(np.uint32))
+    return rays
+
+
+def run_query(mgr, q, arg, kernels_side, device):
+    """One query step on one side: (answers, or the RT_E_* code of a refusal; RtStats before; RtStats after)."""
+    kind, form, _, _, no_cull, samples = q
+    ctx = mgr.context
+    try:
+        before = ctx.stats()
+        if form == "device" and kernels_side:
+            out_dtype = {"trace_rays": capi.RAY_HIT_DTYPE, "trace_occlusion": np.uint8, "trace_paths": capi.PATH_RADIANCE_DTYPE}[kind]
+            extra = (samples,) if kind == "trace_paths" else (no_cull,)
+            got = device.call(ctx, kind + "_device", arg, out_dtype, *extra)
+            if kind == "trace_occlusion":
+                got = got.view(np.bool_)
+        else:
+            target = mgr if form == "manager" else ctx
+            got = getattr(target, kind)(arg, samples) if kind == "trace_paths" else getattr(target, kind)(arg, no_cull=no_cull)
+        return got, before, ctx.stats()
+    except rt.capi.RtError as e:
+        return e.code, None, None
+
+
+def compare_query(q, o, g, counting, spheres):
+    """None, or what differs between the oracle's (o) and the kernels' (g) results of run_query."""
+    kind = q[0]
+    (wo, bo, ao), (wg, bg, ag) = o, g
+    if isinstance(wo, int) or isinstance(wg, int):
+        return None if (isinstance(wo, int) and isinstance(wg, int) and wo == wg) else f"{kind} refused on one side ({wo if isinstance(wo, int) else 'ok'} vs {wg if isinstance(wg, int) else 'ok'})"
+    if len(wg) != len(wo):
+        return f"{kind}: {len(wg)} answers vs the oracle's {len(wo)}"
+    try:
+        if len(wo):
+            {"trace_rays": assert_hits_equal, "trace_occlusion": assert_occlusion_equal, "trace_paths": assert_radiance_equal}[kind](wg, wo, kind)
+    except AssertionError as e:
+        return str(e)
+    keys = ("rays",) + (("boxTests", "triTests") + (("sphereTests",) if spheres <= 64 else ()) if counting else ())
+    for k in keys:
+        if ag[k] - bg[k] != ao[k] - bo[k]:
+            return f"{kind}: RtStats.{k} grew by {ag[k] - bg[k]} vs the oracle's {ao[k] - bo[k]}"
+    for side, b, a in (("kernels'", bg, ag), ("oracle's", bo, ao)):
+        if a["dispatches"] != b["dispatches"] or a["kernelMs"] != b["kernelMs"]:
+            return f"{kind} moved the {side} dispatches / kernelMs ({b['dispatches']}, {b['kernelMs']} -> {a['dispatches']}, {a['kernelMs']})"
+    return None
 
 
 def random_spheres(rng, n):
@@ -39,17 +148,22 @@ def random_spheres(rng, n):
     return sph
 
 
-def make_script(rng, sc, steps, frames=False):
+def make_script(rng, sc, steps, frames=False, queries=False):
     """A list of (action, arguments) — applied to both managers; ('option', ...) only to the kernels' side.  frames: a step may end in
-    ('frames', (n,)), a batch of n frames, instead of ('frame', ())."""
-    script = []
+    ('frames', (n,)), a batch of n frames, instead of ('frame', ()).  queries: ('query', ...) steps (random_query) before OnEnable,
+    among the scene changes, after raw dispatches and after frames."""
+    script = [random_query(rng)] if queries and rng.rand() < 0.3 else []
     nm = len(sc.models)
     for _ in range(steps):
         for _ in range(int(rng.randint(0, 4))):
-            a = int(rng.randint(0, 11))
-            if a == 10:
+            a = int(rng.randint(0, 12 if queries else 11))
+            if a == 11:
+                script.append(random_query(rng))
+            elif a == 10:
                 # round 2: the ABI below the manager — modelCount set on its own (no ModelInfo re-send), then a dispatch
                 script.append(("rawframe", (int(rng.randint(0, nm + 1)), int(rng.randint(1, 1000)))))
+                if queries and rng.rand() < 0.5:
+                    script.append(random_query(rng))
             elif a == 0:
                 d = float(rng.choice([0.0, 3.0, 5.67, 60.0, 4000.0, 3e5]))
                 script.append(("camera", (float(np.clip(np.degrees(2 * np.arctan(3.0 / max(d, 3.0))), 1e-3, 90.0)),
@@ -77,6 +191,8 @@ def make_script(rng, sc, steps, frames=False):
             script.append(("frames", (int(rng.randint(2, 7)),)))
         else:
             script.append(("frame", ()))
+        if queries and rng.rand() < 0.3:
+            script.append(random_query(rng))
     return script
 
 
@@ -118,25 +234,46 @@ def main():
     ap.add_argument("--lib", default=None)
     ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters after every frame")
     ap.add_argument("--frames", action="store_true", help="steps may render a batch of 2-6 frames in one call (RenderFrames)")
+    ap.add_argument("--queries", action="store_true", help="query steps (rtTraceRays / rtTraceOcclusion / rtTracePaths) anywhere in the script")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
-    bad = 0
+    device = DeviceMemory(lib) if args.queries else None
+    bad, query_steps = 0, {k: 0 for k in QUERY_KINDS + QUERY_FORMS}
     for case in range(args.cases):
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
         sc = random_scene(rng, odd=0.0)
-        script = make_script(rng, sc, args.steps, args.frames)
+        script = make_script(rng, sc, args.steps, args.frames, args.queries)
+        pool = np.concatenate(list(ray_sets(sc, seed=seed, n=48).values())) if args.queries else None
         mgrs = []
         for backend in (ORACLE_LIB, lib):
             m = rt.RayComputeManager(backend)
             scenes.apply(sc, m)
             if args.pixel_stats:
                 m.context.set_option("countStats", 1)
-            m.OnEnable()
             mgrs.append(m)
-        frame_no, failed, resized, chunks = 0, None, False, -1
+        frame_no, failed, resized, chunks, enabled = 0, None, False, -1, False
+        counting, spheres = args.pixel_stats, len(sc.spheres)          # the kernels' side's countStats; the Spheres buffer's length
         try:
             for action, a in script:
+                if action != "query" and not enabled:
+                    for m in mgrs:
+                        m.OnEnable()
+                    enabled = True
+                if action == "query":
+                    batch = query_batch(mgrs[0], a, pool)
+                    o, g = (run_query(m, a, batch, i == 1, device) for i, m in enumerate(mgrs))
+                    failed = compare_query(a, o, g, counting, spheres)
+                    if failed:
+                        failed = f"query {a[:3]} after {frame_no} frames: {failed}"
+                        break
+                    query_steps[a[0]] += 1
+                    query_steps[a[1]] += 1
+                    continue
+                if action == "option" and a[0] == "countStats":
+                    counting = bool(a[1])
+                if action == "spheres":
+                    spheres = len(a[0])
                 if action == "screen":
                     resized = True                      # the textures follow at the next RenderFrame (InitFrame): no raw dispatch in between
                 if action == "rawframe" and resized:
@@ -189,11 +326,12 @@ def main():
             m.OnDestroy()
         if failed:
             bad += 1
-            brief = [(act, a if act in ("option", "setting", "screen") else "...") for act, a in script]
+            brief = [(act, a if act in ("option", "setting", "screen", "query") else "...") for act, a in script]
             print(f"case seed {seed}: {failed}; {len(sc.models)} models, {len(sc.spheres)} spheres; script {brief}", flush=True)
         if (case + 1) % 25 == 0:
             print(f"  {case + 1} cases, {bad} findings", flush=True)
-    print(f"{args.cases} cases, {bad} findings")
+    print(f"{args.cases} cases, {bad} findings" +
+          (f"; query steps equal: {sum(query_steps[k] for k in QUERY_KINDS)} (" + ", ".join(f"{k} {v}" for k, v in query_steps.items()) + ")" if args.queries else ""))
     return 1 if bad else 0
 
 
