@@ -1569,6 +1569,24 @@ int rtxPlanPairsOrdered(const RtNode* nodes, int nodeCount, const RtModel* model
     return (int)out.size();
 }
 
+#ifdef RT_POOL_CLOCKS
+/* Cycle account of the pooled kernel (RT_POOL_CLOCKS variant builds only, not part of include/rt_b200.h): copies the 3 x CK_KINDS
+ * counters ([cycles, steps, lanes] per step kind, rt_kernel_pool.cuh) of the current device into out (n >= 3 * CK_KINDS), then zeroes
+ * them if reset != 0.  Returns the number of counters or a negative RT_E_* code. */
+int rtxPoolClocks(unsigned long long* out, int n, int reset)
+{
+    if (!out || n < 3 * CK_KINDS) return RT_E_INVALID;
+    if (cudaDeviceSynchronize() != cudaSuccess) return RT_E_CUDA;
+    if (cudaMemcpyFromSymbol(out, g_poolClocks, sizeof(g_poolClocks)) != cudaSuccess) return RT_E_CUDA;
+    if (reset)
+    {
+        static const unsigned long long zero[3 * CK_KINDS] = {};
+        if (cudaMemcpyToSymbol(g_poolClocks, zero, sizeof(zero)) != cudaSuccess) return RT_E_CUDA;
+    }
+    return 3 * CK_KINDS;
+}
+#endif
+
 /* Device-free test hook (not part of include/rt_b200.h): the TLAS the upload would build over `modelCount` world boxes
  * (6 floats each: min xyz, max xyz).  pairsOut: capacity pairCap records of 64 bytes; leavesOut: modelCount model indices in leaf
  * order; rootOut: 2 ints (start, count).  Returns the number of pair records or a negative RT_E_* code. */

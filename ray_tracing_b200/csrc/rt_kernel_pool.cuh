@@ -9,9 +9,11 @@
 //                 material branch.  Finished pixels are written out; their slots are refilled from the global pixel
 //                 queue (ballot compaction of free slots, ONE atomicAdd per warp per refill); camera rays for new
 //                 samples are generated in compacted batches.
-//   TRACE phase   the warp's M rays are consumed through a warp-local queue: a lane that finishes its ray stores the
-//                 hit record and immediately takes the next ray (ballot-ranked pop from a warp-uniform counter, no
-//                 atomics).  Every lane is a small state machine (inner node / leaf primitive / next model); each
+//   TRACE phase   the warp's M rays are consumed through a warp-local queue: a lane that finishes its ray flips its slot's
+//                 state and immediately takes the next ray (ballot-ranked pop from a warp-uniform counter, no atomics); the
+//                 slot's hit record is written whenever a test improves the result, so the lane keeps only the closest distance,
+//                 the hit kind and the model-local ray in registers, and re-reads the world ray from the slot when it changes
+//                 models.  Every lane is a small state machine (inner node / leaf primitive / next model); each
 //                 iteration one warp reduction counts the lanes per state and the warp executes the step kind most
 //                 lanes wait for (two inner-node visits per census).  When the queue is empty and at most `tailLanes`
 //                 lanes still trace, the phase ends and those rays stay in flight, in their lanes, across the next
@@ -48,10 +50,10 @@ namespace rtd {
 //   RT_LEAF_REPEAT=n   n leaf primitives per census (like RT_INNER_REPEAT for inner nodes)
 //   (RT_PREFETCH_CUR: below)
 //   RT_PREFETCH_NEXT_PAIR   L1 prefetch of the record after the one being fetched (meant for "pairOrder" = 1, where that is child A's)
-//   RT_SMEM_STACK=N    (N a power of two) the top N entries of every lane's traversal stack live in shared memory — a ring, word-major
-//                      across the warp, so lane = bank and a push or pop is two conflict-free 4-byte accesses instead of a local-memory
-//                      access that touches up to 32 different lines (divergent stack depths); deeper entries spill to the local
-//                      array, oldest first.  Costs N * 6 KB of shared memory per CTA (taken from L1).
+//   RT_SMEM_STACK=N    (N a power of two) the top N entries of every lane's traversal stack live in shared memory — a ring, entry-major
+//                      across the warp (entry i = 32 lanes x one int2), so a push or pop is one conflict-free 8-byte access instead of a
+//                      local-memory access that touches up to 32 different lines (divergent stack depths); deeper entries spill to the
+//                      local array, oldest first.  Costs N * 6 KB of shared memory per CTA (taken from L1).
 // RING = entries of the shared-memory ring of a kernel instantiation: RT_SMEM_STACK, except for the 96-slot pools, whose 223 KB of path
 // state leave no room for it (they keep the whole stack in local memory).
 #if defined(RT_SMEM_STACK) && !defined(RT_STACK_TOP_REG)
@@ -73,14 +75,16 @@ template <int M> struct PoolRing { static constexpr int N = 0; };
 #define RT_PUSH(x) do { if (stackCount > 0) stack[stackCount - 1] = stackTop; stackTop = (x); stackCount++; } while (0)
 #define RT_POP(dst) do { (dst) = stackTop; --stackCount; if (stackCount > 0) stackTop = stack[stackCount - 1]; } while (0)
 #else
-// entries [stackSpilled, stackCount) are in the ring at index (i & (RING - 1)); entries [0, stackSpilled) in the local array
+// entries [stackSpilled, stackCount) are in the ring at index (i & (RING - 1)); entries [0, stackSpilled) in the local array.
+// A ring entry is one int2 (start, count) per lane: entry i of the warp is 32 x 8 bytes, one conflict-free 64-bit access per push / pop.
+// `ringLane` (this lane's word of entry 0) is computed once per kernel, so an access is that base plus (i & (RING - 1)) * 256 bytes.
+#define RT_RING(i) ringLane[((i) & (RING - 1)) * 32]
 #define RT_PUSH(x) do { if constexpr (RING > 0) { \
-                            if (stackCount - stackSpilled == RING) { NodeRef sp_; const int r_ = (stackSpilled & (RING - 1)) * 64; \
-                                sp_.start = ring[r_ + (int)lane]; sp_.count = ring[r_ + 32 + (int)lane]; stack[stackSpilled++] = sp_; } \
-                            const NodeRef px_ = (x); const int w_ = (stackCount & (RING - 1)) * 64; ring[w_ + (int)lane] = px_.start; ring[w_ + 32 + (int)lane] = px_.count; stackCount++; } \
+                            if (stackCount - stackSpilled == RING) { const int2 sp_ = RT_RING(stackSpilled); stack[stackSpilled++] = node_ref(sp_); } \
+                            const NodeRef px_ = (x); RT_RING(stackCount) = make_int2(px_.start, px_.count); stackCount++; } \
                         else { stack[stackCount++] = (x); } } while (0)
 #define RT_POP(dst) do { if constexpr (RING > 0) { --stackCount; if (stackCount < stackSpilled) { (dst) = stack[--stackSpilled]; } \
-                             else { const int w_ = (stackCount & (RING - 1)) * 64; (dst).start = ring[w_ + (int)lane]; (dst).count = ring[w_ + 32 + (int)lane]; } } \
+                             else { (dst) = node_ref(RT_RING(stackCount)); } } \
                          else { (dst) = stack[--stackCount]; } } while (0)
 #endif
 #define RT_STACK_RESET() stackSpilled = 0
@@ -129,6 +133,27 @@ template <int M> struct PoolRing { static constexpr int N = 0; };
 #else
 #define RT_PF_CUR() do { } while (0)
 #endif
+// RT_POOL_CLOCKS (variant build only, tools/build_variants.py "clocks", read by tools/pool_clocks.py): a cycle account of the kernel.
+// Lane 0 of every warp adds, per step kind, the clock64() cycles since the previous mark, the number of such steps and the lanes (or
+// slots) they served into 32-bit counters in shared memory (96 bytes per warp after the stack rings); when the warp ends it adds them
+// to g_poolClocks.  The marks cost a few instructions per step: on the default workload the build runs 16-21 % slower (DESIGN §5).
+#if defined(RT_POOL_CLOCKS) && !defined(RT_SIMT_EMU)
+enum : int { CK_CENSUS = 0, CK_INNER, CK_LEAF, CK_NEXT, CK_SHADE, CK_REFILL, CK_CAMERA, CK_QUEUE, CK_KINDS };
+constexpr int POOL_CLOCK_BYTES = 3 * CK_KINDS * 4;                  // per warp: [cycles, steps, lanes] x kind
+__device__ unsigned long long g_poolClocks[3 * CK_KINDS];
+#define RT_CK_INIT() unsigned* ckAcc = reinterpret_cast<unsigned*>(poolBase + (size_t)POOL_WARPS * POOL_BYTES + (size_t)POOL_THREADS * RING * 8) \
+                                       + warp * (3 * CK_KINDS); \
+                     if (lane < 3u * CK_KINDS) ckAcc[lane] = 0u; __syncwarp(); long long ckT = clock64()
+#define RT_CK(kind, lanes) do { const long long t_ = clock64(); \
+                                if (lane == 0) { ckAcc[3 * (kind)] += (unsigned)(t_ - ckT); ckAcc[3 * (kind) + 1]++; ckAcc[3 * (kind) + 2] += (unsigned)(lanes); } \
+                                ckT = t_; } while (0)
+#define RT_CK_FLUSH() do { __syncwarp(); if (lane < 3u * CK_KINDS) atomicAdd(g_poolClocks + lane, (unsigned long long)ckAcc[lane]); } while (0)
+#else
+constexpr int POOL_CLOCK_BYTES = 0;
+#define RT_CK_INIT() do { } while (0)
+#define RT_CK(kind, lanes) do { } while (0)
+#define RT_CK_FLUSH() do { } while (0)
+#endif
 constexpr int POOL_WARPS = RT_POOL_WARPS;      // warps per CTA (one persistent CTA per SM)
 constexpr int POOL_THREADS = POOL_WARPS * 32;
 constexpr int POOL_WORDS = 24;                 // 32-bit words of state per path slot
@@ -156,6 +181,8 @@ static_assert(F_HMODEL == POOL_WORDS - 1, "pool layout");
 #endif
 constexpr int POOL_COLD_WORDS = POOL_WORDS - POOL_HOT_WORDS;
 
+RT_DI NodeRef node_ref(int2 v) { NodeRef r; r.start = v.x; r.count = v.y; return r; }
+
 RT_DI unsigned info_pack(unsigned sample, unsigned bounce, unsigned state) { return (sample << 12) | (bounce << 4) | state; }
 RT_DI unsigned info_state(unsigned i) { return i & 15u; }
 RT_DI unsigned info_bounce(unsigned i) { return (i >> 4) & 255u; }
@@ -173,6 +200,12 @@ template <int M> struct PoolView
     RT_DI int& i(int field, int e) const { return *reinterpret_cast<int*>(at(field, e)); }
     RT_DI f3 get3(int field, int e) const { return make_f3(f(field, e), f(field + 1, e), f(field + 2, e)); }
     RT_DI void set3(int field, int e, f3 v) const { f(field, e) = v.x; f(field + 1, e) = v.y; f(field + 2, e) = v.z; }
+    // the hit record of slot e (the running result of the ray traced on it): a triangle of a model ...
+    RT_DI void set_hit(int e, float dst, int prim, float u, float v, float det, int model) const
+    { f(F_HDST, e) = dst; i(F_HPRIM, e) = prim; f(F_HU, e) = u; f(F_HV, e) = v; f(F_HDET, e) = det; i(F_HMODEL, e) = model; }
+    // ... or sphere s of the Spheres buffer (u, v and model keep their values: the shade phase does not read them for spheres)
+    RT_DI void set_sphere_hit(int e, float dst, int s, bool inside) const
+    { f(F_HDST, e) = dst; i(F_HPRIM, e) = -(s + 1); f(F_HDET, e) = inside ? -1.0f : 1.0f; }
 };
 
 // Build in `order` the list of slots whose state is in [lo, hi], grouped by state (ascending); returns the count.
@@ -252,9 +285,10 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
     pool.order = reinterpret_cast<unsigned char*>(pool.w + POOL_HOT_WORDS * M);
     pool.g = POOL_COLD_WORDS ? P.poolCold + ((size_t)blockIdx.x * POOL_WARPS + warp) * (size_t)(POOL_COLD_WORDS * M) : nullptr;
     constexpr int RING = PoolRing<M>::N;
-    int* ring = reinterpret_cast<int*>(poolBase + (size_t)POOL_WARPS * POOL_BYTES) + (size_t)warp * (RING * 64);     // this warp's RING x 2 x 32 words
+    // this warp's RING x 32 int2 entries; ringLane = this lane's word of entry 0
+    int2* ringLane = reinterpret_cast<int2*>(poolBase + (size_t)POOL_WARPS * POOL_BYTES) + (size_t)warp * (RING * 32) + lane;
     int stackSpilled = 0;
-    (void)ring; (void)stackSpilled;
+    (void)ringLane; (void)stackSpilled;
 
     // ---- stage the tree tops (TMA bulk copy) and the spheres; initialise the pool -------------------------------------
     const uint32_t mbar = smem_u32(&hdr->mbar);
@@ -281,6 +315,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
     for (int c = 0; c < M / 32; c++) pool.u(F_INFO, c * 32 + (int)lane) = info_pack(0, 0, PS_EMPTY);
     if (P.smemPairs > 0) { while (!mbar_try_wait(mbar, 0)) { } }
     __syncthreads();
+    RT_CK_INIT();
 
     Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
     // STATS: the counters when this lane fetched the ray it traces (which may stay in flight across shade phases); the difference
@@ -298,9 +333,13 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
     enum { T_IDLE = 0, T_INNER = 1, T_LEAF = 2, T_NEXT = 3 };
     int mode = T_IDLE;
     int myEntry = -1;                                                // slot this lane is tracing
-    f3 rayPos = splat3(0.0f), rayDir = splat3(0.0f), lpos = splat3(0.0f), ldir = splat3(0.0f), linv = splat3(0.0f);
-    float resDst = inf32(), resU = 0.0f, resV = 0.0f, resDet = 0.0f; int resPrim = 0, resModel = 0; unsigned resKind = PS_HIT_MISS;
-    float bestDst = 0.0f, bestU = 0.0f, bestV = 0.0f, bestDet = 0.0f; int bestTri = -1;
+    f3 lpos = splat3(0.0f), ldir = splat3(0.0f), linv = splat3(0.0f);
+    // The ray's running result lives in its slot's hit words (F_HDST .. F_HMODEL): an improving hit writes them at once (rare,
+    // predicated stores), so T_NEXT only flips the slot's state when the ray ends.  The registers keep what the tests compare
+    // against: bestDst (= result.dst; every model starts from it, HL:359, so a model's winner always becomes the result), the
+    // hit kind, and for the sphere accelerator's first-index tie rule the buffer index of its best sphere.  The world ray is
+    // re-read from F_POS / F_DIR in the T_NEXT step, the only one that needs it.
+    float bestDst = inf32(); int bestTri = -1; unsigned hitKind = PS_HIT_MISS;
     int model = 0; bool cull = true;
     NodeRef cur; cur.start = 0; cur.count = 0;
     int leafK = 0;
@@ -405,6 +444,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                 }
             }
             __syncwarp();
+            RT_CK(CK_SHADE, n);
         }
 
         // (2) refill free slots from the global pixel queue (ballot compaction, one atomic per warp per pass)
@@ -456,6 +496,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
             }
         }
         __syncwarp();
+        RT_CK(CK_REFILL, 0);
 
         // (3) camera rays for the slots that start a sample (HL:567-576), in compacted batches
         {
@@ -479,10 +520,12 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                 }
             }
             __syncwarp();
+            RT_CK(CK_CAMERA, n);
         }
 
         // ================================================= TRACE phase =================================================
         const int nRays = P.sortRays ? CompactRaysByOctant<M>(pool, lane) : CompactByState<M>(pool, lane, PS_RAY, PS_RAY);
+        RT_CK(CK_QUEUE, nRays);
         if (nRays == 0 && __ballot_sync(0xffffffffu, mode != T_IDLE) == 0u) break;   // every slot is DONE: this warp is finished
         int next = 0;                                                // warp-uniform queue head
         bool finishedAny = false;                                    // warp-uniform: some ray completed in this phase
@@ -505,29 +548,32 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                 {
                     myEntry = pool.order[idx];
                     pool.u(F_INFO, myEntry) = (pool.u(F_INFO, myEntry) & ~15u) | PS_FLIGHT;
-                    rayPos = pool.get3(F_POS, myEntry); rayDir = pool.get3(F_DIR, myEntry);
                     if (STATS) rayStart = cnt;
                     cnt.rays++;
 #ifdef RT_CACHE_RAYINV
-                    rayInvW = rcp3(rayDir);
+                    rayInvW = rcp3(pool.get3(F_DIR, myEntry));
 #endif
-                    resDst = inf32(); resPrim = 0; resModel = 0; resKind = PS_HIT_MISS; resU = resV = resDet = 0.0f;
+                    bestDst = inf32(); hitKind = PS_HIT_MISS;
+                    pool.set_hit(myEntry, inf32(), 0, 0.0f, 0.0f, 0.0f, 0);
                     // spheres first (extension; where the reference's commented call sits, HL:341)
                     // A large Spheres buffer is searched through its accelerator by the same state machine as the meshes
                     // ("model -1": inner nodes = padded sphere boxes, leaves = spheres), see the T_NEXT / T_INNER / T_LEAF blocks.
-                    if (!(EXT && P.sphBvh))
-                    for (int s = 0; s < P.sphereCount; s++)
+                    if (!(EXT && P.sphBvh) && P.sphereCount > 0)
                     {
-                        float cx, cy, cz, r2; int flag;
-                        if (s < WAVE_MAX_SMEM_SPHERES) { const DevSphere sp = smemSpheres[s]; cx = sp.cx; cy = sp.cy; cz = sp.cz; r2 = sp.r2; flag = sp.pad0; }
-                        else { const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.spheres + s)); cx = s0.x; cy = s0.y; cz = s0.z;
-                               r2 = __ldg(&P.spheres[s].r2); flag = __ldg(&P.spheres[s].pad0); }
-                        float dst; bool inside;
-                        if (STATS) cnt.sph++;
-                        if (RaySphereCore(rayPos, rayDir, make_f3(cx, cy, cz), r2, dst, inside) && dst < resDst)
+                        const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
+                        for (int s = 0; s < P.sphereCount; s++)
                         {
-                            resDst = dst; resPrim = -(s + 1); resDet = inside ? -1.0f : 1.0f;
-                            resKind = flag == RT_MATERIAL_GLASS ? PS_HIT_GLASS : PS_HIT_OPAQUE;
+                            float cx, cy, cz, r2; int flag;
+                            if (s < WAVE_MAX_SMEM_SPHERES) { const DevSphere sp = smemSpheres[s]; cx = sp.cx; cy = sp.cy; cz = sp.cz; r2 = sp.r2; flag = sp.pad0; }
+                            else { const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.spheres + s)); cx = s0.x; cy = s0.y; cz = s0.z;
+                                   r2 = __ldg(&P.spheres[s].r2); flag = __ldg(&P.spheres[s].pad0); }
+                            float dst; bool inside;
+                            if (STATS) cnt.sph++;
+                            if (RaySphereCore(rayPos, rayDir, make_f3(cx, cy, cz), r2, dst, inside) && dst < bestDst)
+                            {
+                                bestDst = dst; hitKind = flag == RT_MATERIAL_GLASS ? PS_HIT_GLASS : PS_HIT_OPAQUE;
+                                pool.set_sphere_hit(myEntry, dst, s, inside);
+                            }
                         }
                     }
                     model = (EXT && P.sphBvh) ? -2 : -1; mode = T_NEXT;
@@ -543,6 +589,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
             // iteration would run each at a fraction of the warp.  One kind per iteration keeps the executed block dense,
             // the others catch up when their kind becomes the majority.  The per-ray visiting order is unchanged.
             // (RT_VOTE_W*: cost-weighted vote, see the macro block at the top; all weights 1 = the plain majority)
+            RT_CK(CK_CENSUS, 32 - nIdle);         // (census, fetch and vote of this iteration and of the fetch iterations before it)
             const int scoreInner = nInner * RT_VOTE_WI, scoreLeaf = nLeaf * RT_VOTE_WL, scoreNext = nNext * RT_VOTE_WN;
             if (scoreNext >= scoreInner && scoreNext >= scoreLeaf)
             {
@@ -551,16 +598,8 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                 bool fin = false;
                 if (mode == T_NEXT)
                 {
-                    if (model >= 0 && bestDst < resDst)              // HL:362-370 (normal / position are rebuilt when shading)
-                    {
-                        resDst = bestDst; resPrim = bestTri; resU = bestU; resV = bestV; resDet = bestDet; resModel = model;
-                        resKind = cull ? PS_HIT_OPAQUE : PS_HIT_GLASS;   // cull == (flag != GLASS)
-                    }
-                    if (EXT && P.sphBvh && model == -1 && bestTri != 0x7fffffff)     // sphere phase finished with a winner (bestTri = buffer index)
-                    {
-                        resDst = bestDst; resPrim = -(bestTri + 1); resDet = bestDet;
-                        resKind = __float_as_int(bestU) == RT_MATERIAL_GLASS ? PS_HIT_GLASS : PS_HIT_OPAQUE;
-                    }
+                    // (a model's winner, HL:362-370, and the sphere phase's are in the slot's hit words already)
+                    const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
                     model++;
                     // skip the models this ray cannot reach before its current best hit (not in the instrumented build, which
                     // walks every model like the reference so that the test counts stay identical)
@@ -573,22 +612,23 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
 #endif
                         if (useTlas)
                         {
-                            if (model == 0) TlasCollect(P, rayPos, rayInv, resDst, tlasMask);
+                            if (model == 0) TlasCollect(P, rayPos, rayInv, bestDst, tlasMask);
                             for (;;)
                             {
                                 model = TlasNext(tlasMask, model, P.modelCount);
-                                if (model >= P.modelCount || !ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, resDst)) break;
+                                if (model >= P.modelCount || !ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, bestDst)) break;
                                 model++;
                             }
                         }
                         else
-                        while (model < P.modelCount && ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, resDst)) model++;
+                        while (model < P.modelCount && ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, bestDst)) model++;
                     }
                     if (EXT && P.sphBvh && model == -1)
                     {
-                        // sphere phase: world-space ray against the accelerator of the Spheres buffer (semantics of TraverseSpheres)
+                        // sphere phase: world-space ray against the accelerator of the Spheres buffer (semantics of TraverseSpheres).
+                        // It comes first, so bestDst is still inf (no small-buffer sphere loop runs with an accelerator).
                         lpos = rayPos; ldir = rayDir; linv = rcp3(rayDir);
-                        bestDst = inf32(); bestTri = 0x7fffffff; bestDet = 1.0f; bestU = 0.0f;
+                        bestTri = 0x7fffffff;
                         cur.start = P.sphRootStart; cur.count = P.sphRootCount; leafK = 0; stackCount = 0; RT_STACK_RESET();
                         mode = cur.count > 0 ? T_LEAF : T_INNER; RT_PF_CUR();
                     }
@@ -601,17 +641,14 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         lpos = mul_rm(w2l, rayPos, 1.0f);
                         ldir = mul_rm(w2l, rayDir, 0.0f);
                         linv = rcp3(ldir);
-                        cull = meta.z != 0;
-                        bestDst = resDst; bestTri = -1;              // result.dst is the ray length shared across models (HL:359)
+                        cull = meta.z != 0;                          // bestDst: result.dst is the ray length shared across models (HL:359)
                         cur.start = meta.x; cur.count = meta.y; leafK = 0; stackCount = 0; RT_STACK_RESET();
                         mode = cur.count > 0 ? T_LEAF : T_INNER; RT_PF_CUR();
                     }
                     else
                     {
-                        pool.f(F_HDST, myEntry) = resDst; pool.i(F_HPRIM, myEntry) = resPrim;
-                        pool.f(F_HU, myEntry) = resU; pool.f(F_HV, myEntry) = resV; pool.f(F_HDET, myEntry) = resDet; pool.i(F_HMODEL, myEntry) = resModel;
                         const unsigned info = pool.u(F_INFO, myEntry);
-                        pool.u(F_INFO, myEntry) = (info & ~15u) | resKind;
+                        pool.u(F_INFO, myEntry) = (info & ~15u) | hitKind;
                         if (STATS)
                         {
                             const unsigned xy = pool.u(F_XY, myEntry);
@@ -621,6 +658,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     }
                 }
                 if (__any_sync(0xffffffffu, fin)) finishedAny = true;
+                RT_CK(CK_NEXT, nNext);
             }
             else if (scoreInner >= scoreLeaf)
             {
@@ -667,12 +705,10 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     if constexpr (RING > 0)
                     {
                         // the push runs with few of 32 lanes: only the spill of a full ring stays a branch,
-                        // the two ring stores are predicated
+                        // the ring store is predicated
                         const bool push = (dstFar * cs - cb) < bestDst && stackCount < WAVE_STACK;
-                        if (push && stackCount - stackSpilled == RING)
-                        { NodeRef sp_; const int r_ = (stackSpilled & (RING - 1)) * 64; sp_.start = ring[r_ + (int)lane]; sp_.count = ring[r_ + 32 + (int)lane]; stack[stackSpilled++] = sp_; }
-                        const int w_ = (stackCount & (RING - 1)) * 64;
-                        if (push) { ring[w_ + (int)lane] = farRef.start; ring[w_ + 32 + (int)lane] = farRef.count; }
+                        if (push && stackCount - stackSpilled == RING) { const int2 sp_ = RT_RING(stackSpilled); stack[stackSpilled++] = node_ref(sp_); }
+                        if (push) RT_RING(stackCount) = make_int2(farRef.start, farRef.count);
                         stackCount += push ? 1 : 0;
                     }
                     else
@@ -688,8 +724,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     {
                         const bool goNear = (dstNear * cs - cb) < bestDst;
                         const bool ringHas = stackCount > stackSpilled;
-                        const int w_ = ((stackCount - 1) & (RING - 1)) * 64;
-                        NodeRef top; top.start = ring[w_ + (int)lane]; top.count = ring[w_ + 32 + (int)lane];
+                        NodeRef top = node_ref(RT_RING(stackCount - 1));
                         if (!goNear && !ringHas && stackCount > 0) { top = stack[stackSpilled - 1]; --stackSpilled; }      // rare: the ring ran empty above spilled entries
                         const bool pop = !goNear && stackCount > 0;
                         cur = goNear ? nearRef : top;
@@ -707,6 +742,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     else mode = T_NEXT;
                     }
                 }
+                RT_CK(CK_INNER, nInner);
             }
             else
             {
@@ -728,7 +764,12 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     if (RaySphereCore(lpos, ldir, make_f3(s0.x, s0.y, s0.z), s1.x, dst, inside))
                     {
                         const int orig = __float_as_int(s1.z);
-                        if (dst < bestDst || (dst == bestDst && orig < bestTri)) { bestDst = dst; bestTri = orig; bestDet = inside ? -1.0f : 1.0f; bestU = s1.y; }
+                        if (dst < bestDst || (dst == bestDst && orig < bestTri))
+                        {
+                            bestDst = dst; bestTri = orig;
+                            hitKind = __float_as_int(s1.y) == RT_MATERIAL_GLASS ? PS_HIT_GLASS : PS_HIT_OPAQUE;
+                            pool.set_sphere_hit(myEntry, dst, orig, inside);
+                        }
                     }
                     leafK++;
                     if (leafK >= cur.count)
@@ -746,7 +787,11 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                     const bool didHit = RayTriangleCore(lpos, ldir, make_f3(g0.x, g0.y, g0.z), make_f3(g0.w, g1.x, g1.y), make_f3(g1.z, g1.w, g2.x),
                                                         make_f3(g2.y, g2.z, g2.w), cull, dst, u, v, det);
                     if (STATS) cnt.tri++;
-                    if (didHit && dst < bestDst) { bestDst = dst; bestTri = cur.start + leafK; bestU = u; bestV = v; bestDet = det; }
+                    if (didHit && dst < bestDst)
+                    {
+                        bestDst = dst; hitKind = cull ? PS_HIT_OPAQUE : PS_HIT_GLASS;   // cull == (flag != GLASS)
+                        pool.set_hit(myEntry, dst, cur.start + leafK, u, v, det, model);
+                    }
                     leafK++;
                     if (leafK >= cur.count)
                     {
@@ -754,10 +799,12 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         else mode = T_NEXT;
                     }
                 }
+                RT_CK(CK_LEAF, nLeaf);
             }
         }
         __syncwarp();
     }
+    RT_CK_FLUSH();
 
     // ---- counters ---------------------------------------------------------------------------------------------------------------
     const unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
@@ -802,7 +849,8 @@ __global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_tlas_frames(c
 template <int M> inline size_t pool_smem_bytes(const DevParams& P)
 {
     const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
-    return sizeof(WaveSmemHeader) + (size_t)P.smemPairs * sizeof(NodePair) + (size_t)nS * sizeof(DevSphere) + (size_t)POOL_WARPS * (POOL_HOT_WORDS * M * 4 + M) + (size_t)POOL_THREADS * PoolRing<M>::N * 8;
+    return sizeof(WaveSmemHeader) + (size_t)P.smemPairs * sizeof(NodePair) + (size_t)nS * sizeof(DevSphere) + (size_t)POOL_WARPS * (POOL_HOT_WORDS * M * 4 + M) + (size_t)POOL_THREADS * PoolRing<M>::N * 8
+         + (size_t)POOL_WARPS * POOL_CLOCK_BYTES;
 }
 
 template <int M> inline cudaError_t pool_configure_one()
@@ -832,7 +880,8 @@ inline int pool_max_smem_pairs(int M, int sphereCount)
 {
     const int nS = sphereCount < WAVE_MAX_SMEM_SPHERES ? sphereCount : WAVE_MAX_SMEM_SPHERES;
     const long long left = 227LL * 1024 - (long long)sizeof(WaveSmemHeader) - (long long)nS * (long long)sizeof(DevSphere)
-                         - (long long)POOL_WARPS * (POOL_HOT_WORDS * M * 4 + M) - (long long)POOL_THREADS * (M >= 96 && !POOL_COLD_WORDS ? 0 : RT_RING_DEFAULT) * 8 - 1024;
+                         - (long long)POOL_WARPS * (POOL_HOT_WORDS * M * 4 + M) - (long long)POOL_THREADS * (M >= 96 && !POOL_COLD_WORDS ? 0 : RT_RING_DEFAULT) * 8
+                         - (long long)POOL_WARPS * POOL_CLOCK_BYTES - 1024;
     return left <= 0 ? 0 : (int)(left / (long long)sizeof(NodePair));
 }
 

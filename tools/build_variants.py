@@ -73,6 +73,8 @@ VARIANTS = {
     "pw28_c": ("RT_POOL_WARPS=28", "RT_VOTE_WL=3", "RT_VOTE_WN=2", "RT_LEAF_REPEAT=2", "RT_SPHERE_SAH_DEPTH=14"),
     "pw32_c": ("RT_POOL_WARPS=32", "RT_VOTE_WL=3", "RT_VOTE_WN=2", "RT_LEAF_REPEAT=2", "RT_SPHERE_SAH_DEPTH=14"),
     "all_mesh": ("RT_TREELET_PREFETCH", "RT_STACK_TOP_REG", "RT_TRI_LOAD_POLICY=1", "RT_LEAF_REPEAT=2"),
+    # the pooled kernel's cycle account per step kind (tools/pool_clocks.py)
+    "clocks": ("RT_POOL_CLOCKS",),
 }
 OUT_DIR = os.path.join(build.PKG_DIR, "variants")
 
