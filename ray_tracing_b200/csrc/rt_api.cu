@@ -1608,6 +1608,38 @@ int rtxPlanTlas(const float* boxes, int modelCount, void* pairsOut, int pairCap,
     return (int)out.size();
 }
 
+/* Device-free test hook: the sphere accelerator's tree the upload would build over n spheres (4 floats each: centre xyz, radius) for
+ * ray origins in originBox (min xyz, max xyz).  Outputs as rtxPlanTlas; leavesOut holds n sphere indices. */
+int rtxPlanSpheres(const float* spheres, int n, const float* originBox, void* pairsOut, int pairCap, int* leavesOut, int* rootOut)
+{
+    if (!spheres || n < 1 || !originBox || !pairsOut || !leavesOut || !rootOut) return RT_E_INVALID;
+    std::vector<RtSphere> sp(n);
+    for (int i = 0; i < n; i++)
+    {
+        memset(&sp[i], 0, sizeof(RtSphere));
+        for (int a = 0; a < 3; a++) sp[i].centre[a] = spheres[4 * i + a];
+        sp[i].radius = spheres[4 * i + 3];
+    }
+    std::vector<NodePair> out; std::vector<int> order;
+    RepackState::planSpheres(sp.data(), (size_t)n, originBox, originBox + 3, order, out, rootOut[0], rootOut[1]);
+    if ((int)out.size() > pairCap) return RT_E_INVALID;
+    if (!out.empty()) memcpy(pairsOut, out.data(), out.size() * sizeof(NodePair));
+    memcpy(leavesOut, order.data(), order.size() * sizeof(int));
+    return (int)out.size();
+}
+
+/* Device-free test hook: for a tree over n items (which = 0: the sphere accelerator, 1: the TLAS), the surface-area levels the host
+ * builds, the most stack entries a walk of that tree can need (SplitTreeStackBound) and the entries the device walk keeps. */
+int rtxTreeStackLimits(int which, long long n, int* sahDepthOut, int* boundOut, int* stackOut)
+{
+    if (n < 1 || !sahDepthOut || !boundOut || !stackOut) return RT_E_INVALID;
+    if (which == 0) { *sahDepthOut = RepackState::sphereSahDepth(n); *stackOut = RT_SPHERE_STACK; }
+    else if (which == 1 && n <= RT_TLAS_MAX_MODELS) { *sahDepthOut = RT_TLAS_SAH_DEPTH; *stackOut = RT_TLAS_STACK; }
+    else return RT_E_INVALID;
+    *boundOut = SplitTreeStackBound(n, *sahDepthOut);
+    return RT_OK;
+}
+
 static int one_rtGetStats(RtContext* c, RtStats* out);
 int rtGetStats(RtContext* c, RtStats* out)
 {

@@ -426,11 +426,15 @@ RT_DI bool RaySphereCore(f3 rayPos, f3 rayDir, f3 centre, float r2, float& dst, 
 //     a computed hit point always lies inside its sphere's box;
 //   * a box is skipped only if its entry distance, reduced by a relative 2^-18 and an absolute 1e-6, still exceeds the best
 //     dst so far (strictly), so equal-distance candidates with a smaller index are never lost.
+// The walk keeps RT_SPHERE_STACK entries; the host limits the tree's depth to fit (sphereSahDepth, rt_repack.cuh), so the guard on
+// the push below never drops an entry.
+constexpr int RT_SPHERE_STACK = 48;
+
 RT_DNI void TraverseSpheres(const DevParams& P, f3 rayPos, f3 rayDir, float& bestDst, int& bestIndex, bool& bestInside, int& bestFlag,
                            Counters& cnt, bool countStats)
 {
     const f3 invDir = rcp3(rayDir);
-    int2 stack[48];
+    int2 stack[RT_SPHERE_STACK];
     int stackCount = 0;
     int2 cur = make_int2(P.sphRootStart, P.sphRootCount);
     for (;;)
@@ -467,7 +471,7 @@ RT_DNI void TraverseSpheres(const DevParams& P, f3 rayPos, f3 rayDir, float& bes
             const float dNear = nearA ? dA : dB, dFar = nearA ? dB : dA;
             const int2 a = make_int2(__float_as_int(q1.z), __float_as_int(q1.w)), b = make_int2(__float_as_int(q3.z), __float_as_int(q3.w));
             const int2 nearRef = nearA ? a : b, farRef = nearA ? b : a;
-            if (dFar < inf32() && (dFar * 0.99999619f - 1e-6f) <= bestDst && stackCount < 48) stack[stackCount++] = farRef;
+            if (dFar < inf32() && (dFar * 0.99999619f - 1e-6f) <= bestDst && stackCount < RT_SPHERE_STACK) stack[stackCount++] = farRef;
             if (dNear < inf32() && (dNear * 0.99999619f - 1e-6f) <= bestDst) cur = nearRef;
             else { if (stackCount == 0) return; cur = stack[--stackCount]; }
         }

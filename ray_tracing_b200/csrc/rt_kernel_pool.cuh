@@ -78,12 +78,14 @@ template <int M> struct PoolRing { static constexpr int N = 0; };
 // entries [stackSpilled, stackCount) are in the ring at index (i & (RING - 1)); entries [0, stackSpilled) in the local array.
 // A ring entry is one int2 (start, count) per lane: entry i of the warp is 32 x 8 bytes, one conflict-free 64-bit access per push / pop.
 // `ringLane` (this lane's word of entry 0) is computed once per kernel, so an access is that base plus (i & (RING - 1)) * 256 bytes.
+// (RT_PROF 28 / 29 of the profile build count spills of the ring's oldest entry and pops that reload an entry from the local array;
+// 30 the reloads of the inner step's branchless pop among them.)
 #define RT_RING(i) ringLane[((i) & (RING - 1)) * 32]
 #define RT_PUSH(x) do { if constexpr (RING > 0) { \
-                            if (stackCount - stackSpilled == RING) { const int2 sp_ = RT_RING(stackSpilled); stack[stackSpilled++] = node_ref(sp_); } \
+                            if (stackCount - stackSpilled == RING) { const int2 sp_ = RT_RING(stackSpilled); stack[stackSpilled++] = node_ref(sp_); RT_PROF(28, 1); } \
                             const NodeRef px_ = (x); RT_RING(stackCount) = make_int2(px_.start, px_.count); stackCount++; } \
                         else { stack[stackCount++] = (x); } } while (0)
-#define RT_POP(dst) do { if constexpr (RING > 0) { --stackCount; if (stackCount < stackSpilled) { (dst) = stack[--stackSpilled]; } \
+#define RT_POP(dst) do { if constexpr (RING > 0) { --stackCount; if (stackCount < stackSpilled) { (dst) = stack[--stackSpilled]; RT_PROF(29, 1); } \
                              else { (dst) = node_ref(RT_RING(stackCount)); } } \
                          else { (dst) = stack[--stackCount]; } } while (0)
 #endif
@@ -707,9 +709,10 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         // the push runs with few of 32 lanes: only the spill of a full ring stays a branch,
                         // the ring store is predicated
                         const bool push = (dstFar * cs - cb) < bestDst && stackCount < WAVE_STACK;
-                        if (push && stackCount - stackSpilled == RING) { const int2 sp_ = RT_RING(stackSpilled); stack[stackSpilled++] = node_ref(sp_); }
+                        if (push && stackCount - stackSpilled == RING) { const int2 sp_ = RT_RING(stackSpilled); stack[stackSpilled++] = node_ref(sp_); RT_PROF(28, 1); }
                         if (push) RT_RING(stackCount) = make_int2(farRef.start, farRef.count);
                         stackCount += push ? 1 : 0;
+                        if (push) { RT_PROF(11, 1); RT_PROF(32 + (stackCount < 31 ? stackCount : 31), 1); }
                     }
                     else
 #endif
@@ -725,7 +728,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         const bool goNear = (dstNear * cs - cb) < bestDst;
                         const bool ringHas = stackCount > stackSpilled;
                         NodeRef top = node_ref(RT_RING(stackCount - 1));
-                        if (!goNear && !ringHas && stackCount > 0) { top = stack[stackSpilled - 1]; --stackSpilled; }      // rare: the ring ran empty above spilled entries
+                        if (!goNear && !ringHas && stackCount > 0) { top = stack[stackSpilled - 1]; --stackSpilled; RT_PROF(29, 1); RT_PROF(30, 1); }      // rare: the ring ran empty above spilled entries
                         const bool pop = !goNear && stackCount > 0;
                         cur = goNear ? nearRef : top;
                         stackCount -= pop ? 1 : 0;

@@ -171,6 +171,15 @@ inline void BuildMedianSplitPairs(const std::vector<float>& lo, const std::vecto
     }
 }
 
+// The most entries a stack walk of a BuildMedianSplitPairs tree over n items can hold (one per inner node above a leaf, rounded up):
+// sahDepth + ceil(log2 n) + 1.
+constexpr int SplitTreeStackBound(long long n, int sahDepth)
+{
+    int lg = 0;
+    while (lg < 62 && (1LL << lg) < n) lg++;
+    return sahDepth + lg + 1;
+}
+
 #ifndef RT_ORIGIN_PAD_SCALE
 #define RT_ORIGIN_PAD_SCALE 2e-5      // of the largest coordinate R a ray origin can have (~170 ulp(R)); see buildModels.  Measured on the interpreter
                                       // build: 144 differing values with 0, none with 1e-7 (about 1 ulp) and above; the error estimate is <= 40 ulp(R)
@@ -429,7 +438,8 @@ struct RepackState
 #ifndef RT_TLAS_SAH_DEPTH
 #define RT_TLAS_SAH_DEPTH 10                                         // levels split by the surface-area heuristic; below: median (depth <= 10 + 11 < RT_TLAS_STACK)
 #endif
-    static constexpr int TLAS_AUTO_THRESHOLD = 128;                  // below it the linear test of every model box is cheaper than the TLAS walk
+    static_assert(SplitTreeStackBound(RT_TLAS_MAX_MODELS, RT_TLAS_SAH_DEPTH) <= RT_TLAS_STACK, "the TLAS walk's stack must hold the deepest TLAS");
+    static constexpr int TLAS_AUTO_THRESHOLD = 128;                 // below it the linear test of every model box is cheaper than the TLAS walk
 
     // mode: 0 = off, 1 = on whenever it is possible, -1 = automatic (more than TLAS_AUTO_THRESHOLD models)
     static bool tlasWanted(int mode, int modelCount)
@@ -588,6 +598,27 @@ struct RepackState
 #define RT_SPHERE_SAH_DEPTH 0                                        // top levels of the sphere tree by the surface-area sweep (see BuildMedianSplitPairs; 20 by default since round 2, rt_devmath.cuh); 0 = the measured median tree
 #endif
 
+    // Levels of the sphere tree split by the surface-area sweep for n spheres: RT_SPHERE_SAH_DEPTH, fewer where the deepest tree would
+    // not fit TraverseSpheres' stack (beyond 2^27 spheres; a push that does not fit would lose a subtree).
+    static int sphereSahDepth(long long n)
+    {
+        const int room = RT_SPHERE_STACK - SplitTreeStackBound(n, 0);
+        return room < RT_SPHERE_SAH_DEPTH ? (room > 0 ? room : 0) : RT_SPHERE_SAH_DEPTH;
+    }
+
+    // Host only (no CUDA call): the accelerator's tree over the padded boxes of n spheres; order = sphere indices in leaf order.
+    static void planSpheres(const RtSphere* sp, size_t n, const float originLo[3], const float originHi[3], std::vector<int>& order,
+                            std::vector<NodePair>& pairsOut, int& rootStart, int& rootCount)
+    {
+        std::vector<float> lo(3 * n), hi(3 * n), cen(3 * n);
+        for (size_t i = 0; i < n; i++)
+        {
+            paddedSphereBox(sp[i].centre, sp[i].radius, originLo, originHi, &lo[3 * i], &hi[3 * i]);
+            for (int a = 0; a < 3; a++) cen[3 * i + a] = sp[i].centre[a];
+        }
+        BuildMedianSplitPairs(lo, hi, cen, n, RT_SPHERE_LEAF, order, pairsOut, rootStart, rootCount, sphereSahDepth((long long)n));
+    }
+
     bool sphereBoundCovers(const float lo[3], const float hi[3]) const
     {
         for (int a = 0; a < 3; a++) if (lo[a] < sphBoundLo[a] || hi[a] > sphBoundHi[a]) return false;
@@ -620,16 +651,10 @@ struct RepackState
         // padding of sphere i: paddedSphereBox
         for (int a = 0; a < 3; a++) { sphBoundLo[a] = originLo[a]; sphBoundHi[a] = originHi[a]; }
         const size_t n = sp.size();
-        std::vector<float> lo(3 * n), hi(3 * n), cen(3 * n);
-        for (size_t i = 0; i < n; i++)
-        {
-            paddedSphereBox(sp[i].centre, sp[i].radius, originLo, originHi, &lo[3 * i], &hi[3 * i]);
-            for (int a = 0; a < 3; a++) cen[3 * i + a] = sp[i].centre[a];
-        }
-        // median split on the widest centroid axis, leaves of <= 4 spheres; pairs emitted parent-before-children
+        // surface-area splits at the top, median splits below, leaves of RT_SPHERE_LEAF spheres; pairs emitted parent-before-children
         std::vector<int> order;
         std::vector<NodePair> pairsOut;
-        BuildMedianSplitPairs(lo, hi, cen, n, RT_SPHERE_LEAF, order, pairsOut, sphRootStart, sphRootCount, RT_SPHERE_SAH_DEPTH);
+        planSpheres(sp.data(), n, originLo, originHi, order, pairsOut, sphRootStart, sphRootCount);
         std::vector<DevSphere> leaves(n);
         for (size_t k = 0; k < n; k++) leaves[k] = out[order[k]];
         if ((e = sphPairs.ensure(std::max<size_t>(pairsOut.size(), 1))) != cudaSuccess) return e;
