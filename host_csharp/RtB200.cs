@@ -75,6 +75,14 @@ public static class RtB200
     public struct PathRadiance { public UnityEngine.Vector3 rgb; public uint rngState; }
     [DllImport(Lib)] public static extern int rtTracePaths(IntPtr ctx, PathRay[] rays, int n, int samples, [Out] PathRadiance[] output);
     [DllImport(Lib)] public static extern int rtTracePathsDevice(IntPtr ctx, IntPtr dRays, IntPtr dOut, int n, int samples);
+    // one pixel of "FeatureFrame": object = ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1 (dst = +inf, the rest 0)
+    [StructLayout(LayoutKind.Sequential)]
+    public struct PixelFeatures { public UnityEngine.Vector3 albedo; public float dst; public UnityEngine.Vector3 normal; public int objectId; }
+    // first-hit feature images (denoiser guides) of every pixel's own camera ray, and those rays (W*H PathRay, [y][x], bytes = W*H*28)
+    [DllImport(Lib)] public static extern int rtDispatchFeatures(IntPtr ctx, int groupsX, int groupsY, int groupsZ);
+    [DllImport(Lib)] public static extern int rtCameraRays(IntPtr ctx, [Out] PathRay[] rays, UIntPtr bytes);
+    [DllImport(Lib)] public static extern int rtCameraRaysDevice(IntPtr ctx, IntPtr dRays, UIntPtr bytes);
+    [DllImport(Lib, EntryPoint = "rtReadback")] public static extern int rtReadbackFeatures(IntPtr ctx, string tex, [Out] PixelFeatures[] dst, UIntPtr bytes);   // tex = "FeatureFrame", bytes = W*H*32
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

@@ -188,10 +188,74 @@ int rtTraceOcclusionDevice(RtContext* ctx, const void* dSegs, void* dOccluded, i
 int rtTracePaths(RtContext* ctx, const RtPathRay* rays, int n, int samples, RtPathRadiance* out);
 int rtTracePathsDevice(RtContext* ctx, const void* dRays, void* dOut, int n, int samples);
 
+/* Extension: first-hit feature images for denoisers (albedo, shading normal, depth, object id: the guides OIDN, a-trous / SVGF filters
+ * and mattes take next to the colour), and the camera's own rays.
+ *
+ * The FEATURE RAY of pixel (x, y) is the ray RayTrace starts that pixel's first path of the current frame with: the per-pixel setup
+ * for thread id (x, y) under the current "Resolution", "CamLocalToWorldMatrix", "ViewParams", "Frame" and "renderSeed" (RC:15,
+ * HL:547-558: uv = id / (Resolution - 1), the pixel index recomputed from uv as there, rngState = pixelIndex + Frame * 719393 +
+ * renderSeed modulo 2^32), then ONE camera sample (HL:567-576: four draws, the defocus disc by "DefocusStrength", the jitter by
+ * "DivergeStrength", the normalised direction).  With "NumRaysPerPixel" = 1 it is exactly the ray the frame's path started with, so the
+ * guides are anti-aliased and defocused like the colour.  With more samples per pixel it is the FIRST sample's ray only: a later sample
+ * starts from the RNG state the whole path before it left behind (one chain per pixel, HL:563-579), which only tracing those paths
+ * can produce.
+ *
+ * rtCameraRays / rtCameraRaysDevice write, for every pixel of the image, W*H RtPathRay in [y][x] order (row 0 = bottom): the feature
+ * ray's origin and direction and the RNG state after its four draws: what rtTracePaths takes (rtTracePaths(rays, samples = 1).rgb is
+ * FrameRender.rgb of a 1-sample rtDispatch of this frame, bit for bit) and what rtTraceRays takes in its first 24 bytes.
+ *   - A query about the camera, not a render: partial dispatch and rtSetTile do not apply; no scene is needed; nothing the context
+ *     exposes changes (no image, no RtStats field).
+ *   - Refused: ctx NULL, rays NULL, bytes != W*H*28, a device pointer not 4-byte aligned -> RT_E_INVALID; before rtResize, "Resolution"
+ *     different from the render textures or above 65535, a member context of a group other than the one rtCreateMulti returned ->
+ *     RT_E_STATE.
+ *   - rtCameraRays: host memory, through a device buffer of W*H*28 bytes the context keeps for later calls (freed by rtDestroy and by
+ *     rtResize to a new size); synchronises.  rtCameraRaysDevice: device memory of the context's device, no allocation; asynchronous
+ *     on the context's stream (rtSetStream).
+ *
+ * rtDispatchFeatures covers the pixels rtDispatch(RT_KERNEL_RAYTRACE, groupsX, groupsY, groupsZ) would cover (8x8 groups, partial
+ * dispatch, this context's rtSetTile row bands) and touches no other.  For each, hit = CalculateRayCollision(feature ray,
+ * forceDontCullBack = false) (HL:335-374, HL:487; the sphere extension first: rtTraceRays' hit of that ray with flags 0) and the
+ * pixel's RtPixelFeatures record (rt_types.h) in the device image "FeatureFrame" (W*H records, [y][x], row 0 = bottom) becomes
+ *     miss:                   albedo (0, 0, 0), dst +inf, normal (0, 0, 0), object -1
+ *     hit:                    dst = hit.dst, normal = hit.normal, object = m for ModelInfo[m], -2 - s for Spheres[s]
+ *       material.flag == 2:   albedo (1, 1, 1)       (glass: the usual convention for a transmissive surface)
+ *       any other material:   albedo = GetMaterialColour(material, hit.pos, hit.normal, isSpecularBounce = false) as written at
+ *                             HL:450-466: diffuseCol, or for flag == 1 the checker pattern choosing between diffuseCol and emissionCol,
+ *                             then lerp(col, specularCol, 0) = col + (specularCol - col) * 0 evaluated in binary32 (a non-finite
+ *                             specularCol - col gives NaN, as it does in Trace)
+ * With "accumulate" != 0 a HIT is also added into two float4 images, one binary32 addition per component:
+ *     AccumulatedAlbedo[pixel] += (albedo.r, albedo.g, albedo.b, 1)        AccumulatedNormal[pixel] += (normal.x, normal.y, normal.z, dst)
+ * and a miss changes neither.  So AccumulatedAlbedo.w counts the feature rays that hit, AccumulatedNormal.w / AccumulatedAlbedo.w is
+ * the mean depth over hits, AccumulatedNormal.xyz / AccumulatedAlbedo.w the mean normal, and AccumulatedAlbedo.rgb /
+ * numAccumulatedFrames the anti-aliased albedo (a miss counts as black).  With "accumulate" = 0 only FeatureFrame is written.
+ *   - The three images are allocated, zero-filled, by the first rtDispatchFeatures (even one that covers no pixel).  rtResize to a new
+ *     size zeroes all three.  rtDispatch(RT_KERNEL_RESET_ACCUMULATED, gx, gy, gz) also zeroes the region it covers in both accumulators,
+ *     if they exist, and leaves FeatureFrame: a host that resets its colour accumulation resets its guides with the same call.  A context
+ *     that never calls rtDispatchFeatures allocates nothing and behaves as before.
+ *   - Reads the scene buffers, "modelCount", the camera uniforms, "Frame", "renderSeed", "accumulate" and "Resolution".  Does not read
+ *     "NumRaysPerPixel", "MaxBounceCount" or the sky.  Leaves FrameRender, AccumulatedRender, PixelStats, "Frame", RtStats.dispatches and
+ *     kernelMs alone and does not change what later dispatches render.  Call it before or after the frame's rtDispatch, with the same
+ *     "Frame"; it does not advance anything.
+ *   - RtStats.rays grows by the pixels traced.  With "countStats" = 1 the box / triangle / sphere counters grow as a counting
+ *     dispatch's first segments do (every model walked).
+ *   - Model skipping, the TLAS and the sphere accelerator are used as for the camera rays of rtDispatch (which these are), with the
+ *     same preparation and the open grazing-ray defect of model skipping (DESIGN.md section 5); "modelSkip" = 0 avoids it.
+ *   - Reading: rtReadback and rtGetDevicePointer accept "FeatureFrame" (bytes = W*H*32), "AccumulatedAlbedo" and "AccumulatedNormal"
+ *     (W*H*16); RT_E_STATE before the first rtDispatchFeatures.  rtReadbackAsync serves the two colour images only.
+ *   - Refused: ctx NULL, a negative group count -> RT_E_INVALID; before rtResize, "Resolution" different from the render textures or
+ *     above 65535, the scene checks of rtDispatch (modelCount beyond ModelInfo, models without Nodes / Triangles, an offset out of range,
+ *     a tree deeper than 63 inner levels), and any context of a group (rtCreateMulti: the tile exchange carries the two colour images
+ *     only) -> RT_E_STATE.  A single context with rtSetTile works and writes only its bands.
+ * Asynchronous on the context's stream. */
+int rtDispatchFeatures(RtContext* ctx, int groupsX, int groupsY, int groupsZ);
+int rtCameraRays(RtContext* ctx, RtPathRay* rays, size_t bytes);
+int rtCameraRaysDevice(RtContext* ctx, void* dRays, size_t bytes);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),
- * bytes must equal W·H·16.  Synchronises. */
+ * bytes must equal W·H·16.  After the first rtDispatchFeatures also "AccumulatedAlbedo",
+ * "AccumulatedNormal" (float4 as well) and "FeatureFrame" (W·H RtPixelFeatures: bytes must equal W·H·32).  Synchronises. */
 int rtReadback(RtContext* ctx, const char* tex, float* dst, size_t bytes);
 
 /* Replaces: RayTraceDisplay.OnRenderImage -> Graphics.Blit(rt, destination, displayMat) with Display.shader
@@ -272,7 +336,7 @@ int rtCommDestroy(RtContext* ctx);
 int rtExchangeTiles(RtContext* ctx);
 
 /* Device address + size of a named device object, for zero-copy plumbing (NCCL, torch views).
- * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv","PixelStats"}. */
+ * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv","PixelStats","FeatureFrame","AccumulatedAlbedo","AccumulatedNormal"}. */
 int rtGetDevicePointer(RtContext* ctx, const char* name, void** devPtr, size_t* bytes);
 
 /* Replaces `new BVH(mesh.vertices, mesh.triangles, mesh.normals, quality)` (BVH.cs:26; called once per shared mesh from

@@ -115,6 +115,14 @@ typedef struct RtPathRadiance {
     uint32_t rngState;     /* the state after the last sample: a caller continues the chain with it */
 } RtPathRadiance;
 
+/* One pixel of rtDispatchFeatures' "FeatureFrame" (include/rt_b200.h): what the pixel's feature ray hits first.  32 bytes. */
+typedef struct RtPixelFeatures {
+    float   albedo[3];    /* (0, 0, 0) on a miss; (1, 1, 1) for glass; GetMaterialColour (HL:450-466) otherwise */
+    float   dst;          /* RtRayHit.dst of the feature ray; +inf on a miss */
+    float   normal[3];    /* RtRayHit.normal; 0 on a miss */
+    int32_t object;       /* ModelInfo index m -> m;  Spheres index s -> -2 - s;  miss -> -1 */
+} RtPixelFeatures;
+
 #pragma pack(pop)
 
 #ifdef __cplusplus
@@ -125,6 +133,7 @@ static_assert(sizeof(RtRayHit) == 48, "RtRayHit record");
 static_assert(sizeof(RtRaySegment) == 28, "RtRaySegment record");
 static_assert(sizeof(RtPathRay) == 28, "RtPathRay record");
 static_assert(sizeof(RtPathRadiance) == 16, "RtPathRadiance record");
+static_assert(sizeof(RtPixelFeatures) == 32, "RtPixelFeatures record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

@@ -119,6 +119,12 @@ def make_path_rays(origins, dirs=None, rng_state=None) -> np.ndarray:
     return rays
 
 
+# rtDispatchFeatures: one pixel of "FeatureFrame" (RtPixelFeatures).  object: ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1
+PIXEL_FEATURES_DTYPE = np.dtype([("albedo", "<f4", 3), ("dst", "<f4"), ("normal", "<f4", 3), ("object", "<i4")])
+assert PIXEL_FEATURES_DTYPE.itemsize == 32
+FEATURE_IMAGES = ("FeatureFrame", "AccumulatedAlbedo", "AccumulatedNormal")
+
+
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
                 ("dispatches", C.c_uint64), ("kernelMs", C.c_double), ("sphereBoxTests", C.c_uint64), ("exchangeMs", C.c_double)]
@@ -186,12 +192,16 @@ class RtLib:
             "rtTraceOcclusionDevice": ([vp, vp, vp, ci, ci], ci),
             "rtTracePaths": ([vp, vp, ci, ci, vp], ci),
             "rtTracePathsDevice": ([vp, vp, vp, ci, ci], ci),
+            "rtDispatchFeatures": ([vp, ci, ci, ci], ci),
+            "rtCameraRays": ([vp, vp, C.c_size_t], ci),
+            "rtCameraRaysDevice": ([vp, vp, C.c_size_t], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
-                            "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice"):      # absent from older experimental builds used in A/B runs
+                            "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
+                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -345,9 +355,30 @@ class RtContext:
         memory of the context's GPU (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtTracePathsDevice(self._h, C.c_void_p(rays_ptr), C.c_void_p(out_ptr), int(n), int(samples)))
 
+    def dispatch_features(self, gx: Optional[int] = None, gy: Optional[int] = None, gz: int = 1):
+        """rtDispatchFeatures: the first-hit feature images (albedo, dst, normal, object id) of every pixel's own camera ray of the
+        current "Frame", into "FeatureFrame" and, with "accumulate", the two accumulators.  Groups default to the whole image.  Read
+        with readback("FeatureFrame") -> (H, W) PIXEL_FEATURES_DTYPE, readback("AccumulatedAlbedo" / "AccumulatedNormal")."""
+        gx = (self.width + 7) // 8 if gx is None else gx
+        gy = (self.height + 7) // 8 if gy is None else gy
+        self._ck(self._L.rtDispatchFeatures(self._h, int(gx), int(gy), int(gz)))
+
+    def camera_rays(self) -> np.ndarray:
+        """rtCameraRays: (H, W) PATH_RAY_DTYPE, row 0 = bottom: every pixel's jittered camera ray for the current "Frame" / "renderSeed"
+        and the RNG state after its four draws: what trace_paths takes, and trace_rays in origin / dir."""
+        out = np.empty((self.height, self.width), dtype=PATH_RAY_DTYPE)
+        self._ck(self._L.rtCameraRays(self._h, out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out
+
+    def camera_rays_device(self, rays_ptr: int, nbytes: int):
+        """rtCameraRaysDevice: the same W*H RtPathRay into device memory of the context's GPU (4-byte aligned, nbytes = W*H*28).
+        Asynchronous on the context's stream (set_stream)."""
+        self._ck(self._L.rtCameraRaysDevice(self._h, C.c_void_p(rays_ptr), int(nbytes)))
+
     def readback(self, tex: str, out: Optional[np.ndarray] = None) -> np.ndarray:
         if out is None:
-            out = np.empty((self.height, self.width, 4), dtype=np.float32)
+            out = (np.empty((self.height, self.width), dtype=PIXEL_FEATURES_DTYPE) if tex == "FeatureFrame" else
+                   np.empty((self.height, self.width, 4), dtype=np.float32))
         self._ck(self._L.rtReadback(self._h, tex.encode(), out.ctypes.data_as(C.c_void_p), out.nbytes))
         return out
 

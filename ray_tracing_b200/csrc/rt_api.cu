@@ -10,6 +10,7 @@
 #include "rt_kernel_wave.cuh"
 #include "rt_kernel_pool.cuh"
 #include "rt_kernel_query.cuh"
+#include "rt_kernel_features.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -103,6 +104,9 @@ struct RtContext
     DevBuf<RtRay> queryRays; DevBuf<RtRayHit> queryHits;     // rtTraceRays: device copies of one batch (<= RT_TRACE_CHUNK_RAYS) of the caller's host arrays
                                                              // (rtTraceOcclusion: its segments in queryHits, its bytes in queryRays;
                                                              //  rtTracePaths: its RtPathRay in queryHits, its RtPathRadiance in queryRays)
+    // rtDispatchFeatures: "FeatureFrame", "AccumulatedAlbedo", "AccumulatedNormal" (W*H each, allocated by the first call);
+    // rtCameraRays: the device copy of the image's rays (host form only)
+    DevBuf<RtPixelFeatures> featureFrame; DevBuf<float4> accumAlbedo, accumNormal; DevBuf<RtPathRay> cameraRays;
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -212,6 +216,7 @@ int rtDestroy(RtContext* c)
     for (int k = 0; k < 2; k++) { if (c->stageBuf[k]) cudaFreeHost(c->stageBuf[k]); if (c->stageEv[k]) cudaEventDestroy(c->stageEv[k]); }
     c->frame.release(); c->accum.release(); c->tileSend.release(); c->tileRecv.release(); c->display.release();
     c->pixelStats.release(); c->queryRays.release(); c->queryHits.release();
+    c->featureFrame.release(); c->accumAlbedo.release(); c->accumNormal.release(); c->cameraRays.release();
     c->repack.release();
     closePeers(c);
     for (auto& ev : c->pending) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
@@ -374,6 +379,14 @@ static int one_rtResize(RtContext* c, int w, int h)
             CK(c->pixelStats.ensure(n));
             CK(cudaMemsetAsync(c->pixelStats.p, 0, n * sizeof(RtPixelStats), c->stream));
         }
+        if (c->featureFrame.p)                              // so do the feature images
+        {
+            CK(c->featureFrame.ensure(n)); CK(c->accumAlbedo.ensure(n)); CK(c->accumNormal.ensure(n));
+            CK(cudaMemsetAsync(c->featureFrame.p, 0, n * sizeof(RtPixelFeatures), c->stream));
+            CK(cudaMemsetAsync(c->accumAlbedo.p, 0, n * 16, c->stream));
+            CK(cudaMemsetAsync(c->accumNormal.p, 0, n * 16, c->stream));
+        }
+        c->cameraRays.release();
         c->width = w; c->height = h;
         c->tileSend.release(); c->tileRecv.release();
         closePeers(c);                                      // peer mappings refer to images of the old size
@@ -698,6 +711,11 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     {
         if (limX == 0 || limY == 0) return RT_OK;
         CK(cudaMemset2DAsync(c->accum.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
+        if (c->accumAlbedo.p)                                  // the guides are averaged over the same frames as the colour
+        {
+            CK(cudaMemset2DAsync(c->accumAlbedo.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
+            CK(cudaMemset2DAsync(c->accumNormal.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
+        }
         return RT_OK;
     }
     if (kernelIndex != RT_KERNEL_RAYTRACE) return fail(c, RT_E_INVALID, "rtDispatch: kernelIndex must be 0 (RayTrace) or 1 (ResetAccumulated)");
@@ -800,14 +818,26 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     return RT_OK;
 }
 
+// The feature images exist after the first rtDispatchFeatures, on a single context
+static int featuresReady(RtContext* c, const char* what)
+{
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, std::string(what) + ": the feature images are not available on a group context (rtCreateMulti)");
+    if (!c->featureFrame.p) return fail(c, RT_E_STATE, std::string(what) + ": no rtDispatchFeatures yet");
+    return RT_OK;
+}
+
 int rtReadback(RtContext* c, const char* tex, float* dst, size_t bytes)
 {
     if (!c || !tex || !dst) return fail(c, RT_E_INVALID, "rtReadback: bad argument");
     const std::string n(tex);
-    const float4* src = n == "FrameRender" ? c->frame.p : n == "AccumulatedRender" ? c->accum.p : nullptr;
-    if (n != "FrameRender" && n != "AccumulatedRender") return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
+    const bool feature = n == "FeatureFrame" || n == "AccumulatedAlbedo" || n == "AccumulatedNormal";
+    if (feature) { int rc = featuresReady(c, "rtReadback"); if (rc != RT_OK) return rc; }
+    const void* src = n == "FrameRender" ? (const void*)c->frame.p : n == "AccumulatedRender" ? (const void*)c->accum.p : n == "FeatureFrame" ? (const void*)c->featureFrame.p :
+                      n == "AccumulatedAlbedo" ? (const void*)c->accumAlbedo.p : n == "AccumulatedNormal" ? (const void*)c->accumNormal.p : nullptr;
+    if (n != "FrameRender" && n != "AccumulatedRender" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
     if (!src) return fail(c, RT_E_STATE, "rtReadback: rtResize has not been called");
-    if (bytes != (size_t)c->width * c->height * 16) return fail(c, RT_E_INVALID, "rtReadback: bytes must equal W*H*16");
+    if (bytes != (size_t)c->width * c->height * (n == "FeatureFrame" ? sizeof(RtPixelFeatures) : 16))
+        return fail(c, RT_E_INVALID, n == "FeatureFrame" ? "rtReadback: bytes must equal W*H*32" : "rtReadback: bytes must equal W*H*16");
     CK(cudaSetDevice(c->device));
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
@@ -1225,6 +1255,94 @@ int rtTracePathsDevice(RtContext* c, const void* dRays, void* dOut, int n, int s
     return pathsLocal(c, (const RtPathRay*)dRays, (RtPathRadiance*)dOut, n, samples);
 }
 
+// ---- first-hit feature images and the camera's own rays (rtDispatchFeatures, rtCameraRays, rt_kernel_features.cuh) ---------------------
+// The image a camera call works on: rtResize done, "Resolution" equal to it, within the kernels' coordinate range
+static int cameraImage(RtContext* c, const char* what)
+{
+    if (c->width == 0) return fail(c, RT_E_STATE, std::string(what) + ": rtResize has not been called");
+    if ((int)c->P.W != c->width || (int)c->P.H != c->height) return fail(c, RT_E_STATE, std::string(what) + ": Resolution does not match the render textures");
+    if (c->P.W > 65535u || c->P.H > 65535u) return fail(c, RT_E_STATE, std::string(what) + ": a resolution above 65535 is not supported");
+    return RT_OK;
+}
+
+int rtDispatchFeatures(RtContext* c, int gx, int gy, int gz)
+{
+    if (!c) return RT_E_INVALID;
+    if (gx < 0 || gy < 0 || gz < 0) return fail(c, RT_E_INVALID, "rtDispatchFeatures: bad argument");
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDispatchFeatures: not available on a group context (rtCreateMulti)");
+    int rc = cameraImage(c, "rtDispatchFeatures"); if (rc != RT_OK) return rc;
+    CK(cudaSetDevice(c->device));
+    const unsigned W = c->P.W, H = c->P.H;
+    if (!c->featureFrame.p)                                    // the first call allocates the three images, zero-filled
+    {
+        const size_t n = (size_t)W * H;
+        CK(c->featureFrame.ensure(n)); CK(c->accumAlbedo.ensure(n)); CK(c->accumNormal.ensure(n));
+        CK(cudaMemsetAsync(c->featureFrame.p, 0, n * sizeof(RtPixelFeatures), c->stream));
+        CK(cudaMemsetAsync(c->accumAlbedo.p, 0, n * 16, c->stream));
+        CK(cudaMemsetAsync(c->accumNormal.p, 0, n * 16, c->stream));
+    }
+    unsigned limX = (unsigned long long)gx * 8ull < W ? (unsigned)gx * 8u : W;
+    unsigned limY = (unsigned long long)gy * 8ull < H ? (unsigned)gy * 8u : H;
+    if (gz == 0 || limX == 0 || limY == 0) return RT_OK;
+    if ((rc = prepareQueryScene(c, "rtDispatchFeatures")) != RT_OK) return rc;
+    DevParams P = c->P;
+    bindScene(c, P);
+    P.limX = limX; P.limY = limY;
+    P.tileRank = c->tileRank; P.tileWorld = c->tileWorld; P.bandRows = c->bandRows; P.countStats = c->optCountStats;
+    P.smemPairs = 0; P.zeroDefocus = 0;                        // no tree-top staging: every record from global memory
+    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    FeatureParams F = {};
+    F.features = c->featureFrame.p; F.accumAlbedo = c->accumAlbedo.p; F.accumNormal = c->accumNormal.p;
+    cudaError_t e = features_launch(P, F, c->numSMs, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "rtDispatchFeatures launch");
+    return RT_OK;
+}
+
+// What both forms of rtCameraRays check before anything is allocated or launched
+static int cameraRaysArgs(RtContext* c, const char* what, const void* rays, size_t bytes)
+{
+    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; call it on the context rtCreateMulti returned");
+    if (!rays) return fail(c, RT_E_INVALID, std::string(what) + ": rays is NULL");
+    int rc = cameraImage(c, what); if (rc != RT_OK) return rc;
+    if (bytes != (size_t)c->width * c->height * sizeof(RtPathRay)) return fail(c, RT_E_INVALID, std::string(what) + ": bytes must equal W*H*28");
+    return RT_OK;
+}
+
+// W*H rays of the whole image into device memory; asynchronous on the context's stream
+static int cameraRaysLocal(RtContext* c, RtPathRay* dRays)
+{
+    DevParams P = c->P;
+    P.limX = P.W; P.limY = P.H;
+    P.tileRank = 0; P.tileWorld = 1; P.bandRows = 1;          // the whole image: a query about the camera, not a render
+    P.zeroDefocus = 0;
+    FeatureParams F = {};
+    F.rays = dRays;
+    cudaError_t e = camera_rays_launch(P, F, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "rtCameraRays launch");
+    return RT_OK;
+}
+
+int rtCameraRays(RtContext* c, RtPathRay* rays, size_t bytes)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = cameraRaysArgs(c, "rtCameraRays", rays, bytes); if (rc != RT_OK) return rc;
+    CK(cudaSetDevice(c->device));
+    CK(c->cameraRays.ensure((size_t)c->width * c->height));
+    if ((rc = cameraRaysLocal(c, c->cameraRays.p)) != RT_OK) return rc;
+    if ((rc = stagedD2H(c, rays, c->cameraRays.p, bytes)) != RT_OK) return rc;
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rtCameraRaysDevice(RtContext* c, void* dRays, size_t bytes)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = cameraRaysArgs(c, "rtCameraRaysDevice", dRays, bytes); if (rc != RT_OK) return rc;
+    if ((uintptr_t)dRays & 3u) return fail(c, RT_E_INVALID, "rtCameraRaysDevice: dRays must be 4-byte aligned");
+    CK(cudaSetDevice(c->device));
+    return cameraRaysLocal(c, (RtPathRay*)dRays);
+}
+
 int rtExchangeTiles(RtContext* c)
 {
     if (!c) return RT_E_INVALID;
@@ -1340,6 +1458,13 @@ int rtGetDevicePointer(RtContext* c, const char* name, void** devPtr, size_t* by
     {
         if (!c->pixelStats.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: PixelStats is allocated by the first counting dispatch");
         *devPtr = c->pixelStats.p; *bytes = c->pixelStats.count * sizeof(RtPixelStats);
+    }
+    else if (n == "FeatureFrame" || n == "AccumulatedAlbedo" || n == "AccumulatedNormal")
+    {
+        int rc = featuresReady(c, "rtGetDevicePointer"); if (rc != RT_OK) return rc;
+        if (n == "FeatureFrame") { *devPtr = c->featureFrame.p; *bytes = c->featureFrame.count * sizeof(RtPixelFeatures); }
+        else if (n == "AccumulatedAlbedo") { *devPtr = c->accumAlbedo.p; *bytes = c->accumAlbedo.count * 16; }
+        else { *devPtr = c->accumNormal.p; *bytes = c->accumNormal.count * 16; }
     }
     else if (n == "TileSend" || n == "TileRecv")
     {

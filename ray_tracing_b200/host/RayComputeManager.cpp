@@ -32,6 +32,8 @@ std::string RtApi::Load(const char* path)
     TraceRays = reinterpret_cast<decltype(TraceRays)>(dlsym(dl, "rtTraceRays"));
     TraceOcclusion = reinterpret_cast<decltype(TraceOcclusion)>(dlsym(dl, "rtTraceOcclusion"));
     TracePaths = reinterpret_cast<decltype(TracePaths)>(dlsym(dl, "rtTracePaths"));
+    DispatchFeatures = reinterpret_cast<decltype(DispatchFeatures)>(dlsym(dl, "rtDispatchFeatures"));
+    CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
     return "";
 }
 
@@ -321,6 +323,34 @@ int RayComputeManager::TracePaths(const RtPathRay* rays, int n, int samples, RtP
     int rc;
     if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
     TRY(api.TracePaths(ctx, rays, n, samples, out));
+    return RT_OK;
+}
+
+int RayComputeManager::RenderFeatures()
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.DispatchFeatures) { lastError = "the library does not export rtDispatchFeatures"; return RT_E_STATE; }
+    if (!IsRendering()) return RT_OK;
+    int rc = InitFrame();                        // Frame = numAccumulatedFrames: the frame the next RenderFrame renders
+    if (rc != RT_OK) return rc;
+    TRY(api.DispatchFeatures(ctx, (texWidth + 7) / 8, (texHeight + 7) / 8, 1));
+    return RT_OK;
+}
+
+int RayComputeManager::ReadFeatureImage(const char* name, void* dst, size_t bytes)
+{
+    if (!ctx) return RT_E_STATE;
+    TRY(api.Readback(ctx, name, static_cast<float*>(dst), bytes));
+    return RT_OK;
+}
+
+int RayComputeManager::CameraRays(RtPathRay* rays, size_t bytes)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.CameraRaysFn) { lastError = "the library does not export rtCameraRays"; return RT_E_STATE; }
+    int rc = InitFrame();
+    if (rc != RT_OK) return rc;
+    TRY(api.CameraRaysFn(ctx, rays, bytes));
     return RT_OK;
 }
 

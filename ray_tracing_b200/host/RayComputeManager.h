@@ -60,6 +60,8 @@ struct RtApi
     decltype(&rtTraceRays) TraceRays = nullptr;             // optional: closest-hit queries (TraceRays / Pick)
     decltype(&rtTraceOcclusion) TraceOcclusion = nullptr;   // optional: occlusion queries (TraceOcclusion)
     decltype(&rtTracePaths) TracePaths = nullptr;           // optional: radiance along caller rays (TracePaths)
+    decltype(&rtDispatchFeatures) DispatchFeatures = nullptr;   // optional: first-hit feature images (RenderFeatures)
+    decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -137,6 +139,15 @@ public:
     // not in the reference: the path tracer's radiance along caller-supplied rays, the mean of `samples` paths on each ray's RNG chain
     // (rtTracePaths) — custom cameras, probe baking.  The scene is uploaded first as for TraceRays.
     int TracePaths(const RtPathRay* rays, int n, int samples, RtPathRadiance* out);
+    // not in the reference: the denoiser guides of the frame the NEXT RenderFrame() renders (rtDispatchFeatures over the whole image):
+    // the upload sequence of RenderFrame, Frame = numAccumulatedFrames, and no step of the frame counter.  Call it right before that
+    // RenderFrame; ResetAccumulatedRender resets the accumulated guides with the colour.
+    // ReadFeatureImage: "FeatureFrame" (W*H RtPixelFeatures), "AccumulatedAlbedo" or "AccumulatedNormal" (W*H float4).
+    int RenderFeatures();
+    int ReadFeatureImage(const char* name, void* dst, size_t bytes);
+    // not in the reference: the jittered camera ray of every pixel for that same frame and the RNG state after its four draws
+    // (rtCameraRays; W*H records, [y][x]): what TracePaths and TraceRays take.
+    int CameraRays(RtPathRay* rays, size_t bytes);
     // picking / autofocus: the un-jittered camera ray through pixel (x, y) of the screen — SetupPixel's operations (HL:547-558) on the
     // manager's own camera fields — and its closest hit
     void PickRay(float x, float y, RtRay* ray) const;

@@ -242,6 +242,10 @@ int rcmTraceOcclusion(void* hv, const RtRaySegment* segs, int n, uint8_t* occlud
 
 int rcmTracePaths(void* hv, const RtPathRay* rays, int n, int samples, RtPathRadiance* out)
 { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TracePaths(rays, n, samples, out); } CATCH_ALL(h) }
+
+int rcmRenderFeatures(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFeatures(); } CATCH_ALL(h) }
+int rcmReadFeatureImage(void* hv, const char* name, void* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadFeatureImage(name, dst, bytes); }
+int rcmCameraRays(void* hv, RtPathRay* rays, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->CameraRays(rays, bytes); } CATCH_ALL(h) }
 /* the pick ray through pixel (x, y) into *ray (may be NULL) and its closest hit into *hit (may be NULL: the ray alone) */
 int rcmPick(void* hv, float x, float y, RtRay* ray, RtRayHit* hit)
 {

@@ -66,6 +66,9 @@ def host_lib() -> C.CDLL:
         L.rcmTraceRays.argtypes = [vp, vp, ci, vp, ci]
         L.rcmTraceOcclusion.argtypes = [vp, vp, ci, vp, ci]
         L.rcmTracePaths.argtypes = [vp, vp, ci, ci, vp]
+        L.rcmRenderFeatures.argtypes = [vp]
+        L.rcmReadFeatureImage.argtypes = [vp, cp, vp, C.c_size_t]
+        L.rcmCameraRays.argtypes = [vp, vp, C.c_size_t]
         L.rcmPick.argtypes = [vp, cf, cf, vp, vp]
         _host = L
     return _host
@@ -306,6 +309,43 @@ class RayComputeManager:
         r = capi.make_path_rays(rays)
         out = np.empty(r.shape[0], dtype=capi.PATH_RADIANCE_DTYPE)
         self._ck(self._L.rcmTracePaths(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), int(samples), out.ctypes.data if out.size else None))
+        return out
+
+    # -- denoiser guides (rtDispatchFeatures) and the camera's own rays (rtCameraRays)
+    def RenderFeatures(self):
+        """The first-hit feature images of the frame the NEXT RenderFrame() renders: the upload sequence of RenderFrame, then
+        rtDispatchFeatures over the whole image; the frame counter does not move.  Read them with feature_frame / accumulated_albedo /
+        accumulated_normal; ResetAccumulatedRender resets the two accumulated ones with the colour."""
+        self._ck(self._L.rcmRenderFeatures(self._h))
+
+    def _read_feature(self, name: str, out: np.ndarray) -> np.ndarray:
+        self._ck(self._L.rcmReadFeatureImage(self._h, name.encode(), out.ctypes.data, out.nbytes))
+        return out
+
+    @property
+    def feature_frame(self) -> np.ndarray:
+        """(H, W) array of capi.PIXEL_FEATURES_DTYPE, row 0 = bottom: albedo, dst, normal and object id of each pixel's feature ray."""
+        w, h = self._size
+        return self._read_feature("FeatureFrame", np.empty((h, w), dtype=capi.PIXEL_FEATURES_DTYPE))
+
+    @property
+    def accumulated_albedo(self) -> np.ndarray:
+        """(H, W, 4) float32: the sum of (albedo, 1) over the feature rays that hit since the last reset."""
+        w, h = self._size
+        return self._read_feature("AccumulatedAlbedo", np.empty((h, w, 4), dtype=np.float32))
+
+    @property
+    def accumulated_normal(self) -> np.ndarray:
+        """(H, W, 4) float32: the sum of (normal, dst) over the feature rays that hit since the last reset."""
+        w, h = self._size
+        return self._read_feature("AccumulatedNormal", np.empty((h, w, 4), dtype=np.float32))
+
+    def camera_rays(self) -> np.ndarray:
+        """(H, W) array of capi.PATH_RAY_DTYPE, row 0 = bottom: every pixel's jittered camera ray for the frame the next RenderFrame()
+        renders and the RNG state after its four draws: what trace_paths and (origin, dir) trace_rays take."""
+        w, h = self._size
+        out = np.empty((h, w), dtype=capi.PATH_RAY_DTYPE)
+        self._ck(self._L.rcmCameraRays(self._h, out.ctypes.data, out.nbytes))
         return out
 
     def pick_ray(self, x: float, y: float) -> np.ndarray:
