@@ -83,6 +83,10 @@ public static class RtB200
     [DllImport(Lib)] public static extern int rtCameraRays(IntPtr ctx, [Out] PathRay[] rays, UIntPtr bytes);
     [DllImport(Lib)] public static extern int rtCameraRaysDevice(IntPtr ctx, IntPtr dRays, UIntPtr bytes);
     [DllImport(Lib, EntryPoint = "rtReadback")] public static extern int rtReadbackFeatures(IntPtr ctx, string tex, [Out] PixelFeatures[] dst, UIntPtr bytes);   // tex = "FeatureFrame", bytes = W*H*32
+    // the a-trous denoiser guided by the feature images: "DenoisedRender" (W*H float4 through rtReadback, the denoised mean colour) and its
+    // display encode (W*H RGBA8, bytes = W*H*4).  iterations 1 .. 5; the managers default to 5, sigmas 64, 1, 0.1
+    [DllImport(Lib)] public static extern int rtDenoise(IntPtr ctx, int useAccumulated, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth);
+    [DllImport(Lib)] public static extern int rtDisplayDenoised(IntPtr ctx, [Out] byte[] dst, UIntPtr bytes);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

@@ -251,11 +251,57 @@ int rtDispatchFeatures(RtContext* ctx, int groupsX, int groupsY, int groupsZ);
 int rtCameraRays(RtContext* ctx, RtPathRay* rays, size_t bytes);
 int rtCameraRaysDevice(RtContext* ctx, void* dRays, size_t bytes);
 
+/* Extension: an edge-avoiding a-trous wavelet denoiser (Dammertz et al., HPG 2010) guided by the feature images, with the colour
+ * demodulated by the albedo as in SVGF.  rtDenoise filters the whole image into the device image "DenoisedRender": W*H float4, [y][x],
+ * row 0 = bottom, rgb = the denoised MEAN colour (already divided by the frame count), w = 1.  Every bit is stated below; each
+ * operation is one IEEE binary32 operation in the order written (no contraction), max is NaN-ignoring.
+ *
+ * Constants, computed by the host in binary32 from the arguments (K = iterations):
+ *     invC = 1 / (sigmaColour * sigmaColour)      cK[k] = invC * 4^k (k = 0 .. K-1)      invN = 1 / (sigmaNormal * sigmaNormal)
+ *     invZ = 1 / sigmaDepth                       rd[k][d] = 2^-(k + d - 1) = 1 / (2^k * d) for d = 1, 2 (exact)
+ *     h = (1/16, 1/4, 3/8, 1/4, 1/16) for offsets -2 .. 2; hh(i, j) = h[i] * h[j] (exact)
+ * Per pixel p, its inputs (c colour, a albedo, n normal, z depth):
+ *     useAccumulated = 1: A = AccumulatedRender, L = AccumulatedAlbedo, N = AccumulatedNormal;
+ *                         c = A.rgb / A.w, a = L.rgb / L.w, n = N.xyz / L.w, z = N.w / L.w (the means over frames and over hits)
+ *     useAccumulated = 0: c = FrameRender.rgb; a, n, z = albedo, normal, dst of FeatureFrame
+ *     m = max(a, 2^-8) per channel, e = c / m per channel (the demodulated colour: the filter smooths lighting, not texture)
+ * p is BACKGROUND when A.w == 0 or L.w == 0 (accumulated), object == -1 (frame), or any of the ten values of c, a, n, z or the three of
+ * e is not finite.  A background pixel is written as (c, 1), with c = (0, 0, 0) when A.w == 0, and is never read as a neighbour.
+ * Iteration k = 0 .. K-1, step s = 2^k, reads only the previous iteration's e (the first reads the e above) and writes e' for every
+ * non-background p = (x, y):
+ *     rz = invZ / z_p;  Sw = Sr = Sg = Sb = +0
+ *     for j = -2 .. 2 (outer), i = -2 .. 2 (inner): q = (x + s*i, y + s*j); a q outside the image or on background is skipped;
+ *         i = j = 0:   w = 9/64
+ *         otherwise:   de = e_p - e_q, dn = n_p - n_q, t = ((z_p - z_q) * rz) * rd[k][max(|i|, |j|)]
+ *                      D = (((de.r*de.r + de.g*de.g) + de.b*de.b) * cK[k] + ((dn.x*dn.x + dn.y*dn.y) + dn.z*dn.z) * invN) + t*t
+ *                      w = hh(i, j) * exp_rt(-D) if D <= 103.972076416015625, else 0 (also for a NaN D: 0*inf, 0/0)
+ *         a tap with w == 0 is skipped (w * e_q is not added); otherwise Sw += w, Sr += w * e_q.r, Sg += w * e_q.g, Sb += w * e_q.b
+ *     e'_p = (Sr / Sw, Sg / Sw, Sb / Sw)       (Sw >= 9/64: the centre is always a tap)
+ * exp_rt is the contract's exponential (DESIGN.md section 2); it returns exactly 0 for arguments below -103.972076416015625, so skipping it
+ * there is bit-exact.  The normal is the mean normal, unnormalised: its shortening at silhouettes is part of the guide.  After the last
+ * iteration DenoisedRender[p] = (e'.r * m.r, e'.g * m.g, e'.b * m.b, 1).
+ *   - Reads the two colour images and the three feature images; leaves FrameRender, AccumulatedRender, FeatureFrame,
+ *     AccumulatedAlbedo, AccumulatedNormal, PixelStats, "Frame" and every RtStats field alone and changes nothing a later dispatch
+ *     renders.  Asynchronous on the context's stream.
+ *   - "DenoisedRender" and the filter's scratch images are allocated by the first rtDenoise: 64 bytes of device memory per pixel in all
+ *     (DenoisedRender 16, scratch 48).  rtResize to a new size zeroes DenoisedRender and frees the scratch; ResetAccumulated leaves both.
+ *     rtReadback and rtGetDevicePointer accept "DenoisedRender" (W*H*16 bytes); RT_E_STATE before the first rtDenoise.
+ *   - Refused: ctx NULL, useAccumulated not 0 or 1, iterations outside 1 .. RT_DENOISE_MAX_ITERATIONS, a sigma that is not finite and
+ *     > 0, or a constant invC * 4^(K-1), invN or invZ that is not finite -> RT_E_INVALID; before rtResize, "Resolution" different from
+ *     the render textures or above 65535, before the first rtDispatchFeatures, any context of a group (rtCreateMulti) and a context
+ *     with rtSetTile world > 1 (its images hold its own bands only) -> RT_E_STATE.
+ * rtDisplayDenoised is rtDisplay's encode of DenoisedRender with Frame = 1: dst receives W*H RGBA8, bytes must equal W*H*4
+ * (RT_E_INVALID otherwise, and for ctx or dst NULL); RT_E_STATE before the first rtDenoise.  Synchronises. */
+#define RT_DENOISE_MAX_ITERATIONS 5
+int rtDenoise(RtContext* ctx, int useAccumulated, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth);
+int rtDisplayDenoised(RtContext* ctx, uint8_t* dst, size_t bytes);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),
  * bytes must equal W·H·16.  After the first rtDispatchFeatures also "AccumulatedAlbedo",
- * "AccumulatedNormal" (float4 as well) and "FeatureFrame" (W·H RtPixelFeatures: bytes must equal W·H·32).  Synchronises. */
+ * "AccumulatedNormal" (float4 as well) and "FeatureFrame" (W·H RtPixelFeatures: bytes must equal W·H·32), and after the first
+ * rtDenoise "DenoisedRender" (float4).  Synchronises. */
 int rtReadback(RtContext* ctx, const char* tex, float* dst, size_t bytes);
 
 /* Replaces: RayTraceDisplay.OnRenderImage -> Graphics.Blit(rt, destination, displayMat) with Display.shader
@@ -336,7 +382,8 @@ int rtCommDestroy(RtContext* ctx);
 int rtExchangeTiles(RtContext* ctx);
 
 /* Device address + size of a named device object, for zero-copy plumbing (NCCL, torch views).
- * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv","PixelStats","FeatureFrame","AccumulatedAlbedo","AccumulatedNormal"}. */
+ * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv","PixelStats","FeatureFrame","AccumulatedAlbedo","AccumulatedNormal",
+ * "DenoisedRender"}. */
 int rtGetDevicePointer(RtContext* ctx, const char* name, void** devPtr, size_t* bytes);
 
 /* Replaces `new BVH(mesh.vertices, mesh.triangles, mesh.normals, quality)` (BVH.cs:26; called once per shared mesh from

@@ -124,6 +124,13 @@ PIXEL_FEATURES_DTYPE = np.dtype([("albedo", "<f4", 3), ("dst", "<f4"), ("normal"
 assert PIXEL_FEATURES_DTYPE.itemsize == 32
 FEATURE_IMAGES = ("FeatureFrame", "AccumulatedAlbedo", "AccumulatedNormal")
 
+# rtDenoise: the defaults of the managers (the C ABI has none), chosen by the quality sweep of DESIGN.md section 7d''''''
+DENOISE_MAX_ITERATIONS = 5
+DENOISE_ITERATIONS = 5
+DENOISE_SIGMA_COLOUR = 64.0
+DENOISE_SIGMA_NORMAL = 1.0
+DENOISE_SIGMA_DEPTH = 0.1
+
 
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
@@ -195,13 +202,15 @@ class RtLib:
             "rtDispatchFeatures": ([vp, ci, ci, ci], ci),
             "rtCameraRays": ([vp, vp, C.c_size_t], ci),
             "rtCameraRaysDevice": ([vp, vp, C.c_size_t], ci),
+            "rtDenoise": ([vp, ci, ci, cf, cf, cf], ci),
+            "rtDisplayDenoised": ([vp, vp, C.c_size_t], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
                             "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
-                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice"):      # absent from older experimental builds used in A/B runs
+                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -374,6 +383,20 @@ class RtContext:
         """rtCameraRaysDevice: the same W*H RtPathRay into device memory of the context's GPU (4-byte aligned, nbytes = W*H*28).
         Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtCameraRaysDevice(self._h, C.c_void_p(rays_ptr), int(nbytes)))
+
+    def denoise(self, use_accumulated: bool = True, iterations: int = DENOISE_ITERATIONS, sigma_colour: float = DENOISE_SIGMA_COLOUR,
+                sigma_normal: float = DENOISE_SIGMA_NORMAL, sigma_depth: float = DENOISE_SIGMA_DEPTH):
+        """rtDenoise: the a-trous filter of the accumulated mean (or of FrameRender) guided by the feature images, into
+        "DenoisedRender" (readback("DenoisedRender") -> (H, W, 4) float32, the denoised mean colour, w = 1).  Asynchronous on the
+        context's stream."""
+        self._ck(self._L.rtDenoise(self._h, 1 if use_accumulated else 0, int(iterations), float(sigma_colour), float(sigma_normal),
+                                   float(sigma_depth)))
+
+    def display_denoised(self) -> np.ndarray:
+        """rtDisplayDenoised: DenoisedRender encoded as rtDisplay encodes (Frame = 1).  (H, W, 4) uint8, row 0 = bottom."""
+        out = np.empty((self.height, self.width, 4), dtype=np.uint8)
+        self._ck(self._L.rtDisplayDenoised(self._h, out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out
 
     def readback(self, tex: str, out: Optional[np.ndarray] = None) -> np.ndarray:
         if out is None:

@@ -11,6 +11,7 @@
 #include "rt_kernel_pool.cuh"
 #include "rt_kernel_query.cuh"
 #include "rt_kernel_features.cuh"
+#include "rt_kernel_denoise.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -107,6 +108,8 @@ struct RtContext
     // rtDispatchFeatures: "FeatureFrame", "AccumulatedAlbedo", "AccumulatedNormal" (W*H each, allocated by the first call);
     // rtCameraRays: the device copy of the image's rays (host form only)
     DevBuf<RtPixelFeatures> featureFrame; DevBuf<float4> accumAlbedo, accumNormal; DevBuf<RtPathRay> cameraRays;
+    // rtDenoise: "DenoisedRender" (W*H) and its scratch images (3*W*H: two demodulated colours, the guide), allocated by the first call
+    DevBuf<float4> denoised, denoiseScratch;
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -217,6 +220,7 @@ int rtDestroy(RtContext* c)
     c->frame.release(); c->accum.release(); c->tileSend.release(); c->tileRecv.release(); c->display.release();
     c->pixelStats.release(); c->queryRays.release(); c->queryHits.release();
     c->featureFrame.release(); c->accumAlbedo.release(); c->accumNormal.release(); c->cameraRays.release();
+    c->denoised.release(); c->denoiseScratch.release();
     c->repack.release();
     closePeers(c);
     for (auto& ev : c->pending) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
@@ -386,6 +390,12 @@ static int one_rtResize(RtContext* c, int w, int h)
             CK(cudaMemsetAsync(c->accumAlbedo.p, 0, n * 16, c->stream));
             CK(cudaMemsetAsync(c->accumNormal.p, 0, n * 16, c->stream));
         }
+        if (c->denoised.p)                                  // the denoised image is zeroed, its scratch freed
+        {
+            CK(c->denoised.ensure(n));
+            CK(cudaMemsetAsync(c->denoised.p, 0, n * 16, c->stream));
+        }
+        c->denoiseScratch.release();
         c->cameraRays.release();
         c->width = w; c->height = h;
         c->tileSend.release(); c->tileRecv.release();
@@ -832,9 +842,11 @@ int rtReadback(RtContext* c, const char* tex, float* dst, size_t bytes)
     const std::string n(tex);
     const bool feature = n == "FeatureFrame" || n == "AccumulatedAlbedo" || n == "AccumulatedNormal";
     if (feature) { int rc = featuresReady(c, "rtReadback"); if (rc != RT_OK) return rc; }
+    if (n == "DenoisedRender" && !c->denoised.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoise yet");
     const void* src = n == "FrameRender" ? (const void*)c->frame.p : n == "AccumulatedRender" ? (const void*)c->accum.p : n == "FeatureFrame" ? (const void*)c->featureFrame.p :
-                      n == "AccumulatedAlbedo" ? (const void*)c->accumAlbedo.p : n == "AccumulatedNormal" ? (const void*)c->accumNormal.p : nullptr;
-    if (n != "FrameRender" && n != "AccumulatedRender" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
+                      n == "AccumulatedAlbedo" ? (const void*)c->accumAlbedo.p : n == "AccumulatedNormal" ? (const void*)c->accumNormal.p :
+                      n == "DenoisedRender" ? (const void*)c->denoised.p : nullptr;
+    if (n != "FrameRender" && n != "AccumulatedRender" && n != "DenoisedRender" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
     if (!src) return fail(c, RT_E_STATE, "rtReadback: rtResize has not been called");
     if (bytes != (size_t)c->width * c->height * (n == "FeatureFrame" ? sizeof(RtPixelFeatures) : 16))
         return fail(c, RT_E_INVALID, n == "FeatureFrame" ? "rtReadback: bytes must equal W*H*32" : "rtReadback: bytes must equal W*H*16");
@@ -1343,6 +1355,61 @@ int rtCameraRaysDevice(RtContext* c, void* dRays, size_t bytes)
     return cameraRaysLocal(c, (RtPathRay*)dRays);
 }
 
+// ---- the a-trous denoiser (rtDenoise, rt_kernel_denoise.cuh) --------------------------------------------------------------------------
+static bool finiteAbove0(float v) { return v > 0.0f && v < INFINITY; }
+
+int rtDenoise(RtContext* c, int useAccumulated, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth)
+{
+    if (!c) return RT_E_INVALID;
+    if (useAccumulated != 0 && useAccumulated != 1) return fail(c, RT_E_INVALID, "rtDenoise: useAccumulated must be 0 or 1");
+    if (iterations < 1 || iterations > RT_DENOISE_MAX_ITERATIONS) return fail(c, RT_E_INVALID, "rtDenoise: iterations must be 1 .. RT_DENOISE_MAX_ITERATIONS");
+    if (!finiteAbove0(sigmaColour) || !finiteAbove0(sigmaNormal) || !finiteAbove0(sigmaDepth)) return fail(c, RT_E_INVALID, "rtDenoise: every sigma must be finite and > 0");
+    // the constants of include/rt_b200.h, one binary32 operation each
+    const float invC = 1.0f / (sigmaColour * sigmaColour), invN = 1.0f / (sigmaNormal * sigmaNormal), invZ = 1.0f / sigmaDepth;
+    DenoisePass passes[RT_DENOISE_MAX_ITERATIONS];
+    for (int k = 0; k < iterations; k++)
+    {
+        passes[k].cK = invC * (float)(1u << (2 * k));
+        passes[k].rd1 = 1.0f / (float)(1u << k); passes[k].rd2 = 1.0f / (float)(2u << k);
+        passes[k].step = 1 << k; passes[k].src = k & 1; passes[k].last = k == iterations - 1;
+    }
+    if (!(passes[iterations - 1].cK < INFINITY) || !(invN < INFINITY) || !(invZ < INFINITY))
+        return fail(c, RT_E_INVALID, "rtDenoise: a sigma too small: invC * 4^(iterations-1), 1 / sigmaNormal^2 or 1 / sigmaDepth is not finite");
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDenoise: not available on a group context (rtCreateMulti)");
+    int rc = cameraImage(c, "rtDenoise"); if (rc != RT_OK) return rc;
+    if (!c->featureFrame.p) return fail(c, RT_E_STATE, "rtDenoise: no rtDispatchFeatures yet");
+    if (c->tileWorld > 1) return fail(c, RT_E_STATE, "rtDenoise: the images of a context with rtSetTile world > 1 hold its own bands only");
+    CK(cudaSetDevice(c->device));
+    const size_t n = (size_t)c->width * c->height;
+    CK(c->denoised.ensure(n)); CK(c->denoiseScratch.ensure(3 * n));
+    DenoiseParams P = {};
+    P.colour = useAccumulated ? c->accum.p : c->frame.p;
+    P.albedo = c->accumAlbedo.p; P.normal = c->accumNormal.p; P.features = c->featureFrame.p;
+    P.e[0] = c->denoiseScratch.p; P.e[1] = c->denoiseScratch.p + n; P.guide = c->denoiseScratch.p + 2 * n;
+    P.out = c->denoised.p;
+    P.W = c->width; P.H = c->height; P.useAccumulated = useAccumulated;
+    P.invN = invN; P.invZ = invZ;
+    cudaError_t e = denoise_launch(P, passes, iterations, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "rtDenoise launch");
+    return RT_OK;
+}
+
+int rtDisplayDenoised(RtContext* c, uint8_t* dst, size_t bytes)
+{
+    if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplayDenoised: bad argument");
+    if (!c->denoised.p) return fail(c, RT_E_STATE, "rtDisplayDenoised: no rtDenoise yet");
+    const size_t n = (size_t)c->width * c->height;
+    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplayDenoised: bytes must equal W*H*4");
+    CK(cudaSetDevice(c->device));
+    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
+    CK(c->display.ensure(n));
+    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, c->denoised.p, c->display.p, n, 1.0f);      // t / 1 is exact
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
 int rtExchangeTiles(RtContext* c)
 {
     if (!c) return RT_E_INVALID;
@@ -1465,6 +1532,11 @@ int rtGetDevicePointer(RtContext* c, const char* name, void** devPtr, size_t* by
         if (n == "FeatureFrame") { *devPtr = c->featureFrame.p; *bytes = c->featureFrame.count * sizeof(RtPixelFeatures); }
         else if (n == "AccumulatedAlbedo") { *devPtr = c->accumAlbedo.p; *bytes = c->accumAlbedo.count * 16; }
         else { *devPtr = c->accumNormal.p; *bytes = c->accumNormal.count * 16; }
+    }
+    else if (n == "DenoisedRender")
+    {
+        if (!c->denoised.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: DenoisedRender is allocated by the first rtDenoise");
+        *devPtr = c->denoised.p; *bytes = c->denoised.count * 16;
     }
     else if (n == "TileSend" || n == "TileRecv")
     {

@@ -24,6 +24,13 @@ class RayTraceDisplay:
     def save_screenshot(self, path: str) -> None:
         write_png(path, self.OnRenderImage()[..., :3])
 
+    def DenoisedImage(self) -> np.ndarray:
+        """The image the last Denoise() of the manager wrote (rtDisplayDenoised), (H, W, 4) uint8, top row first."""
+        return self.raytracer.context.display_denoised()[::-1]
+
+    def save_denoised(self, path: str) -> None:
+        write_png(path, self.DenoisedImage()[..., :3])
+
     def DebugView(self, visMode: int, debugVisScale: float) -> np.ndarray:
         """The reference's debug view (visMode / debugVisScale, RayCommon.hlsl:24-26): heat map of the per-pixel traversal counters
         of the counting launches, (H, W, 4) uint8, top row first.  See RayComputeManager.debug_view."""

@@ -34,6 +34,7 @@ std::string RtApi::Load(const char* path)
     TracePaths = reinterpret_cast<decltype(TracePaths)>(dlsym(dl, "rtTracePaths"));
     DispatchFeatures = reinterpret_cast<decltype(DispatchFeatures)>(dlsym(dl, "rtDispatchFeatures"));
     CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
+    DenoiseFn = reinterpret_cast<decltype(DenoiseFn)>(dlsym(dl, "rtDenoise"));
     return "";
 }
 
@@ -351,6 +352,21 @@ int RayComputeManager::CameraRays(RtPathRay* rays, size_t bytes)
     int rc = InitFrame();
     if (rc != RT_OK) return rc;
     TRY(api.CameraRaysFn(ctx, rays, bytes));
+    return RT_OK;
+}
+
+int RayComputeManager::Denoise(int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.DenoiseFn) { lastError = "the library does not export rtDenoise"; return RT_E_STATE; }
+    TRY(api.DenoiseFn(ctx, accumulate ? 1 : 0, iterations, sigmaColour, sigmaNormal, sigmaDepth));
+    return RT_OK;
+}
+
+int RayComputeManager::ReadDenoised(float* dst, size_t bytes)
+{
+    if (!ctx) return RT_E_STATE;
+    TRY(api.Readback(ctx, "DenoisedRender", dst, bytes));
     return RT_OK;
 }
 

@@ -62,6 +62,7 @@ struct RtApi
     decltype(&rtTracePaths) TracePaths = nullptr;           // optional: radiance along caller rays (TracePaths)
     decltype(&rtDispatchFeatures) DispatchFeatures = nullptr;   // optional: first-hit feature images (RenderFeatures)
     decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
+    decltype(&rtDenoise) DenoiseFn = nullptr;               // optional: the a-trous denoiser (Denoise)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -148,6 +149,11 @@ public:
     // not in the reference: the jittered camera ray of every pixel for that same frame and the RNG state after its four draws
     // (rtCameraRays; W*H records, [y][x]): what TracePaths and TraceRays take.
     int CameraRays(RtPathRay* rays, size_t bytes);
+    // not in the reference: the a-trous denoiser (rtDenoise) over the whole image, guided by the feature images of RenderFeatures():
+    // the accumulated mean when accumulate is on, else the last frame.  The defaults are capi.py's, chosen by the quality sweep of
+    // DESIGN.md section 7d.  ReadDenoised: "DenoisedRender", W*H float4, the denoised mean colour.
+    int Denoise(int iterations = 5, float sigmaColour = 64.0f, float sigmaNormal = 1.0f, float sigmaDepth = 0.1f);
+    int ReadDenoised(float* dst, size_t bytes);
     // picking / autofocus: the un-jittered camera ray through pixel (x, y) of the screen — SetupPixel's operations (HL:547-558) on the
     // manager's own camera fields — and its closest hit
     void PickRay(float x, float y, RtRay* ray) const;

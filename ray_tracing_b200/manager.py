@@ -69,6 +69,8 @@ def host_lib() -> C.CDLL:
         L.rcmRenderFeatures.argtypes = [vp]
         L.rcmReadFeatureImage.argtypes = [vp, cp, vp, C.c_size_t]
         L.rcmCameraRays.argtypes = [vp, vp, C.c_size_t]
+        L.rcmDenoise.argtypes = [vp, ci, cf, cf, cf]
+        L.rcmReadDenoised.argtypes = [vp, vp, C.c_size_t]
         L.rcmPick.argtypes = [vp, cf, cf, vp, vp]
         _host = L
     return _host
@@ -346,6 +348,21 @@ class RayComputeManager:
         w, h = self._size
         out = np.empty((h, w), dtype=capi.PATH_RAY_DTYPE)
         self._ck(self._L.rcmCameraRays(self._h, out.ctypes.data, out.nbytes))
+        return out
+
+    # -- the a-trous denoiser (rtDenoise)
+    def Denoise(self, iterations: int = capi.DENOISE_ITERATIONS, sigma_colour: float = capi.DENOISE_SIGMA_COLOUR,
+                sigma_normal: float = capi.DENOISE_SIGMA_NORMAL, sigma_depth: float = capi.DENOISE_SIGMA_DEPTH):
+        """rtDenoise over the whole image, guided by the feature images RenderFeatures() left: the accumulated mean when accumulate is
+        on, else the last frame.  Read the result with denoised_result."""
+        self._ck(self._L.rcmDenoise(self._h, int(iterations), float(sigma_colour), float(sigma_normal), float(sigma_depth)))
+
+    @property
+    def denoised_result(self) -> np.ndarray:
+        """(H, W, 4) float32, row 0 = bottom: "DenoisedRender", the denoised mean colour, w = 1."""
+        w, h = self._size
+        out = np.empty((h, w, 4), dtype=np.float32)
+        self._ck(self._L.rcmReadDenoised(self._h, out.ctypes.data, out.nbytes))
         return out
 
     def pick_ray(self, x: float, y: float) -> np.ndarray:

@@ -75,6 +75,8 @@ VARIANTS = {
     "all_mesh": ("RT_TREELET_PREFETCH", "RT_STACK_TOP_REG", "RT_TRI_LOAD_POLICY=1", "RT_LEAF_REPEAT=2"),
     # the pooled kernel's cycle account per step kind (tools/pool_clocks.py)
     "clocks": ("RT_POOL_CLOCKS",),
+    # rtDenoise with every tap loaded from global memory instead of the shared-memory sub-lattice tile (tools/denoise_bench.py --ab)
+    "denoise_plain": ("RT_DENOISE_PLAIN",),
 }
 OUT_DIR = os.path.join(build.PKG_DIR, "variants")
 
