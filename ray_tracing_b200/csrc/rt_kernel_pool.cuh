@@ -337,7 +337,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
     int myEntry = -1;                                                // slot this lane is tracing
     f3 lpos = splat3(0.0f), ldir = splat3(0.0f), linv = splat3(0.0f);
     // The ray's running result lives in its slot's hit words (F_HDST .. F_HMODEL): an improving hit writes them at once (rare,
-    // predicated stores), so T_NEXT only flips the slot's state when the ray ends.  The registers keep what the tests compare
+    // predicated stores), so a ray that ends only flips its slot's state.  The registers keep what the tests compare
     // against: bestDst (= result.dst; every model starts from it, HL:359, so a model's winner always becomes the result), the
     // hit kind, and for the sphere accelerator's first-index tie rule the buffer index of its best sphere.  The world ray is
     // re-read from F_POS / F_DIR in the T_NEXT step, the only one that needs it.
@@ -539,50 +539,9 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
             const int nIdle = (int)(census & 255u), nInner = (int)((census >> 8) & 255u), nLeaf = (int)((census >> 16) & 255u), nNext = (int)(census >> 24);
             if (lane == 0) { RT_PROF(0, 1); RT_PROF(1, nIdle); RT_PROF(2, nInner); RT_PROF(3, nLeaf); RT_PROF(4, nNext); }
 
-            // ---- fetch: idle lanes pop the next rays of the warp queue (ballot rank, no atomics) ----
-            if (nIdle != 0 && next < nRays)
-            {
-                const bool need = mode == T_IDLE;
-                const unsigned needMask = __ballot_sync(0xffffffffu, need);
-                const int idx = next + __popc(needMask & ltMask);
-                next += nIdle;
-                if (need && idx < nRays)
-                {
-                    myEntry = pool.order[idx];
-                    pool.u(F_INFO, myEntry) = (pool.u(F_INFO, myEntry) & ~15u) | PS_FLIGHT;
-                    if (STATS) rayStart = cnt;
-                    cnt.rays++;
-#ifdef RT_CACHE_RAYINV
-                    rayInvW = rcp3(pool.get3(F_DIR, myEntry));
-#endif
-                    bestDst = inf32(); hitKind = PS_HIT_MISS;
-                    pool.set_hit(myEntry, inf32(), 0, 0.0f, 0.0f, 0.0f, 0);
-                    // spheres first (extension; where the reference's commented call sits, HL:341)
-                    // A large Spheres buffer is searched through its accelerator by the same state machine as the meshes
-                    // ("model -1": inner nodes = padded sphere boxes, leaves = spheres), see the T_NEXT / T_INNER / T_LEAF blocks.
-                    if (!(EXT && P.sphBvh) && P.sphereCount > 0)
-                    {
-                        const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
-                        for (int s = 0; s < P.sphereCount; s++)
-                        {
-                            float cx, cy, cz, r2; int flag;
-                            if (s < WAVE_MAX_SMEM_SPHERES) { const DevSphere sp = smemSpheres[s]; cx = sp.cx; cy = sp.cy; cz = sp.cz; r2 = sp.r2; flag = sp.pad0; }
-                            else { const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.spheres + s)); cx = s0.x; cy = s0.y; cz = s0.z;
-                                   r2 = __ldg(&P.spheres[s].r2); flag = __ldg(&P.spheres[s].pad0); }
-                            float dst; bool inside;
-                            if (STATS) cnt.sph++;
-                            if (RaySphereCore(rayPos, rayDir, make_f3(cx, cy, cz), r2, dst, inside) && dst < bestDst)
-                            {
-                                bestDst = dst; hitKind = flag == RT_MATERIAL_GLASS ? PS_HIT_GLASS : PS_HIT_OPAQUE;
-                                pool.set_sphere_hit(myEntry, dst, s, inside);
-                            }
-                        }
-                    }
-                    model = (EXT && P.sphBvh) ? -2 : -1; mode = T_NEXT;
-                }
-                continue;                                            // recount: the fetched lanes now wait in T_NEXT
-            }
-            if (nIdle == 32) break;
+            // ---- fetch: idle lanes take the next rays of the warp queue in the T_NEXT step below (ballot rank, no atomics) ----
+            const bool fetch = nIdle != 0 && next < nRays;
+            if (nIdle == 32 && !fetch) break;
             // queue drained and only a few long rays left: go shade what has finished, they continue next phase
             if (next >= nRays && (32 - nIdle) <= P.tailLanes && finishedAny) break;
 
@@ -591,40 +550,107 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
             // iteration would run each at a fraction of the warp.  One kind per iteration keeps the executed block dense,
             // the others catch up when their kind becomes the majority.  The per-ray visiting order is unchanged.
             // (RT_VOTE_W*: cost-weighted vote, see the macro block at the top; all weights 1 = the plain majority)
-            RT_CK(CK_CENSUS, 32 - nIdle);         // (census, fetch and vote of this iteration and of the fetch iterations before it)
+            RT_CK(CK_CENSUS, 32 - nIdle);         // (census and vote of this iteration)
             const int scoreInner = nInner * RT_VOTE_WI, scoreLeaf = nLeaf * RT_VOTE_WL, scoreNext = nNext * RT_VOTE_WN;
-            if (scoreNext >= scoreInner && scoreNext >= scoreLeaf)
+            if (fetch || (scoreNext >= scoreInner && scoreNext >= scoreLeaf))
             {
                 if (lane == 0) { RT_PROF(5, 1); RT_PROF(6, nNext); }
-                // ---- advance to the next model / finish the ray ----
-                bool fin = false;
-                if (mode == T_NEXT)
+                // ---- advance to the next model / finish the ray, and start the next rays of the queue ----
+                // A lane whose ray ends, and at the start of a phase every idle lane, takes the next ray of the queue in this step
+                // and advances it to its first model, instead of going idle for a census, a fetch and another T_NEXT step.  A new
+                // ray that reaches no model ends in its turn, hence the loop: it stops at the first pass that leaves no lane idle
+                // or finds the queue empty (warp-uniform).
+                bool adv = mode == T_NEXT;
+                for (;;)
                 {
-                    // (a model's winner, HL:362-370, and the sphere phase's are in the slot's hit words already)
-                    const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
-                    model++;
-                    // skip the models this ray cannot reach before its current best hit (not in the instrumented build, which
-                    // walks every model like the reference so that the test counts stay identical)
-                    if (!STATS && P.modelSkip && model >= 0)
+                    if (adv)
                     {
-#ifdef RT_CACHE_RAYINV
-                        const f3 rayInv = rayInvW;
-#else
-                        const f3 rayInv = rcp3(rayDir);
-#endif
-                        if (useTlas)
+                        // (a model's winner, HL:362-370, and the sphere phase's are in the slot's hit words already)
+                        const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
+                        model++;
+                        // skip the models this ray cannot reach before its current best hit (not in the instrumented build, which
+                        // walks every model like the reference so that the test counts stay identical)
+                        if (!STATS && P.modelSkip && model >= 0)
                         {
-                            if (model == 0) TlasCollect(P, rayPos, rayInv, bestDst, tlasMask);
-                            for (;;)
+#ifdef RT_CACHE_RAYINV
+                            const f3 rayInv = rayInvW;
+#else
+                            const f3 rayInv = rcp3(rayDir);
+#endif
+                            if (useTlas)
                             {
-                                model = TlasNext(tlasMask, model, P.modelCount);
-                                if (model >= P.modelCount || !ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, bestDst)) break;
-                                model++;
+                                if (model == 0) TlasCollect(P, rayPos, rayInv, bestDst, tlasMask);
+                                for (;;)
+                                {
+                                    model = TlasNext(tlasMask, model, P.modelCount);
+                                    if (model >= P.modelCount || !ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, bestDst)) break;
+                                    model++;
+                                }
+                            }
+                            else
+                            while (model < P.modelCount && ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, bestDst)) model++;
+                        }
+                    }
+                    const bool fin = adv && model >= P.modelCount;
+                    if (fin)
+                    {
+                        const unsigned info = pool.u(F_INFO, myEntry);
+                        pool.u(F_INFO, myEntry) = (info & ~15u) | hitKind;
+                        if (STATS)
+                        {
+                            const unsigned xy = pool.u(F_XY, myEntry);
+                            AddPixelStats(P, (size_t)(xy >> 16) * P.W + (xy & 0xffffu), cnt, rayStart);
+                        }
+                        mode = T_IDLE; myEntry = -1;
+                    }
+                    if (__ballot_sync(0xffffffffu, fin) != 0u) finishedAny = true;
+                    const bool need = mode == T_IDLE;
+                    const unsigned needMask = __ballot_sync(0xffffffffu, need);
+                    if (needMask == 0u || next >= nRays) break;
+                    const int idx = next + __popc(needMask & ltMask);
+                    next += __popc(needMask);
+                    adv = need && idx < nRays;
+                    if (adv)
+                    {
+                        // start the ray of queue entry idx; the next pass advances it to its first model
+                        myEntry = pool.order[idx];
+                        pool.u(F_INFO, myEntry) = (pool.u(F_INFO, myEntry) & ~15u) | PS_FLIGHT;
+                        if (STATS) rayStart = cnt;
+                        cnt.rays++;
+#ifdef RT_CACHE_RAYINV
+                        rayInvW = rcp3(pool.get3(F_DIR, myEntry));
+#endif
+                        bestDst = inf32(); hitKind = PS_HIT_MISS;
+                        pool.set_hit(myEntry, inf32(), 0, 0.0f, 0.0f, 0.0f, 0);
+                        // spheres first (extension; where the reference's commented call sits, HL:341)
+                        // A large Spheres buffer is searched through its accelerator by the same state machine as the meshes
+                        // ("model -1": inner nodes = padded sphere boxes, leaves = spheres), see the T_NEXT / T_INNER / T_LEAF blocks.
+                        if (!(EXT && P.sphBvh) && P.sphereCount > 0)
+                        {
+                            const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
+                            for (int s = 0; s < P.sphereCount; s++)
+                            {
+                                float cx, cy, cz, r2; int flag;
+                                if (s < WAVE_MAX_SMEM_SPHERES) { const DevSphere sp = smemSpheres[s]; cx = sp.cx; cy = sp.cy; cz = sp.cz; r2 = sp.r2; flag = sp.pad0; }
+                                else { const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.spheres + s)); cx = s0.x; cy = s0.y; cz = s0.z;
+                                       r2 = __ldg(&P.spheres[s].r2); flag = __ldg(&P.spheres[s].pad0); }
+                                float dst; bool inside;
+                                if (STATS) cnt.sph++;
+                                if (RaySphereCore(rayPos, rayDir, make_f3(cx, cy, cz), r2, dst, inside) && dst < bestDst)
+                                {
+                                    bestDst = dst; hitKind = flag == RT_MATERIAL_GLASS ? PS_HIT_GLASS : PS_HIT_OPAQUE;
+                                    pool.set_sphere_hit(myEntry, dst, s, inside);
+                                }
                             }
                         }
-                        else
-                        while (model < P.modelCount && ModelOutOfReach(reinterpret_cast<const float4*>(P.models + model), rayPos, rayInv, bestDst)) model++;
+                        model = (EXT && P.sphBvh) ? -2 : -1; mode = T_NEXT;
                     }
+                }
+                // enter the model (or the sphere phase) the advance stopped at: lanes that stay on their ray and lanes that
+                // started a new one together
+                if (mode == T_NEXT)
+                {
+                    const f3 rayPos = pool.get3(F_POS, myEntry), rayDir = pool.get3(F_DIR, myEntry);
                     if (EXT && P.sphBvh && model == -1)
                     {
                         // sphere phase: world-space ray against the accelerator of the Spheres buffer (semantics of TraverseSpheres).
@@ -634,7 +660,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         cur.start = P.sphRootStart; cur.count = P.sphRootCount; leafK = 0; stackCount = 0; RT_STACK_RESET();
                         mode = cur.count > 0 ? T_LEAF : T_INNER; RT_PF_CUR();
                     }
-                    else if (model < P.modelCount)
+                    else
                     {
                         const float4* mr = reinterpret_cast<const float4*>(P.models + model);
                         const float4 r0 = __ldg(mr), r1 = __ldg(mr + 1), r2 = __ldg(mr + 2);
@@ -647,19 +673,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                         cur.start = meta.x; cur.count = meta.y; leafK = 0; stackCount = 0; RT_STACK_RESET();
                         mode = cur.count > 0 ? T_LEAF : T_INNER; RT_PF_CUR();
                     }
-                    else
-                    {
-                        const unsigned info = pool.u(F_INFO, myEntry);
-                        pool.u(F_INFO, myEntry) = (info & ~15u) | hitKind;
-                        if (STATS)
-                        {
-                            const unsigned xy = pool.u(F_XY, myEntry);
-                            AddPixelStats(P, (size_t)(xy >> 16) * P.W + (xy & 0xffffu), cnt, rayStart);
-                        }
-                        mode = T_IDLE; myEntry = -1; fin = true;
-                    }
                 }
-                if (__any_sync(0xffffffffu, fin)) finishedAny = true;
                 RT_CK(CK_NEXT, nNext);
             }
             else if (scoreInner >= scoreLeaf)
