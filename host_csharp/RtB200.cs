@@ -87,6 +87,10 @@ public static class RtB200
     // display encode (W*H RGBA8, bytes = W*H*4).  iterations 1 .. 5; the managers default to 5, sigmas 64, 1, 0.1
     [DllImport(Lib)] public static extern int rtDenoise(IntPtr ctx, int useAccumulated, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth);
     [DllImport(Lib)] public static extern int rtDisplayDenoised(IntPtr ctx, [Out] byte[] dst, UIntPtr bytes);
+    // the temporal (SVGF) denoiser for a moving camera, once per frame after rtDispatch and rtDispatchFeatures: "DenoisedRender" as above and
+    // "TemporalFrame" (W*H float4 through rtReadback: prevX, prevY, history length, variance); the managers default to 5 iterations,
+    // sigmas 8, 1, 0.1, alpha 0.1; resetHistory = 1 on a jump cut
+    [DllImport(Lib)] public static extern int rtDenoiseTemporal(IntPtr ctx, int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

@@ -296,12 +296,83 @@ int rtCameraRaysDevice(RtContext* ctx, void* dRays, size_t bytes);
 int rtDenoise(RtContext* ctx, int useAccumulated, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth);
 int rtDisplayDenoised(RtContext* ctx, uint8_t* dst, size_t bytes);
 
+/* Extension: a temporal denoiser for a moving camera, SVGF (Schied et al., HPG 2017): each pixel's first hit is reprojected into the
+ * previous call's camera, its demodulated colour and luminance moments are blended with the history found there, and the variance of
+ * those moments steers an a-trous filter of the integrated colour.  One call per frame, after the frame's rtDispatch(RAYTRACE) and
+ * rtDispatchFeatures with the same "Frame"; it reads FrameRender (the frame's own colour: any "accumulate" works), FeatureFrame,
+ * "CamLocalToWorldMatrix", "ViewParams" and "Resolution", and writes "DenoisedRender" (as rtDenoise does: W*H float4, w = 1, so
+ * rtDisplayDenoised, rtReadback and rtGetDevicePointer serve it) and "TemporalFrame": W*H float4, [y][x], row 0 = bottom,
+ * (prevX, prevY, len, variance).  The operations are binary32 in the order written, as for rtDenoise; min / max are NaN-ignoring.
+ *
+ * Constants: RT_TEMPORAL_TAU_Z, RT_TEMPORAL_TAU_N, RT_TEMPORAL_MAX_HISTORY, RT_TEMPORAL_EPSILON below; from the arguments, in binary32:
+ *     invN = 1 / (sigmaNormal * sigmaNormal)     invZ = 1 / sigmaDepth     invL = 1 / sigmaLuminance
+ *     lum(v) = (0.2126 * v.r + 0.7152 * v.g) + 0.0722 * v.b       (the binary32 literals)
+ * Per pixel p = (x, y): c = FrameRender.rgb; a, z, n, object from FeatureFrame; m = max(a, 2^-8), e = c / m; p is BACKGROUND under
+ * rtDenoise's frame rule (object == -1 or one of c, a, n, z, e not finite).  A background pixel gets DenoisedRender (c, 1),
+ * TemporalFrame (NaN, NaN, 0, 0), no history record, and is never read.  Otherwise l = lum(e), and:
+ * 1. Reprojection.  The previous camera is that of the last successful call, unless resetHistory = 1, rtResize to a new size came
+ *    between, or there is none: then (prevX, prevY) = (NaN, NaN).  If the previous call's "CamLocalToWorldMatrix" and "ViewParams" equal
+ *    the current ones bit for bit (the image size is equal: a new size discards the history), prevX = x, prevY = y and zexp = z.
+ *    Otherwise, with camOrigin and focusPoint of the pixel's SetupPixel (HL:547-558) and the previous camera M', VP':
+ *        d = normalize(focusPoint - camOrigin)   X = camOrigin + d * z (per component: o + d * z)
+ *        A = M' rows 0..2, columns 0..2; t = M' column 3 rows 0..2.  In float64: cofactors c_rc of A, det = (a00*c00 + a01*c01) + a02*c02,
+ *        R[r][k] = c_kr / det; b[r] = -((R[r][0]*t0 + R[r][1]*t1) + R[r][2]*t2); each R and b entry then rounded once to binary32.
+ *        L[r] = ((R[r][0]*X.x + R[r][1]*X.y) + R[r][2]*X.z) + b[r]
+ *        u = (L.x / L.z) * kx + 0.5, v = (L.y / L.z) * ky + 0.5 with kx = VP'.z / VP'.x, ky = VP'.z / VP'.y (binary32)
+ *        prevX = u * (W - 1), prevY = v * (H - 1);  zexp = sqrt((dx*dx + dy*dy) + dz*dz), (dx, dy, dz) = X - t (binary32 t)
+ *    and the projection fails ((prevX, prevY) = (NaN, NaN)) unless L.z > 0 and X, L, u, v, prevX, prevY and zexp are all finite.
+ * 2. History.  With (prevX, prevY) not NaN and -1 < prevX < W, -1 < prevY < H: x0 = floor(prevX), fx = prevX - x0 (y likewise), and
+ *    the taps (x0, y0), (x0 + 1, y0), (x0, y0 + 1), (x0 + 1, y0 + 1) in that order with weight w = wx * wy, wx = 1 - fx or fx,
+ *    wy = 1 - fy or fy.  A tap q counts when w != 0, q is inside the image, q has a history record (not background in the previous
+ *    call), object_q == object, |z_q - zexp| <= RT_TEMPORAL_TAU_Z * zexp and (n.x*n_q.x + n.y*n_q.y) + n.z*n_q.z >= RT_TEMPORAL_TAU_N.
+ *    Over the counted taps: Sw += w, Sc += w * colour_q (per channel), S1 += w * m1_q, S2 += w * m2_q, lenH = max(lenH, len_q).
+ * 3. Integration.  No counted tap: len = 1, colour = e, (m1, m2) = (l, l*l).  Otherwise h = Sc / Sw, h1 = S1 / Sw, h2 = S2 / Sw,
+ *    len = min(lenH + 1, RT_TEMPORAL_MAX_HISTORY), a = max(alpha, 1 / len), colour = h + a * (e - h), m1 = h1 + a * (l - h1),
+ *    m2 = h2 + a * (l*l - h2).  p's history record becomes (n, z, object, m1, m2, len).  TemporalFrame.xyz = (prevX, prevY, len).
+ * 4. Variance.  len >= 4: var = max(m2 - m1*m1, 0).  Otherwise, over the 7x7 neighbours q = (x + i, y + j), j = -3 .. 3 (outer),
+ *    i = -3 .. 3, inside the image and not background: w = 1 for q = p, else with dn = n - n_q, t = (z - z_q) * (invZ / z):
+ *        D = (|m1 - m1_q| * invL + ((dn.x*dn.x + dn.y*dn.y) + dn.z*dn.z) * invN) + t*t, w = exp_rt(-D) (0 when D > 103.972076416015625
+ *        or NaN); a tap with w == 0 is skipped; Sw += w, S1 += w * m1_q, S2 += w * m2_q
+ *    and var = max(S2 / Sw - (S1 / Sw) * (S1 / Sw), 0) * (4 / len).  TemporalFrame.w = var.
+ * 5. Filter.  Iterations k = 0 .. K-1 run rtDenoise's pass (step s = 2^k, the same taps, order, hh(i, j), t with rd[k][d], skip rules
+ *    and sums, over the current guides n, z) on the pair (colour, var), starting from step 3's colour and step 4's var, with two changes:
+ *        gv_p = Sg / Sk over the 3x3 immediate neighbours q = (x + i, y + j), j = -1 .. 1 (outer), i = -1 .. 1, inside the image
+ *               and not background, of this iteration's input var (SVGF's prefilter, at every step):
+ *               k = k1[i] * k1[j], k1 = (1/4, 1/2, 1/4); Sk += k, Sg += k * var_q
+ *        kL = 1 / (sigmaLuminance * sqrt(gv_p) + RT_TEMPORAL_EPSILON)
+ *        D = (|lum(colour_p) - lum(colour_q)| * kL + ((dn.x*dn.x + dn.y*dn.y) + dn.z*dn.z) * invN) + t*t     (no colour distance)
+ *        for each added tap also Sv += (w * w) * var_q (the centre: w = 9/64), and var'_p = Sv / (Sw * Sw).
+ *    The output colour of iteration 0 is p's colour history for the next call.  After the last iteration DenoisedRender[p] =
+ *    (colour'.r * m.r, colour'.g * m.g, colour'.b * m.b, 1).
+ *   - Geometry is assumed static between calls: a moved model gets no motion vectors; the object, depth and normal tests are what
+ *     limit its ghosting.
+ *   - Leaves FrameRender, AccumulatedRender, the feature images, PixelStats, "Frame", every RtStats field and what later dispatches
+ *     render alone.  rtDenoise and rtDenoiseTemporal do not affect each other's results (they share only DenoisedRender and the
+ *     filter's scratch images).  ResetAccumulated leaves the history alone.  Asynchronous on the context's stream.
+ *   - Memory: "TemporalFrame" and the history are allocated by the first call, 112 bytes of device memory per pixel (TemporalFrame 16,
+ *     two alternating sets of guide, moments and colour history 96), plus rtDenoise's 64 if rtDenoise has not allocated them.
+ *     rtResize to a new size zeroes TemporalFrame and discards the history.  rtReadback and rtGetDevicePointer accept "TemporalFrame"
+ *     (W*H*16 bytes); RT_E_STATE before the first rtDenoiseTemporal.
+ *   - Refused: ctx NULL, iterations outside 1 .. RT_DENOISE_MAX_ITERATIONS, a sigma that is not finite and > 0, invN, invZ or invL not
+ *     finite, alpha outside (0, 1], resetHistory not 0 or 1 -> RT_E_INVALID; before rtResize, "Resolution" different from the render
+ *     textures or above 65535, before the first rtDispatchFeatures, any context of a group and a context with rtSetTile world > 1 ->
+ *     RT_E_STATE.  A refused call leaves the history and the previous camera as they were. */
+#ifndef RT_TEMPORAL_TAU_Z                  /* overridable only by the A/B build variants of tools/build_variants.py */
+#define RT_TEMPORAL_TAU_Z 0.05f
+#endif
+#ifndef RT_TEMPORAL_TAU_N
+#define RT_TEMPORAL_TAU_N 0.9f
+#endif
+#define RT_TEMPORAL_MAX_HISTORY 32
+#define RT_TEMPORAL_EPSILON 0.0000152587890625f     /* 2^-16 */
+int rtDenoiseTemporal(RtContext* ctx, int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),
  * bytes must equal W·H·16.  After the first rtDispatchFeatures also "AccumulatedAlbedo",
  * "AccumulatedNormal" (float4 as well) and "FeatureFrame" (W·H RtPixelFeatures: bytes must equal W·H·32), and after the first
- * rtDenoise "DenoisedRender" (float4).  Synchronises. */
+ * rtDenoise "DenoisedRender" (float4), and after the first rtDenoiseTemporal "TemporalFrame" (float4).  Synchronises. */
 int rtReadback(RtContext* ctx, const char* tex, float* dst, size_t bytes);
 
 /* Replaces: RayTraceDisplay.OnRenderImage -> Graphics.Blit(rt, destination, displayMat) with Display.shader
@@ -383,7 +454,7 @@ int rtExchangeTiles(RtContext* ctx);
 
 /* Device address + size of a named device object, for zero-copy plumbing (NCCL, torch views).
  * name ∈ {"FrameRender","AccumulatedRender","TileSend","TileRecv","PixelStats","FeatureFrame","AccumulatedAlbedo","AccumulatedNormal",
- * "DenoisedRender"}. */
+ * "DenoisedRender","TemporalFrame"}. */
 int rtGetDevicePointer(RtContext* ctx, const char* name, void** devPtr, size_t* bytes);
 
 /* Replaces `new BVH(mesh.vertices, mesh.triangles, mesh.normals, quality)` (BVH.cs:26; called once per shared mesh from

@@ -131,6 +131,14 @@ DENOISE_SIGMA_COLOUR = 64.0
 DENOISE_SIGMA_NORMAL = 1.0
 DENOISE_SIGMA_DEPTH = 0.1
 
+# rtDenoiseTemporal: the defaults of the managers, chosen by the quality sweep of DESIGN.md section 7d'''''''
+TEMPORAL_ITERATIONS = 5
+TEMPORAL_SIGMA_LUMINANCE = 8.0
+TEMPORAL_SIGMA_NORMAL = 1.0
+TEMPORAL_SIGMA_DEPTH = 0.1
+TEMPORAL_ALPHA = 0.1
+TEMPORAL_MAX_HISTORY = 32          # RT_TEMPORAL_MAX_HISTORY
+
 
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
@@ -204,13 +212,14 @@ class RtLib:
             "rtCameraRaysDevice": ([vp, vp, C.c_size_t], ci),
             "rtDenoise": ([vp, ci, ci, cf, cf, cf], ci),
             "rtDisplayDenoised": ([vp, vp, C.c_size_t], ci),
+            "rtDenoiseTemporal": ([vp, ci, cf, cf, cf, cf, ci], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
                             "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
-                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised"):      # absent from older experimental builds used in A/B runs
+                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -391,6 +400,19 @@ class RtContext:
         context's stream."""
         self._ck(self._L.rtDenoise(self._h, 1 if use_accumulated else 0, int(iterations), float(sigma_colour), float(sigma_normal),
                                    float(sigma_depth)))
+
+    def denoise_temporal(self, iterations: int = TEMPORAL_ITERATIONS, sigma_luminance: float = TEMPORAL_SIGMA_LUMINANCE,
+                         sigma_normal: float = TEMPORAL_SIGMA_NORMAL, sigma_depth: float = TEMPORAL_SIGMA_DEPTH, alpha: float = TEMPORAL_ALPHA,
+                         reset_history: bool = False):
+        """rtDenoiseTemporal: FrameRender filtered with its reprojected history (SVGF), guided by the feature images, into
+        "DenoisedRender"; the motion vectors, history lengths and variances into "TemporalFrame" (temporal_frame()).  Asynchronous on
+        the context's stream."""
+        self._ck(self._L.rtDenoiseTemporal(self._h, int(iterations), float(sigma_luminance), float(sigma_normal), float(sigma_depth),
+                                           float(alpha), 1 if reset_history else 0))
+
+    def temporal_frame(self) -> np.ndarray:
+        """"TemporalFrame": (H, W, 4) float32, row 0 = bottom, (prevX, prevY, history length, variance) per pixel."""
+        return self.readback("TemporalFrame")
 
     def display_denoised(self) -> np.ndarray:
         """rtDisplayDenoised: DenoisedRender encoded as rtDisplay encodes (Frame = 1).  (H, W, 4) uint8, row 0 = bottom."""

@@ -12,6 +12,7 @@
 #include "rt_kernel_query.cuh"
 #include "rt_kernel_features.cuh"
 #include "rt_kernel_denoise.cuh"
+#include "rt_kernel_temporal.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -110,6 +111,11 @@ struct RtContext
     DevBuf<RtPixelFeatures> featureFrame; DevBuf<float4> accumAlbedo, accumNormal; DevBuf<RtPathRay> cameraRays;
     // rtDenoise: "DenoisedRender" (W*H) and its scratch images (3*W*H: two demodulated colours, the guide), allocated by the first call
     DevBuf<float4> denoised, denoiseScratch;
+    // rtDenoiseTemporal: "TemporalFrame" (W*H) and the history (6*W*H: two sets of guide, moments and colour history that alternate
+    // between calls, set temporalSet written last), allocated by the first call; the camera of the last call that left a history
+    DevBuf<float4> temporalFrame, temporalHist;
+    int temporalSet = 0; bool temporalHistory = false;
+    float temporalCam[16] = {}, temporalVP[3] = {};
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -220,7 +226,7 @@ int rtDestroy(RtContext* c)
     c->frame.release(); c->accum.release(); c->tileSend.release(); c->tileRecv.release(); c->display.release();
     c->pixelStats.release(); c->queryRays.release(); c->queryHits.release();
     c->featureFrame.release(); c->accumAlbedo.release(); c->accumNormal.release(); c->cameraRays.release();
-    c->denoised.release(); c->denoiseScratch.release();
+    c->denoised.release(); c->denoiseScratch.release(); c->temporalFrame.release(); c->temporalHist.release();
     c->repack.release();
     closePeers(c);
     for (auto& ev : c->pending) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
@@ -396,6 +402,12 @@ static int one_rtResize(RtContext* c, int w, int h)
             CK(cudaMemsetAsync(c->denoised.p, 0, n * 16, c->stream));
         }
         c->denoiseScratch.release();
+        if (c->temporalFrame.p)                             // TemporalFrame is zeroed, the temporal history discarded
+        {
+            CK(c->temporalFrame.ensure(n));
+            CK(cudaMemsetAsync(c->temporalFrame.p, 0, n * 16, c->stream));
+        }
+        c->temporalHist.release(); c->temporalHistory = false;
         c->cameraRays.release();
         c->width = w; c->height = h;
         c->tileSend.release(); c->tileRecv.release();
@@ -843,10 +855,11 @@ int rtReadback(RtContext* c, const char* tex, float* dst, size_t bytes)
     const bool feature = n == "FeatureFrame" || n == "AccumulatedAlbedo" || n == "AccumulatedNormal";
     if (feature) { int rc = featuresReady(c, "rtReadback"); if (rc != RT_OK) return rc; }
     if (n == "DenoisedRender" && !c->denoised.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoise yet");
+    if (n == "TemporalFrame" && !c->temporalFrame.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoiseTemporal yet");
     const void* src = n == "FrameRender" ? (const void*)c->frame.p : n == "AccumulatedRender" ? (const void*)c->accum.p : n == "FeatureFrame" ? (const void*)c->featureFrame.p :
                       n == "AccumulatedAlbedo" ? (const void*)c->accumAlbedo.p : n == "AccumulatedNormal" ? (const void*)c->accumNormal.p :
-                      n == "DenoisedRender" ? (const void*)c->denoised.p : nullptr;
-    if (n != "FrameRender" && n != "AccumulatedRender" && n != "DenoisedRender" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
+                      n == "DenoisedRender" ? (const void*)c->denoised.p : n == "TemporalFrame" ? (const void*)c->temporalFrame.p : nullptr;
+    if (n != "FrameRender" && n != "AccumulatedRender" && n != "DenoisedRender" && n != "TemporalFrame" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
     if (!src) return fail(c, RT_E_STATE, "rtReadback: rtResize has not been called");
     if (bytes != (size_t)c->width * c->height * (n == "FeatureFrame" ? sizeof(RtPixelFeatures) : 16))
         return fail(c, RT_E_INVALID, n == "FeatureFrame" ? "rtReadback: bytes must equal W*H*32" : "rtReadback: bytes must equal W*H*16");
@@ -1394,6 +1407,83 @@ int rtDenoise(RtContext* c, int useAccumulated, int iterations, float sigmaColou
     return RT_OK;
 }
 
+// ---- the temporal denoiser (rtDenoiseTemporal, rt_kernel_temporal.cuh) ------------------------------------------------------------------
+// The previous camera's inverse affine map as include/rt_b200.h states it: adjugate / determinant in float64, each entry rounded once
+static void temporalInverse(const float* m, float inv[12])
+{
+    const double a00 = m[0], a01 = m[4], a02 = m[8], a10 = m[1], a11 = m[5], a12 = m[9], a20 = m[2], a21 = m[6], a22 = m[10];
+    const double t[3] = {m[12], m[13], m[14]};
+    const double c00 = a11 * a22 - a12 * a21, c01 = a12 * a20 - a10 * a22, c02 = a10 * a21 - a11 * a20;
+    const double c10 = a02 * a21 - a01 * a22, c11 = a00 * a22 - a02 * a20, c12 = a01 * a20 - a00 * a21;
+    const double c20 = a01 * a12 - a02 * a11, c21 = a02 * a10 - a00 * a12, c22 = a00 * a11 - a01 * a10;
+    const double det = (a00 * c00 + a01 * c01) + a02 * c02;
+    const double R[3][3] = {{c00 / det, c10 / det, c20 / det}, {c01 / det, c11 / det, c21 / det}, {c02 / det, c12 / det, c22 / det}};
+    for (int r = 0; r < 3; r++)
+    {
+        for (int k = 0; k < 3; k++) inv[4 * r + k] = (float)R[r][k];
+        inv[4 * r + 3] = (float)-((R[r][0] * t[0] + R[r][1] * t[1]) + R[r][2] * t[2]);
+    }
+}
+
+int rtDenoiseTemporal(RtContext* c, int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory)
+{
+    if (!c) return RT_E_INVALID;
+    if (iterations < 1 || iterations > RT_DENOISE_MAX_ITERATIONS) return fail(c, RT_E_INVALID, "rtDenoiseTemporal: iterations must be 1 .. RT_DENOISE_MAX_ITERATIONS");
+    if (!finiteAbove0(sigmaLuminance) || !finiteAbove0(sigmaNormal) || !finiteAbove0(sigmaDepth)) return fail(c, RT_E_INVALID, "rtDenoiseTemporal: every sigma must be finite and > 0");
+    if (!(alpha > 0.0f && alpha <= 1.0f)) return fail(c, RT_E_INVALID, "rtDenoiseTemporal: alpha must be in (0, 1]");
+    if (resetHistory != 0 && resetHistory != 1) return fail(c, RT_E_INVALID, "rtDenoiseTemporal: resetHistory must be 0 or 1");
+    const float invN = 1.0f / (sigmaNormal * sigmaNormal), invZ = 1.0f / sigmaDepth, invL = 1.0f / sigmaLuminance;
+    if (!(invN < INFINITY) || !(invZ < INFINITY) || !(invL < INFINITY))
+        return fail(c, RT_E_INVALID, "rtDenoiseTemporal: a sigma too small: 1 / sigmaNormal^2, 1 / sigmaDepth or 1 / sigmaLuminance is not finite");
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDenoiseTemporal: not available on a group context (rtCreateMulti)");
+    int rc = cameraImage(c, "rtDenoiseTemporal"); if (rc != RT_OK) return rc;
+    if (!c->featureFrame.p) return fail(c, RT_E_STATE, "rtDenoiseTemporal: no rtDispatchFeatures yet");
+    if (c->tileWorld > 1) return fail(c, RT_E_STATE, "rtDenoiseTemporal: the images of a context with rtSetTile world > 1 hold its own bands only");
+    CK(cudaSetDevice(c->device));
+    const size_t n = (size_t)c->width * c->height;
+    if (!c->temporalHist.p) c->temporalHistory = false;
+    CK(c->denoised.ensure(n)); CK(c->denoiseScratch.ensure(3 * n)); CK(c->temporalFrame.ensure(n)); CK(c->temporalHist.ensure(6 * n));
+    DenoisePass passes[RT_DENOISE_MAX_ITERATIONS];
+    for (int k = 0; k < iterations; k++)
+    {
+        passes[k].cK = 0.0f;
+        passes[k].rd1 = 1.0f / (float)(1u << k); passes[k].rd2 = 1.0f / (float)(2u << k);
+        passes[k].step = 1 << k; passes[k].src = k & 1; passes[k].last = k == iterations - 1;
+    }
+    const int cur = c->temporalSet ^ 1;
+    float4* const set[2] = {c->temporalHist.p, c->temporalHist.p + 3 * n};       // guide, moments, colour history
+    TemporalParams T = {};
+    T.colour = c->frame.p; T.features = c->featureFrame.p;
+    T.e = c->denoiseScratch.p; T.out = c->denoised.p; T.frame = c->temporalFrame.p;
+    T.guide = set[cur]; T.mom = set[cur] + n;
+    T.prevGuide = set[cur ^ 1]; T.prevMom = set[cur ^ 1] + n; T.prevColour = set[cur ^ 1] + 2 * n;
+    T.W = c->width; T.H = c->height;
+    T.alpha = alpha; T.invN = invN; T.invZ = invZ; T.invL = invL;
+    T.mode = TEMPORAL_NONE;
+    if (c->temporalHistory && !resetHistory)
+    {
+        if (memcmp(c->temporalCam, c->P.cam, sizeof(c->temporalCam)) == 0 && memcmp(c->temporalVP, c->P.ViewParams, sizeof(c->temporalVP)) == 0)
+            T.mode = TEMPORAL_STATIC;
+        else
+        {
+            T.mode = TEMPORAL_REPROJECT;
+            temporalInverse(c->temporalCam, T.inv);
+            T.prevOrigin[0] = c->temporalCam[12]; T.prevOrigin[1] = c->temporalCam[13]; T.prevOrigin[2] = c->temporalCam[14];
+            T.kx = c->temporalVP[2] / c->temporalVP[0]; T.ky = c->temporalVP[2] / c->temporalVP[1];
+        }
+    }
+    TemporalPassParams Pp = {};
+    Pp.e[0] = c->denoiseScratch.p; Pp.e[1] = c->denoiseScratch.p + n; Pp.guide = T.guide; Pp.out = c->denoised.p;
+    Pp.W = c->width; Pp.H = c->height; Pp.invN = invN; Pp.invZ = invZ;
+    Pp.hist = set[cur] + 2 * n; Pp.sigmaL = sigmaLuminance;
+    Pp.gv = reinterpret_cast<float*>(c->denoiseScratch.p + 2 * n);                // rtDenoise's guide slot, unused here
+    cudaError_t e = temporal_launch(T, c->P, Pp, passes, iterations, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "rtDenoiseTemporal launch");
+    c->temporalSet = cur; c->temporalHistory = true;
+    memcpy(c->temporalCam, c->P.cam, sizeof(c->temporalCam)); memcpy(c->temporalVP, c->P.ViewParams, sizeof(c->temporalVP));
+    return RT_OK;
+}
+
 int rtDisplayDenoised(RtContext* c, uint8_t* dst, size_t bytes)
 {
     if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplayDenoised: bad argument");
@@ -1537,6 +1627,11 @@ int rtGetDevicePointer(RtContext* c, const char* name, void** devPtr, size_t* by
     {
         if (!c->denoised.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: DenoisedRender is allocated by the first rtDenoise");
         *devPtr = c->denoised.p; *bytes = c->denoised.count * 16;
+    }
+    else if (n == "TemporalFrame")
+    {
+        if (!c->temporalFrame.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: TemporalFrame is allocated by the first rtDenoiseTemporal");
+        *devPtr = c->temporalFrame.p; *bytes = c->temporalFrame.count * 16;
     }
     else if (n == "TileSend" || n == "TileRecv")
     {

@@ -82,7 +82,19 @@ __global__ void __launch_bounds__(256) k_denoise_prepare(const __grid_constant__
     P.out[p] = make_float4(m.x, m.y, m.z, 1.0f);
 }
 
-__global__ void __launch_bounds__(DN_TX * DN_TY) k_denoise_pass(const __grid_constant__ DenoiseParams P, const DenoisePass S)
+// rtDenoiseTemporal's passes (rt_kernel_temporal.cuh) run the same tiling with the variance-guided weights: e.w carries the variance
+struct TemporalPassParams : DenoiseParams
+{
+    float4* hist;                            // the colour history: iteration 0's output
+    float* gv;                               // this iteration's prefiltered variance (k_temporal_prefilter)
+    float sigmaL;
+};
+
+RT_DI float luminance(float4 e) { return (0.2126f * e.x + 0.7152f * e.y) + 0.0722f * e.z; }
+
+// One iteration of either filter: SVGF = false is rtDenoise's, true rtDenoiseTemporal's (include/rt_b200.h states both)
+template <bool SVGF, class PP>
+RT_DI void denoise_pass_body(const PP& P, const DenoisePass& S)
 {
     const int s = S.step;
     const int rx = (int)blockIdx.z % s, ry = (int)blockIdx.z / s;             // the residue class of this CTA's lattice
@@ -124,6 +136,33 @@ __global__ void __launch_bounds__(DN_TX * DN_TY) k_denoise_pass(const __grid_con
     if (gp.w != gp.w) return;                                                  // background: DenoisedRender already holds (c, 1)
     const float rz = P.invZ / gp.w;
     float sw = 0.0f, sr = 0.0f, sg = 0.0f, sb = 0.0f;
+    float kL = 0.0f, lp = 0.0f, sv = 0.0f;
+    if constexpr (SVGF)
+    {
+#ifdef RT_TEMPORAL_LATTICE_PREFILTER
+        // build variant for the A/B of DESIGN.md section 7d''''''' (tools/build_variants.py temporal_lattice): the 3x3 Gaussian over
+        // the lattice neighbours at +-s, read from the staged tile.  Not SVGF's form and not the header's: no oracle restates it.
+        float gw = 0.0f, gv = 0.0f;
+#pragma unroll
+        for (int j = -1; j <= 1; j++)
+        {
+#pragma unroll
+            for (int i = -1; i <= 1; i++)
+            {
+                float4 eq = make_float4(0.0f, 0.0f, 0.0f, 0.0f), gq;
+                RT_DN_TAP(i, j, eq, gq);
+                if (gq.w != gq.w) continue;
+                const float k = (i == 0 ? 0.5f : 0.25f) * (j == 0 ? 0.5f : 0.25f);
+                gw = gw + k; gv = gv + k * eq.w;
+            }
+        }
+        const float gvp = gv / gw;
+#else
+        const float gvp = P.gv[(size_t)y * P.W + x];                           // SVGF's 3x3 Gaussian over the immediate neighbours
+#endif
+        kL = 1.0f / (P.sigmaL * sqrtf(gvp) + RT_TEMPORAL_EPSILON);
+        lp = luminance(ep);
+    }
 #pragma unroll
     for (int j = -2; j <= 2; j++)
     {
@@ -142,24 +181,53 @@ __global__ void __launch_bounds__(DN_TX * DN_TY) k_denoise_pass(const __grid_con
                 const float nx = gp.x - gq.x, ny = gp.y - gq.y, nz = gp.z - gq.z;
                 const int d = (i < 0 ? -i : i) > (j < 0 ? -j : j) ? (i < 0 ? -i : i) : (j < 0 ? -j : j);
                 const float t = ((gp.w - gq.w) * rz) * (d == 1 ? S.rd1 : S.rd2);
-                const float D = (((dr * dr + dg * dg) + db * db) * S.cK + ((nx * nx + ny * ny) + nz * nz) * P.invN) + t * t;
+                const float D = SVGF ? (fabsf(lp - luminance(eq)) * kL + ((nx * nx + ny * ny) + nz * nz) * P.invN) + t * t
+                                     : (((dr * dr + dg * dg) + db * db) * S.cK + ((nx * nx + ny * ny) + nz * nz) * P.invN) + t * t;
                 if (!(D <= 103.972076416015625f)) continue;                    // exp_rt is exactly 0 there; a NaN D weighs 0 too
                 w = (hi * hj) * exp_rt(-D);
                 if (w == 0.0f) continue;
             }
             sw = sw + w;
             sr = sr + w * eq.x; sg = sg + w * eq.y; sb = sb + w * eq.z;
+            if constexpr (SVGF) sv = sv + (w * w) * eq.w;
         }
     }
 #undef RT_DN_TAP
     const size_t p = (size_t)y * P.W + x;
     const float er = sr / sw, eg = sg / sw, eb = sb / sw;
+    if constexpr (SVGF) { if (s == 1) P.hist[p] = make_float4(er, eg, eb, 0.0f); }
     if (S.last)
     {
         const float4 m = P.out[p];
         P.out[p] = make_float4(er * m.x, eg * m.y, eb * m.z, 1.0f);
     }
-    else P.e[S.src ^ 1][p] = make_float4(er, eg, eb, 0.0f);
+    else P.e[S.src ^ 1][p] = make_float4(er, eg, eb, SVGF ? sv / (sw * sw) : 0.0f);
+}
+
+__global__ void __launch_bounds__(DN_TX * DN_TY) k_denoise_pass(const __grid_constant__ DenoiseParams P, const DenoisePass S)
+{
+    denoise_pass_body<false>(P, S);
+}
+
+__global__ void __launch_bounds__(DN_TX * DN_TY) k_temporal_pass(const __grid_constant__ TemporalPassParams P, const DenoisePass S)
+{
+    denoise_pass_body<true>(P, S);
+}
+
+// `iterations` filter passes of KERNEL on `stream`
+template <class PP>
+inline cudaError_t denoise_passes(void (*kernel)(PP, DenoisePass), const PP& P, const DenoisePass* passes, int iterations, cudaStream_t stream)
+{
+    cudaError_t e = cudaSuccess;
+    for (int k = 0; k < iterations && e == cudaSuccess; k++)
+    {
+        const int s = passes[k].step;
+        const unsigned LW = (unsigned)((P.W + s - 1) / s), LH = (unsigned)((P.H + s - 1) / s);
+        const dim3 grid((LW + DN_TX - 1) / DN_TX, (LH + DN_TY - 1) / DN_TY, (unsigned)(s * s));
+        RT_LAUNCH(grid, DN_TX * DN_TY, 0, stream, kernel, P, passes[k]);
+        e = cudaGetLastError();
+    }
+    return e;
 }
 
 // The prepare pass and `iterations` filter passes on `stream`.  The caller has checked the arguments and computed the constants.
@@ -168,15 +236,7 @@ inline cudaError_t denoise_launch(const DenoiseParams& P, const DenoisePass* pas
     const size_t n = (size_t)P.W * P.H;
     RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, stream, k_denoise_prepare, P);
     cudaError_t e = cudaGetLastError();
-    for (int k = 0; k < iterations && e == cudaSuccess; k++)
-    {
-        const int s = passes[k].step;
-        const unsigned LW = (unsigned)((P.W + s - 1) / s), LH = (unsigned)((P.H + s - 1) / s);
-        const dim3 grid((LW + DN_TX - 1) / DN_TX, (LH + DN_TY - 1) / DN_TY, (unsigned)(s * s));
-        RT_LAUNCH(grid, DN_TX * DN_TY, 0, stream, k_denoise_pass, P, passes[k]);
-        e = cudaGetLastError();
-    }
-    return e;
+    return e == cudaSuccess ? denoise_passes(k_denoise_pass, P, passes, iterations, stream) : e;
 }
 
 } // namespace rtd

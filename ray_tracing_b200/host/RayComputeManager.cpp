@@ -35,6 +35,7 @@ std::string RtApi::Load(const char* path)
     DispatchFeatures = reinterpret_cast<decltype(DispatchFeatures)>(dlsym(dl, "rtDispatchFeatures"));
     CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
     DenoiseFn = reinterpret_cast<decltype(DenoiseFn)>(dlsym(dl, "rtDenoise"));
+    DenoiseTemporalFn = reinterpret_cast<decltype(DenoiseTemporalFn)>(dlsym(dl, "rtDenoiseTemporal"));
     return "";
 }
 
@@ -360,6 +361,14 @@ int RayComputeManager::Denoise(int iterations, float sigmaColour, float sigmaNor
     if (!ctx) return RT_E_STATE;
     if (!api.DenoiseFn) { lastError = "the library does not export rtDenoise"; return RT_E_STATE; }
     TRY(api.DenoiseFn(ctx, accumulate ? 1 : 0, iterations, sigmaColour, sigmaNormal, sigmaDepth));
+    return RT_OK;
+}
+
+int RayComputeManager::DenoiseTemporal(int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.DenoiseTemporalFn) { lastError = "the library does not export rtDenoiseTemporal"; return RT_E_STATE; }
+    TRY(api.DenoiseTemporalFn(ctx, iterations, sigmaLuminance, sigmaNormal, sigmaDepth, alpha, resetHistory));
     return RT_OK;
 }
 

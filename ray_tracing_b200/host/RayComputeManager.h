@@ -63,6 +63,7 @@ struct RtApi
     decltype(&rtDispatchFeatures) DispatchFeatures = nullptr;   // optional: first-hit feature images (RenderFeatures)
     decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
     decltype(&rtDenoise) DenoiseFn = nullptr;               // optional: the a-trous denoiser (Denoise)
+    decltype(&rtDenoiseTemporal) DenoiseTemporalFn = nullptr;  // optional: the temporal denoiser (DenoiseTemporal)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -153,6 +154,11 @@ public:
     // the accumulated mean when accumulate is on, else the last frame.  The defaults are capi.py's, chosen by the quality sweep of
     // DESIGN.md section 7d.  ReadDenoised: "DenoisedRender", W*H float4, the denoised mean colour.
     int Denoise(int iterations = 5, float sigmaColour = 64.0f, float sigmaNormal = 1.0f, float sigmaDepth = 0.1f);
+    // not in the reference: the temporal denoiser (rtDenoiseTemporal, SVGF) of the last frame, for a moving camera: call it once per
+    // frame after RenderFeatures() and RenderFrame(); resetHistory = 1 on a jump cut.  The defaults are capi.py's, chosen by the
+    // quality sweep of DESIGN.md section 7d.  The result is read with ReadDenoised.
+    int DenoiseTemporal(int iterations = 5, float sigmaLuminance = 8.0f, float sigmaNormal = 1.0f, float sigmaDepth = 0.1f, float alpha = 0.1f,
+                        int resetHistory = 0);
     int ReadDenoised(float* dst, size_t bytes);
     // picking / autofocus: the un-jittered camera ray through pixel (x, y) of the screen — SetupPixel's operations (HL:547-558) on the
     // manager's own camera fields — and its closest hit

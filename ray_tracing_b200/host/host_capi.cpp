@@ -248,6 +248,8 @@ int rcmReadFeatureImage(void* hv, const char* name, void* dst, size_t bytes) { H
 int rcmCameraRays(void* hv, RtPathRay* rays, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->CameraRays(rays, bytes); } CATCH_ALL(h) }
 int rcmDenoise(void* hv, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth)
 { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->Denoise(iterations, sigmaColour, sigmaNormal, sigmaDepth); } CATCH_ALL(h) }
+int rcmDenoiseTemporal(void* hv, int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->DenoiseTemporal(iterations, sigmaLuminance, sigmaNormal, sigmaDepth, alpha, resetHistory); } CATCH_ALL(h) }
 int rcmReadDenoised(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadDenoised(dst, bytes); }
 /* the pick ray through pixel (x, y) into *ray (may be NULL) and its closest hit into *hit (may be NULL: the ray alone) */
 int rcmPick(void* hv, float x, float y, RtRay* ray, RtRayHit* hit)

@@ -71,6 +71,7 @@ def host_lib() -> C.CDLL:
         L.rcmCameraRays.argtypes = [vp, vp, C.c_size_t]
         L.rcmDenoise.argtypes = [vp, ci, cf, cf, cf]
         L.rcmReadDenoised.argtypes = [vp, vp, C.c_size_t]
+        L.rcmDenoiseTemporal.argtypes = [vp, ci, cf, cf, cf, cf, ci]
         L.rcmPick.argtypes = [vp, cf, cf, vp, vp]
         _host = L
     return _host
@@ -356,6 +357,14 @@ class RayComputeManager:
         """rtDenoise over the whole image, guided by the feature images RenderFeatures() left: the accumulated mean when accumulate is
         on, else the last frame.  Read the result with denoised_result."""
         self._ck(self._L.rcmDenoise(self._h, int(iterations), float(sigma_colour), float(sigma_normal), float(sigma_depth)))
+
+    def DenoiseTemporal(self, iterations: int = capi.TEMPORAL_ITERATIONS, sigma_luminance: float = capi.TEMPORAL_SIGMA_LUMINANCE,
+                        sigma_normal: float = capi.TEMPORAL_SIGMA_NORMAL, sigma_depth: float = capi.TEMPORAL_SIGMA_DEPTH,
+                        alpha: float = capi.TEMPORAL_ALPHA, reset_history: bool = False):
+        """rtDenoiseTemporal of the last frame with its reprojected history, for a moving camera: once per frame after RenderFeatures()
+        and RenderFrame(); reset_history on a jump cut.  Read the result with denoised_result."""
+        self._ck(self._L.rcmDenoiseTemporal(self._h, int(iterations), float(sigma_luminance), float(sigma_normal), float(sigma_depth),
+                                            float(alpha), 1 if reset_history else 0))
 
     @property
     def denoised_result(self) -> np.ndarray:

@@ -77,6 +77,15 @@ VARIANTS = {
     "clocks": ("RT_POOL_CLOCKS",),
     # rtDenoise with every tap loaded from global memory instead of the shared-memory sub-lattice tile (tools/denoise_bench.py --ab)
     "denoise_plain": ("RT_DENOISE_PLAIN",),
+    # rtDenoiseTemporal's variance prefilter over the lattice neighbours at +-s from the staged tile instead of SVGF's immediate
+    # neighbours, and its history tolerances (tools/temporal_denoise_bench.py --ab); none of these is bit-exact against the oracle
+    "temporal_lattice": ("RT_TEMPORAL_LATTICE_PREFILTER",),
+    "temporal_tauz02": ("RT_TEMPORAL_TAU_Z=0.02f",),
+    "temporal_tauz10": ("RT_TEMPORAL_TAU_Z=0.1f",),
+    "temporal_tauz20": ("RT_TEMPORAL_TAU_Z=0.2f",),
+    "temporal_taun80": ("RT_TEMPORAL_TAU_N=0.8f",),
+    "temporal_taun95": ("RT_TEMPORAL_TAU_N=0.95f",),
+    "temporal_taun50": ("RT_TEMPORAL_TAU_N=0.5f",),
 }
 OUT_DIR = os.path.join(build.PKG_DIR, "variants")
 
