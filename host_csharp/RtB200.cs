@@ -91,6 +91,10 @@ public static class RtB200
     // "TemporalFrame" (W*H float4 through rtReadback: prevX, prevY, history length, variance); the managers default to 5 iterations,
     // sigmas 8, 1, 0.1, alpha 0.1; resetHistory = 1 on a jump cut
     [DllImport(Lib)] public static extern int rtDenoiseTemporal(IntPtr ctx, int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory);
+    // adaptive sampling: the next accumulated frame only in the pixels whose error estimate is still above threshold; activePixels gets
+    // the number traced (0 = converged).  "AdaptiveMoments" (W*H float4 through rtReadback); rtDisplayMean shows A / A.w per pixel.
+    [DllImport(Lib)] public static extern int rtDispatchAdaptive(IntPtr ctx, int gx, int gy, int gz, float threshold, int minFrames, int maxFrames, out long activePixels);
+    [DllImport(Lib)] public static extern int rtDisplayMean(IntPtr ctx, [Out] byte[] dst, UIntPtr bytes);
     // multi-GPU inside the boundary.  A Unity host is ONE process: rtCreateMulti(out ctx, null, 8) instead of rtCreate, and nothing else changes —
     // every rtSet* / rtSetBuffer reaches all GPUs, rtDispatch(kernelRayTrace) traces tile r of 8 on GPU r and ends with the NCCL all-gather of the frame's
     // tiles, rtReadback / rtDisplay read GPU 0.  One process per GPU instead: rtGetUniqueId on rank 0, rtCommInit on every rank.

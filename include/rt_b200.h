@@ -367,6 +367,46 @@ int rtDisplayDenoised(RtContext* ctx, uint8_t* dst, size_t bytes);
 #define RT_TEMPORAL_EPSILON 0.0000152587890625f     /* 2^-16 */
 int rtDenoiseTemporal(RtContext* ctx, int iterations, float sigmaLuminance, float sigmaNormal, float sigmaDepth, float alpha, int resetHistory);
 
+/* Extension: adaptive sampling.  One call renders the next frame of a progressive accumulation only in the pixels whose estimated error
+ * is still above `threshold`.  Covered pixels are those rtDispatch(RT_KERNEL_RAYTRACE, groupsX, groupsY, groupsZ) covers (8x8 groups,
+ * partial dispatch, this context's rtSetTile row bands).
+ *   - "AdaptiveMoments": W*H float4, [y][x], row 0 = bottom; per pixel (s1, s2, n, 0) = the sums of l and l*l and the number of frames
+ *     over the frames rtDispatchAdaptive traced there.  It counts adaptive frames only: rtDispatch, rtDispatchFrames and rtResetStats
+ *     leave it alone.
+ *   - Selection, per covered pixel, on the moments as they were before the call (binary32, one operation each in the order written,
+ *     no contraction; max ignores NaN):
+ *         mu = s1 / n;   v = max(s2 / n - mu * mu, 0)
+ *         active = n < (float)minFrames || (n < (float)maxFrames && v > ((threshold * threshold) * n) * (mu * mu + RT_ADAPTIVE_EPSILON))
+ *     i.e. the standard error of the mean luminance is above threshold times the mean, with an absolute floor for dark pixels.  A pixel
+ *     whose moments are not finite becomes inactive after minFrames (the comparison with NaN is false); maxFrames bounds every pixel.
+ *   - Tracing: each active pixel is traced exactly as rtDispatch(RAYTRACE) traces it at the current "Frame" (FrameRender,
+ *     AccumulatedRender, PixelStats with "countStats" = 1 and the traversal counters, bit for bit); then, with (r, g, b) the frame
+ *     colour it wrote, l = (0.2126f * r + 0.7152f * g) + 0.0722f * b (rtDenoiseTemporal's lum) and AdaptiveMoments = (s1 + l,
+ *     s2 + l * l, n + 1, 0).  Inactive and uncovered pixels are not touched in any image.  Which lane traces which pixel, and in which
+ *     order, changes no bit.
+ *   - *activePixels (may be NULL) receives the number of pixels traced.  The call synchronises once, between the device-side selection
+ *     and the render launch, and returns with the render queued.  With at least one active pixel RtStats.dispatches grows by 1, kernelMs
+ *     by the render launch's time, rays and the test counters by what was traced; with none, nothing is rendered and no RtStats field
+ *     changes.  "Frame" is read and not advanced, as in rtDispatch.
+ *   - Memory: AdaptiveMoments is allocated, zero-filled, by the first call, with a pixel list: 20 bytes of device memory per pixel plus
+ *     4 bytes per 32 pixels of selection scratch.  rtResize to a new size zeroes it; rtDispatch(RT_KERNEL_RESET_ACCUMULATED, ...) zeroes
+ *     the region it covers.  A context that never calls rtDispatchAdaptive allocates none of it.  rtReadback and rtGetDevicePointer
+ *     accept "AdaptiveMoments" (W*H*16 bytes); RT_E_STATE before the first call.
+ *   - Refused: ctx NULL, a negative group count, threshold not finite or < 0 or threshold * threshold not finite, minFrames < 2,
+ *     maxFrames < minFrames or > RT_ADAPTIVE_MAX_FRAMES -> RT_E_INVALID; every state refusal of rtDispatch, "accumulate" = 0,
+ *     "sampleChunks" forced to 2 or more, a group context (rtCreateMulti), a context with a communicator (rtCommInit) or with peers
+ *     (rtSetPeers) -> RT_E_STATE.  A refused call changes nothing.
+ * rtDisplayMean: W*H RGBA8, [y][x]: (0, 0, 0, 255) where AccumulatedRender.w == 0, else rtDisplay's encode of all four components of
+ * A / A.w (the per-pixel mean of an adaptively sampled image).  Where every A.w equals "Frame" it is byte-equal to rtDisplay(1, Frame).
+ * bytes != W*H*4 -> RT_E_INVALID.  Its scratch is the W*H float4 image rtReadbackAsync snapshots into (allocated by the first use of
+ * either).  Synchronises. */
+#ifndef RT_ADAPTIVE_EPSILON                /* overridable only by the A/B build variants of tools/build_variants.py */
+#define RT_ADAPTIVE_EPSILON 0.00390625f    /* 2^-8 */
+#endif
+#define RT_ADAPTIVE_MAX_FRAMES (1 << 24)    /* the frame count is a binary32 in the moments image: exact up to 2^24 */
+int rtDispatchAdaptive(RtContext* ctx, int groupsX, int groupsY, int groupsZ, float threshold, int minFrames, int maxFrames, int64_t* activePixels);
+int rtDisplayMean(RtContext* ctx, uint8_t* dst, size_t bytes);
+
 /* Replaces: reading the RenderTexture back (ComputeHelper.ReadbackData / AsyncGPUReadback; the
  * reference itself only samples it on-GPU in Display.shader).  tex ∈ {"FrameRender",
  * "AccumulatedRender"}; dst receives W·H float4 in [y][x] order (row 0 = bottom of the view plane),

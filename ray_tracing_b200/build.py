@@ -96,10 +96,11 @@ def build_oracle(force: bool = False) -> str:
     # (tests/oracle_ext/rt_oracle_paths.cpp); rtDispatchFeatures / rtCameraRays are its camera sample, CalculateRayCollision and
     # GetMaterialColour per pixel around that (tests/oracle_ext/rt_oracle_features.cpp); rtDenoise is the a-trous filter over those
     # images around that (tests/oracle_ext/rt_oracle_denoise.cpp); rtDenoiseTemporal is the reprojected, variance-guided filter with its
-    # history around that (tests/oracle_ext/rt_oracle_temporal.cpp, the translation unit built here)
+    # history around that (tests/oracle_ext/rt_oracle_temporal.cpp); rtDispatchAdaptive is the selection on its moments and Kernel_RayTrace
+    # per active pixel around that (tests/oracle_ext/rt_oracle_adaptive.cpp, the translation unit built here)
     srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(ORACLE_EXT, (".cpp",)) + _glob(INCLUDE, (".h",))
     if force or _newer(LIB_ORACLE, srcs):
-        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_temporal.cpp")])
+        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_adaptive.cpp")])
     return LIB_ORACLE
 
 

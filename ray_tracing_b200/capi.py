@@ -139,6 +139,12 @@ TEMPORAL_SIGMA_DEPTH = 0.1
 TEMPORAL_ALPHA = 0.1
 TEMPORAL_MAX_HISTORY = 32          # RT_TEMPORAL_MAX_HISTORY
 
+# rtDispatchAdaptive: the defaults of the managers, chosen by the quality sweep of DESIGN.md section 7d''''''''
+ADAPTIVE_MAX_FRAMES_LIMIT = 1 << 24     # RT_ADAPTIVE_MAX_FRAMES
+ADAPTIVE_THRESHOLD = 0.2
+ADAPTIVE_MIN_FRAMES = 8
+ADAPTIVE_MAX_FRAMES = 64
+
 
 class RtStats(C.Structure):
     _fields_ = [("rays", C.c_uint64), ("boxTests", C.c_uint64), ("triTests", C.c_uint64), ("sphereTests", C.c_uint64),
@@ -213,13 +219,16 @@ class RtLib:
             "rtDenoise": ([vp, ci, ci, cf, cf, cf], ci),
             "rtDisplayDenoised": ([vp, vp, C.c_size_t], ci),
             "rtDenoiseTemporal": ([vp, ci, cf, cf, cf, cf, ci], ci),
+            "rtDispatchAdaptive": ([vp, ci, ci, ci, cf, ci, ci, C.POINTER(C.c_int64)], ci),
+            "rtDisplayMean": ([vp, vp, C.c_size_t], ci),
         }
         for name, (args, res) in sig.items():
             if not hasattr(L, name):
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
                             "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
-                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal"):      # absent from older experimental builds used in A/B runs
+                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
+                            "rtDispatchAdaptive", "rtDisplayMean"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
             fn = getattr(L, name)
@@ -330,6 +339,29 @@ class RtContext:
         gx = (self.width + 7) // 8 if gx is None else gx
         gy = (self.height + 7) // 8 if gy is None else gy
         self._ck(self._L.rtDispatchFrames(self._h, int(gx), int(gy), int(gz), int(n)))
+
+    def dispatch_adaptive(self, threshold: float = ADAPTIVE_THRESHOLD, min_frames: int = ADAPTIVE_MIN_FRAMES, max_frames: int = ADAPTIVE_MAX_FRAMES,
+                          gx: Optional[int] = None, gy: Optional[int] = None, gz: int = 1) -> int:
+        """rtDispatchAdaptive: the next accumulated RayTrace frame of the current "Frame", traced only in the covered pixels whose
+        estimated error is still above `threshold` (or that have fewer than min_frames adaptive frames); their luminance moments go to
+        "AdaptiveMoments" (adaptive_moments()).  Returns the number of pixels traced: 0 = converged.  Groups default to the whole image.
+        Synchronises once before the render launch, which stays queued."""
+        gx = (self.width + 7) // 8 if gx is None else gx
+        gy = (self.height + 7) // 8 if gy is None else gy
+        active = C.c_int64(0)
+        self._ck(self._L.rtDispatchAdaptive(self._h, int(gx), int(gy), int(gz), float(threshold), int(min_frames), int(max_frames), C.byref(active)))
+        return int(active.value)
+
+    def adaptive_moments(self) -> np.ndarray:
+        """"AdaptiveMoments": (H, W, 4) float32, row 0 = bottom, (sum of l, sum of l*l, frames, 0) per pixel over its adaptive frames."""
+        return self.readback("AdaptiveMoments")
+
+    def display_mean(self) -> np.ndarray:
+        """rtDisplayMean: the per-pixel mean AccumulatedRender / AccumulatedRender.w encoded as rtDisplay encodes; (0, 0, 0, 255)
+        where nothing was accumulated.  (H, W, 4) uint8, row 0 = bottom."""
+        out = np.empty((self.height, self.width, 4), dtype=np.uint8)
+        self._ck(self._L.rtDisplayMean(self._h, out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out
 
     def trace_rays(self, rays, dirs=None, no_cull: bool = False) -> np.ndarray:
         """rtTraceRays: the closest hit of every ray against the current scene, as the path tracer computes it.  rays: a RAY_DTYPE

@@ -13,6 +13,7 @@
 #include "rt_kernel_features.cuh"
 #include "rt_kernel_denoise.cuh"
 #include "rt_kernel_temporal.cuh"
+#include "rt_kernel_adaptive.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -116,6 +117,9 @@ struct RtContext
     DevBuf<float4> temporalFrame, temporalHist;
     int temporalSet = 0; bool temporalHistory = false;
     float temporalCam[16] = {}, temporalVP[3] = {};
+    // rtDispatchAdaptive: "AdaptiveMoments" (W*H, allocated zero-filled by the first traced call), the pixel list (W*H), the selection's
+    // scratch (a ballot word per 32 jobs, then the block counts and the list length) and the pinned word the length is read into
+    DevBuf<float4> moments; DevBuf<unsigned int> adaptiveList, adaptiveScratch; unsigned int* adaptiveCount = nullptr;
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -227,6 +231,8 @@ int rtDestroy(RtContext* c)
     c->pixelStats.release(); c->queryRays.release(); c->queryHits.release();
     c->featureFrame.release(); c->accumAlbedo.release(); c->accumNormal.release(); c->cameraRays.release();
     c->denoised.release(); c->denoiseScratch.release(); c->temporalFrame.release(); c->temporalHist.release();
+    c->moments.release(); c->adaptiveList.release(); c->adaptiveScratch.release();
+    if (c->adaptiveCount) cudaFreeHost(c->adaptiveCount);
     c->repack.release();
     closePeers(c);
     for (auto& ev : c->pending) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
@@ -408,6 +414,12 @@ static int one_rtResize(RtContext* c, int w, int h)
             CK(cudaMemsetAsync(c->temporalFrame.p, 0, n * 16, c->stream));
         }
         c->temporalHist.release(); c->temporalHistory = false;
+        if (c->moments.p)                                   // the moments start again from zero
+        {
+            CK(c->moments.ensure(n));
+            CK(cudaMemsetAsync(c->moments.p, 0, n * 16, c->stream));
+        }
+        c->adaptiveList.release(); c->adaptiveScratch.release();
         c->cameraRays.release();
         c->width = w; c->height = h;
         c->tileSend.release(); c->tileRecv.release();
@@ -716,9 +728,15 @@ static void bindScene(const RtContext* c, DevParams& P)
     P.tlasRootStart = c->repack.tlasRootStart; P.tlasRootCount = c->repack.tlasRootCount;
 }
 
+// rtDispatchAdaptive's arguments (dispatchLocal); `active` receives the number of pixels traced
+struct AdaptiveCall { float threshold; int minFrames, maxFrames; long long active; };
+
+static int adaptiveSelect(RtContext* c, unsigned limX, unsigned limY, AdaptiveCall& ad);
+
 // One GPU's share of a dispatch: the RayTrace kernel over this context's tile (the whole image without rtSetTile).
 // frames > 1 (rtDispatchFrames, RayTrace only): frames Frame .. Frame + frames - 1 in one launch of a FRAMES kernel.
-static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, int frames = 1)
+// ad (rtDispatchAdaptive, RayTrace only): the selected pixels only, in one launch of a list-driven kernel.
+static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, int frames = 1, AdaptiveCall* ad = nullptr)
 {
     if (!c || gx < 0 || gy < 0 || gz < 0) return fail(c, RT_E_INVALID, "rtDispatch: bad argument");
     if (c->width == 0) return fail(c, RT_E_STATE, "rtDispatch: rtResize has not been called");
@@ -738,6 +756,8 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
             CK(cudaMemset2DAsync(c->accumAlbedo.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
             CK(cudaMemset2DAsync(c->accumNormal.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
         }
+        if (c->moments.p)                                      // so are the adaptive moments
+            CK(cudaMemset2DAsync(c->moments.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
         return RT_OK;
     }
     if (kernelIndex != RT_KERNEL_RAYTRACE) return fail(c, RT_E_INVALID, "rtDispatch: kernelIndex must be 0 (RayTrace) or 1 (ResetAccumulated)");
@@ -753,8 +773,24 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
         c->dispatchPixels = rows * limX;
     }
     c->dispatchFrames = frames;
-    int rc = prepareScene(c);
+    int rc = RT_OK;
+    if (ad)
+    {
+        // the selection (one synchronisation: the host sizes the launch and chooses the kernel from the count, as for an image of that
+        // many pixels); before the scene is prepared, so that the kernel choice sees the count
+        if ((rc = checkScene(c, "rtDispatchAdaptive")) != RT_OK) return rc;
+        if ((rc = adaptiveSelect(c, limX, limY, *ad)) != RT_OK) return rc;
+        if (ad->active == 0) return RT_OK;
+        c->dispatchPixels = (unsigned long long)ad->active;
+    }
+    rc = prepareScene(c);
     if (rc != RT_OK) return rc;
+    if (ad && !c->moments.p)                               // the first traced call allocates the moments, zero-filled
+    {
+        const size_t n = (size_t)W * H;
+        CK(c->moments.ensure(n));
+        CK(cudaMemsetAsync(c->moments.p, 0, n * 16, c->stream));
+    }
     applyL2Persistence(c);
     if (c->optCountStats && !c->pixelStats.p)              // the first counting dispatch allocates the per-pixel counters
     {
@@ -794,7 +830,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     // sample chunks (small tiles): a pixel's chain may change lanes / slots between samples; the hand-off buffers belong to the context
     // (kernel 1 only: in the pooled kernel the same hand-off was slower than whole pixels on small tiles and was taken out again)
     P.chunks = kernel == 1 ? wave_chunks(c->optSampleChunks, c->numSMs, c->dispatchPixels, P.NumRaysPerPixel, P.modelCount) : 1;
-    if (c->dispatchPixels == 0 || frames > 1) P.chunks = 1;      // a rank whose tile is empty (an image lower than the band pattern); a batch of frames runs whole pixels
+    if (c->dispatchPixels == 0 || frames > 1 || ad) P.chunks = 1;      // a rank whose tile is empty (an image lower than the band pattern); a batch of frames or a pixel list runs whole pixels
     if (P.chunks > 1)
     {
         unsigned long long rows = limX ? c->dispatchPixels / limX : 0;
@@ -811,7 +847,33 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
         }
         P.handoff = c->handoff.p; P.chunkSerial = (int)c->chunkSerial;
     }
-    if (kernel == 0)
+    if (ad)
+    {
+        const unsigned count = (unsigned)ad->active;
+        cudaError_t e = cudaSuccess;
+        if (kernel == 0)
+        {
+            CK(cudaEventRecord(ev.a, c->stream));
+            RT_LAUNCH((count + 63u) / 64u, 64, 0, c->stream, k_raytrace_mega_list<64>, P, count, c->adaptiveList.p, c->moments.p);
+            CK(cudaEventRecord(ev.b, c->stream));
+        }
+        else if (kernel == 1)
+        {
+            P.pixelList = c->adaptiveList.p; P.adaptiveMoments = c->moments.p;       // (the hand-off's and the cold pool's slots: unused here)
+            e = wave_launch_list(P, c->numSMs, count, c->stream, ev.a, ev.b);
+        }
+        else
+        {
+            if (POOL_COLD_WORDS > 0)
+            {
+                CK(c->poolCold.ensure((size_t)c->numSMs * POOL_WARPS * POOL_COLD_WORDS * 96));
+                P.poolCold = c->poolCold.p;
+            }
+            e = pool_launch_list(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b, count, c->adaptiveList.p, c->moments.p);
+        }
+        if (e != cudaSuccess) return failCuda(c, e, "adaptive launch");
+    }
+    else if (kernel == 0)
     {
         CK(cudaEventRecord(ev.a, c->stream));
         dim3 grid((limX + 7) / 8, (limY + 7) / 8, 1), block(8, 8, 1);
@@ -856,10 +918,12 @@ int rtReadback(RtContext* c, const char* tex, float* dst, size_t bytes)
     if (feature) { int rc = featuresReady(c, "rtReadback"); if (rc != RT_OK) return rc; }
     if (n == "DenoisedRender" && !c->denoised.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoise yet");
     if (n == "TemporalFrame" && !c->temporalFrame.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoiseTemporal yet");
+    if (n == "AdaptiveMoments" && !c->moments.p) return fail(c, RT_E_STATE, "rtReadback: no rtDispatchAdaptive yet");
     const void* src = n == "FrameRender" ? (const void*)c->frame.p : n == "AccumulatedRender" ? (const void*)c->accum.p : n == "FeatureFrame" ? (const void*)c->featureFrame.p :
                       n == "AccumulatedAlbedo" ? (const void*)c->accumAlbedo.p : n == "AccumulatedNormal" ? (const void*)c->accumNormal.p :
-                      n == "DenoisedRender" ? (const void*)c->denoised.p : n == "TemporalFrame" ? (const void*)c->temporalFrame.p : nullptr;
-    if (n != "FrameRender" && n != "AccumulatedRender" && n != "DenoisedRender" && n != "TemporalFrame" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
+                      n == "DenoisedRender" ? (const void*)c->denoised.p : n == "TemporalFrame" ? (const void*)c->temporalFrame.p :
+                      n == "AdaptiveMoments" ? (const void*)c->moments.p : nullptr;
+    if (n != "FrameRender" && n != "AccumulatedRender" && n != "DenoisedRender" && n != "TemporalFrame" && n != "AdaptiveMoments" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
     if (!src) return fail(c, RT_E_STATE, "rtReadback: rtResize has not been called");
     if (bytes != (size_t)c->width * c->height * (n == "FeatureFrame" ? sizeof(RtPixelFeatures) : 16))
         return fail(c, RT_E_INVALID, n == "FeatureFrame" ? "rtReadback: bytes must equal W*H*32" : "rtReadback: bytes must equal W*H*16");
@@ -1094,6 +1158,72 @@ int rtDispatchFrames(RtContext* c, int gx, int gy, int gz, int frameCount)
     std::vector<RtContext*> all(1, c);                      // one exchange for the whole batch: it carries the last frame and the sum
     all.insert(all.end(), c->followers.begin(), c->followers.end());
     return exchangeTiles(all.data(), (int)all.size());
+}
+
+// rtDispatchAdaptive's selection over this context's covered pixels, in the camera kernels' job order: the list and its length, read
+// back into ad.active (the call's one synchronisation).  Before the first traced call the moments are all zero (none allocated yet).
+static int adaptiveSelect(RtContext* c, unsigned limX, unsigned limY, AdaptiveCall& ad)
+{
+    unsigned int ownedRows = 0;
+    for (unsigned int y0 = 0, b = 0; y0 < limY; y0 += (unsigned int)c->bandRows, b++)
+        if ((int)(b % (unsigned int)c->tileWorld) == c->tileRank) ownedRows += (limY - y0) < (unsigned int)c->bandRows ? (limY - y0) : (unsigned int)c->bandRows;
+    const unsigned int tilesX = (limX + 7u) / 8u;
+    const unsigned long long jobs = (unsigned long long)tilesX * ((ownedRows + 3u) / 4u) * 32ull;       // < 2^32: W, H <= 65535
+    const unsigned int nBlocks = (unsigned int)((jobs + ADAPTIVE_BLOCK - 1) / ADAPTIVE_BLOCK);
+    const size_t n = (size_t)c->width * c->height;
+    CK(c->adaptiveList.ensure(n));
+    CK(c->adaptiveScratch.ensure((size_t)(jobs / 32) + nBlocks + 1));
+    if (!c->adaptiveCount) CK(cudaMallocHost((void**)&c->adaptiveCount, sizeof(unsigned int)));
+    AdaptiveParams A;
+    A.moments = c->moments.p;
+    A.masks = c->adaptiveScratch.p; A.partials = A.masks + jobs / 32; A.count = A.partials + nBlocks; A.list = c->adaptiveList.p;
+    A.W = c->P.W; A.limX = limX; A.ownedRows = ownedRows; A.tilesX = tilesX; A.totalJobs = (unsigned int)jobs; A.nBlocks = nBlocks;
+    A.tileRank = c->tileRank; A.tileWorld = c->tileWorld; A.bandRows = c->bandRows;
+    A.threshold = ad.threshold; A.minFrames = (float)ad.minFrames; A.maxFrames = (float)ad.maxFrames;
+    cudaError_t e = adaptive_select(A, c->stream);
+    if (e != cudaSuccess) return failCuda(c, e, "adaptive selection");
+    CK(cudaMemcpyAsync(c->adaptiveCount, A.count, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    ad.active = (long long)*c->adaptiveCount;
+    return RT_OK;
+}
+
+int rtDispatchAdaptive(RtContext* c, int gx, int gy, int gz, float threshold, int minFrames, int maxFrames, int64_t* activePixels)
+{
+    if (!c || gx < 0 || gy < 0 || gz < 0) return fail(c, RT_E_INVALID, "rtDispatchAdaptive: bad argument");
+    if (!std::isfinite(threshold) || threshold < 0.0f || !std::isfinite(threshold * threshold))
+        return fail(c, RT_E_INVALID, "rtDispatchAdaptive: threshold must be finite and >= 0, with a finite square");
+    if (minFrames < 2) return fail(c, RT_E_INVALID, "rtDispatchAdaptive: minFrames must be at least 2");
+    if (maxFrames < minFrames || maxFrames > RT_ADAPTIVE_MAX_FRAMES)
+        return fail(c, RT_E_INVALID, "rtDispatchAdaptive: maxFrames must lie in minFrames .. RT_ADAPTIVE_MAX_FRAMES");
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDispatchAdaptive: not available on a group context (rtCreateMulti)");
+    if (c->comm) return fail(c, RT_E_STATE, "rtDispatchAdaptive: not available on a context with a communicator (rtCommInit)");
+    if (c->nPeers > 0) return fail(c, RT_E_STATE, "rtDispatchAdaptive: not available on a context with peers (rtSetPeers)");
+    if (!c->P.accumulate) return fail(c, RT_E_STATE, "rtDispatchAdaptive: needs accumulate = 1 (the moments count accumulated frames)");
+    if (c->optSampleChunks >= 2) return fail(c, RT_E_STATE, "rtDispatchAdaptive: a pixel list runs whole pixels; sampleChunks is forced to 2 or more");
+    AdaptiveCall ad; ad.threshold = threshold; ad.minFrames = minFrames; ad.maxFrames = maxFrames; ad.active = 0;
+    const int rc = dispatchLocal(c, RT_KERNEL_RAYTRACE, gx, gy, gz, 1, &ad);
+    if (rc != RT_OK) return rc;
+    if (activePixels) *activePixels = (int64_t)ad.active;
+    return RT_OK;
+}
+
+int rtDisplayMean(RtContext* c, uint8_t* dst, size_t bytes)
+{
+    if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplayMean: bad argument");
+    if (!c->accum.p) return fail(c, RT_E_STATE, "rtDisplayMean: rtResize has not been called");
+    const size_t n = (size_t)c->width * c->height;
+    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplayMean: bytes must equal W*H*4");
+    CK(cudaSetDevice(c->device));
+    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
+    CK(c->display.ensure(n));
+    CK(c->snap.ensure(n));                                  // the pipelined readback's snapshot image is free here (the copy was waited for)
+    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_mean_image, c->accum.p, c->snap.p, n);
+    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, c->snap.p, c->display.p, n, 1.0f);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
 }
 
 // ---- closest-hit and occlusion queries (rtTraceRays, rtTraceOcclusion, rt_kernel_query.cuh) -----------------------------------------
@@ -1632,6 +1762,11 @@ int rtGetDevicePointer(RtContext* c, const char* name, void** devPtr, size_t* by
     {
         if (!c->temporalFrame.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: TemporalFrame is allocated by the first rtDenoiseTemporal");
         *devPtr = c->temporalFrame.p; *bytes = c->temporalFrame.count * 16;
+    }
+    else if (n == "AdaptiveMoments")
+    {
+        if (!c->moments.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: AdaptiveMoments is allocated by the first rtDispatchAdaptive");
+        *devPtr = c->moments.p; *bytes = c->moments.count * 16;
     }
     else if (n == "TileSend" || n == "TileRecv")
     {

@@ -206,11 +206,14 @@ struct DevParams
     // kernel 1 on small tiles: a pixel's samples in `chunks` consecutive jobs (1 = whole pixels); the RNG state and the running sum travel
     // from one chunk to the next through `handoff`: four 64-bit words per pixel job, each {tag, value} with tag = chunkSerial << 8 | chunks
     // completed, so that every word validates itself (aligned 8-byte stores are single-copy atomic: no fence, no flag)
-    int   chunks, chunkSerial; unsigned long long* handoff;
+    // rtDispatchAdaptive's kernel-1 list instantiations (never chunked) take their pixel list in the same slot, and the moments in
+    // poolCold's (kernel 2 only): the slots keep the parameter layout, and wave_body's signature, of every existing kernel
+    int   chunks, chunkSerial;
+    union { unsigned long long* handoff; const unsigned int* pixelList; };
     // "countStats" launches: the W*H per-pixel counters ([y][x], RtPixelStats).  Only the instrumented code reads it (kept at the
     // offset of a retired pointer so that the parameter layout of every kernel stays where it was)
     RtPixelStats* pixelStats;
-    float* poolCold;                        // kernel 2 built with RT_POOL_COLD_GLOBAL: the per-warp blocks of the slot fields kept out of shared memory
+    union { float* poolCold; float4* adaptiveMoments; };   // kernel 2 built with RT_POOL_COLD_GLOBAL: the per-warp blocks of the slot fields kept out of shared memory
 };
 
 struct Counters { unsigned int rays, box, tri, sph, sbox; };
@@ -231,9 +234,18 @@ RT_DI void AddPixelStats(const DevParams& P, size_t o, const Counters& now, cons
 // RC:18-23: write the pixel of this frame and accumulate; with peers, also store both values into every peer GPU's copy
 // (the all-gather of finished tiles fused into the producing kernel: 32 bytes per pixel per peer over NVLink).
 // EXT = the launch has peers (or another extension) — the common single-GPU instantiation carries no trace of them.
-template <bool EXT>
-__device__ __forceinline__ void WritePixel(const DevParams& P, size_t o, float r, float g, float b)
+// ADAPTIVE = the list-driven kernels of rtDispatchAdaptive: the accumulating write also adds the frame's luminance to the pixel's
+// moments (s1 + l, s2 + l*l, n + 1) in `moments` (AdaptiveMoments; the call is refused without accumulation).
+template <bool EXT, bool ADAPTIVE = false>
+__device__ __forceinline__ void WritePixel(const DevParams& P, size_t o, float r, float g, float b, float4* moments = nullptr)
 {
+    if constexpr (ADAPTIVE)
+    {
+        const float l = (0.2126f * r + 0.7152f * g) + 0.0722f * b;
+        float4 m = moments[o];
+        m.x += l; m.y += l * l; m.z += 1.0f;
+        moments[o] = m;
+    }
     const float4 f = make_float4(r, g, b, 1.0f);
     float4 a = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 #if defined(RT_STREAM_IMAGES) && !defined(RT_SIMT_EMU)

@@ -201,4 +201,41 @@ __global__ void __launch_bounds__(64) k_raytrace_mega_frames(const __grid_consta
     FlushCounters(P, cnt);
 }
 
+// rtDispatchAdaptive: k_raytrace_mega over the `count` pixels of the selection's list ((y << 16) | x each), a 1-D grid of BLOCK-thread
+// blocks; the write also updates the pixel's moments.  (A kernel of its own, so that k_raytrace_mega keeps its code; and a template,
+// instantiated where rt_api.cu launches it: defined here as a plain kernel, it moved ahead of the wavefront kernels in the module and
+// the compiler then numbered the registers of the k_raytrace_wave_frames kernels differently.)
+template <unsigned int BLOCK>
+__global__ void __launch_bounds__(BLOCK) k_raytrace_mega_list(const __grid_constant__ DevParams P, const unsigned int count,
+                                                              const unsigned int* __restrict__ list, float4* __restrict__ moments)
+{
+    const unsigned int job = blockIdx.x * BLOCK + threadIdx.x;
+    if (job >= count) return;
+    const unsigned int xy = list[job];
+    const unsigned int idx = xy & 0xffffu, idy = xy >> 16;
+
+    Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
+    const PixelSetup px = SetupPixel(P, idx, idy);
+    uint32_t rngState = px.rngState;
+    f3 totalIncomingLight = splat3(0.0f);
+
+    for (int rayIndex = 0; rayIndex < P.NumRaysPerPixel; rayIndex++)
+    {
+        PathState ray;
+        GenerateCameraRay(P, px, rngState, ray);
+        for (int i = 0; i <= P.MaxBounceCount; i++)
+        {
+            const Hit hit = CalculateRayCollision_ref(P, ray.pos, ray.dir, cnt);
+            if (!ShadeSegment(P, hit, ray, rngState)) break;
+        }
+        totalIncomingLight = totalIncomingLight + ray.totalLight;
+    }
+    const f3 pixelCol = totalIncomingLight / __int2float_rn(P.NumRaysPerPixel);
+
+    const size_t o = (size_t)idy * P.W + idx;
+    WritePixel<true, true>(P, o, pixelCol.x, pixelCol.y, pixelCol.z, moments);
+    if (P.countStats) { Counters zero; zero.rays = zero.box = zero.tri = zero.sph = zero.sbox = 0; AddPixelStats(P, o, cnt, zero); }
+    FlushCounters(P, cnt);
+}
+
 } // namespace rtd

@@ -268,9 +268,13 @@ template <int M> RT_DI int CompactRaysByOctant(const PoolView<M>& pool, unsigned
 // FRAMES = the batch instantiations of rtDispatchFrames: a slot keeps its pixel for frames Frame .. Frame + P.frames - 1.  The sample
 // field of the info word counts the samples of all of them (frame = sample / NumRaysPerPixel); when a frame's samples end the slot
 // writes and accumulates that frame, reseeds and starts the next one instead of freeing itself.
-template <bool STATS, bool EXT, bool TLAS, int M, bool FRAMES = false>
-RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const unsigned int tilesX, const unsigned int ownedRows)
+// LIST = the list-driven instantiations of rtDispatchAdaptive: the refill takes job < totalJobs -> list[job] ((y << 16) | x), and the
+// pixel's write also updates its moments.
+template <bool STATS, bool EXT, bool TLAS, int M, bool FRAMES = false, bool LIST = false>
+RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const unsigned int tilesX, const unsigned int ownedRows,
+                     const unsigned int* list = nullptr, float4* moments = nullptr)
 {
+    static_assert(!(LIST && FRAMES), "a pixel list runs one frame");
     RT_DYNAMIC_SMEM(smemRaw);
     WaveSmemHeader* hdr = reinterpret_cast<WaveSmemHeader*>(smemRaw);
     float4* smemPairs = reinterpret_cast<float4*>(smemRaw + sizeof(WaveSmemHeader));
@@ -424,7 +428,7 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                             const unsigned xy = pool.u(F_XY, e);
                             const size_t o = (size_t)(xy >> 16) * P.W + (xy & 0xffffu);
                             const f3 pixelCol = sum / __int2float_rn(P.NumRaysPerPixel);
-                            WritePixel<EXT>(P, o, pixelCol.x, pixelCol.y, pixelCol.z);
+                            WritePixel<EXT, LIST>(P, o, pixelCol.x, pixelCol.y, pixelCol.z, moments);
                             state = PS_EMPTY;
                             if (FRAMES && sample < (unsigned)P.NumRaysPerPixel * (unsigned)P.frames)
                             {
@@ -467,7 +471,15 @@ RT_DI void pool_body(const DevParams& P, const unsigned int totalJobs, const uns
                 if (need)
                 {
                     const unsigned job = base + (unsigned)__popc(needMask & ltMask);
-                    if (job < totalJobs)
+                    if (LIST && job < totalJobs)
+                    {
+                        const unsigned xy = list[job];
+                        pool.u(F_XY, e) = xy;
+                        pool.u(F_RNG, e) = SetupPixel(P, xy & 0xffffu, xy >> 16).rngState;
+                        pool.set3(F_SUM, e, splat3(0.0f));
+                        pool.u(F_INFO, e) = info_pack(0, 0, PS_GEN);
+                    }
+                    else if (!LIST && job < totalJobs)
                     {
                         const unsigned tile = job >> 5, l = job & 31u;
                         const unsigned x = (tile % tilesX) * 8u + (l & 7u);
@@ -863,6 +875,22 @@ __global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_tlas_frames(c
     pool_body<false, true, true, M, true>(P, totalJobs, tilesX, ownedRows);
 }
 
+// rtDispatchAdaptive: the selection's pixel list (totalJobs = its length), one frame per pixel (kernels of their own, so that the
+// kernels above keep their code)
+template <bool STATS, bool EXT, int M>
+__global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_list(const __grid_constant__ DevParams P, const unsigned int totalJobs,
+                                                                       const unsigned int* __restrict__ list, float4* __restrict__ moments)
+{
+    pool_body<STATS, EXT, false, M, false, true>(P, totalJobs, 0u, 0u, list, moments);
+}
+
+template <int M>
+__global__ void __launch_bounds__(POOL_THREADS, 1) k_raytrace_pool_tlas_list(const __grid_constant__ DevParams P, const unsigned int totalJobs,
+                                                                            const unsigned int* __restrict__ list, float4* __restrict__ moments)
+{
+    pool_body<false, true, true, M, false, true>(P, totalJobs, 0u, 0u, list, moments);
+}
+
 template <int M> inline size_t pool_smem_bytes(const DevParams& P)
 {
     const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
@@ -882,6 +910,11 @@ template <int M> inline cudaError_t pool_configure_one()
     if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas_frames<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<false, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas_list<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
     return cudaFuncSetAttribute(k_raytrace_pool<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
 }
 inline cudaError_t pool_configure()
@@ -948,6 +981,39 @@ inline cudaError_t pool_launch(const DevParams& P, int M, int numSMs, cudaStream
     if (M == 32) return pool_launch_m<32>(P, numSMs, stream, evA, evB, totalJobs, tilesX, ownedRows);
     if (M == 64) return pool_launch_m<64>(P, numSMs, stream, evA, evB, totalJobs, tilesX, ownedRows);
     if (M == 96) return pool_launch_m<96>(P, numSMs, stream, evA, evB, totalJobs, tilesX, ownedRows);
+    return cudaErrorInvalidValue;
+}
+
+// rtDispatchAdaptive: kernel 2 over the `count` pixels of `list`, sized from the count and chosen like pool_launch_m's kernels
+template <int M> inline cudaError_t pool_launch_list_m(const DevParams& P, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB,
+                                                       unsigned count, const unsigned* list, float4* moments)
+{
+    const size_t smemBytes = pool_smem_bytes<M>(P);
+    if (smemBytes > 227 * 1024) return cudaErrorInvalidConfiguration;
+    unsigned grid = (unsigned)numSMs;
+    const unsigned ctasNeeded = (count + POOL_WARPS - 1) / POOL_WARPS;
+    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
+    grid = fit_persistent_grid(P.gridFit, grid, POOL_WARPS * M, count);
+    cudaError_t e;
+    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
+    if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
+    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;
+    if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<true, true, M>), P, count, list, moments);
+                        else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<true, false, M>), P, count, list, moments); }
+    else if (P.tlas && P.modelSkip) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_tlas_list<M>), P, count, list, moments);
+    else { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<false, true, M>), P, count, list, moments);
+           else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<false, false, M>), P, count, list, moments); }
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return cudaEventRecord(evB, stream);
+}
+
+inline cudaError_t pool_launch_list(const DevParams& P, int M, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB,
+                                    unsigned count, const unsigned* list, float4* moments)
+{
+    if (M == 0) M = 64;
+    if (M == 32) return pool_launch_list_m<32>(P, numSMs, stream, evA, evB, count, list, moments);
+    if (M == 64) return pool_launch_list_m<64>(P, numSMs, stream, evA, evB, count, list, moments);
+    if (M == 96) return pool_launch_list_m<96>(P, numSMs, stream, evA, evB, count, list, moments);
     return cudaErrorInvalidValue;
 }
 

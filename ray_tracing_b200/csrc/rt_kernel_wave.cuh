@@ -285,7 +285,10 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
 // The kernel body.  TLAS = the many-model instantiation (its own kernel, k_raytrace_wave_tlas, so that the kernels measured in
 // round 1 keep their code: the TLAS walk and its mask exist only there).  FRAMES = the batch instantiations of rtDispatchFrames (never
 // CHUNKED): a lane keeps its pixel for frames Frame .. Frame + P.frames - 1, writing and accumulating each frame when its samples end.
-template <bool STATS, bool EXT, bool TLAS, bool CHUNKED, bool FRAMES = false>
+// LIST = the list-driven instantiations of rtDispatchAdaptive (never CHUNKED): job j < totalJobs is the pixel P.pixelList[j]
+// ((y << 16) | x), and the write also updates the pixel's moments in P.adaptiveMoments.  (Both come in parameter slots of their own
+// (rt_device.cuh), not as arguments: with two more arguments here the k_raytrace_wave_frames kernels compiled to other code.)
+template <bool STATS, bool EXT, bool TLAS, bool CHUNKED, bool FRAMES = false, bool LIST = false>
 RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const unsigned int tilesX, const unsigned int ownedRows)
 {
     RT_DYNAMIC_SMEM(smemRaw);
@@ -347,6 +350,7 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
     const unsigned int chunkJobs = totalJobs * (unsigned int)chunks;
     int chunk = 0, sampleEnd = P.NumRaysPerPixel; unsigned int pixJob = 0; bool waiting = false;
     static_assert(!(FRAMES && CHUNKED), "a batch of frames runs whole pixels");
+    static_assert(!(LIST && (CHUNKED || FRAMES)), "a pixel list runs whole pixels, one frame");
     unsigned int frame = 0;          // FRAMES: frame of the batch the lane's pixel is in
     (void)frame;
 
@@ -365,6 +369,17 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
             {
                 const unsigned int jobAll = base + (unsigned int)__popc(needMask & laneMaskLt);
                 if (jobAll >= chunkJobs) exhausted = true;
+                else if constexpr (LIST)
+                {
+                    const unsigned int xy = P.pixelList[jobAll];
+                    px = SetupPixel(P, xy & 0xffffu, xy >> 16);
+                    rngState = px.rngState;
+                    totalIncomingLight = splat3(0.0f);
+                    sample = 0; sampleEnd = P.NumRaysPerPixel;
+                    pixelOffset = (size_t)(xy >> 16) * P.W + (xy & 0xffffu);
+                    havePixel = true; pathActive = false;
+                    if (STATS) pixelStart = cnt;
+                }
                 else
                 {
                     const unsigned int job = CHUNKED && chunks > 1 ? jobAll % totalJobs : jobAll;
@@ -444,7 +459,8 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
             if (!CHUNKED || sampleEnd >= P.NumRaysPerPixel)
             {
                 const f3 pixelCol = totalIncomingLight / __int2float_rn(P.NumRaysPerPixel);
-                WritePixel<EXT>(P, pixelOffset, pixelCol.x, pixelCol.y, pixelCol.z);
+                if constexpr (LIST) WritePixel<EXT, true>(P, pixelOffset, pixelCol.x, pixelCol.y, pixelCol.z, P.adaptiveMoments);
+                else WritePixel<EXT>(P, pixelOffset, pixelCol.x, pixelCol.y, pixelCol.z);
             }
             else
             {
@@ -514,6 +530,15 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wa
     wave_body<false, true, true, false, true>(P, totalJobs, tilesX, ownedRows);
 }
 
+// rtDispatchAdaptive: the selection's pixel list (P.pixelList, totalJobs = its length), one frame per pixel (kernels of their own, so
+// that the kernels above keep their code; TLAS = the many-model form, <false, true, true>).  Templates, instantiated where
+// wave_launch_list launches them: a plain kernel defined here changed the register numbering of the k_raytrace_wave_frames kernels.
+template <bool STATS, bool EXT, bool TLAS>
+__global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wave_list(const __grid_constant__ DevParams P, const unsigned int totalJobs)
+{
+    wave_body<STATS, EXT, TLAS, false, false, true>(P, totalJobs, 0u, 0u);
+}
+
 // "gridFit": a pixel's samples cannot be split (one RNG chain), so a persistent lane works through whole pixels.  When the image
 // gives every lane only a few (8 GPUs, config 2: 2.3 pixels per lane) the last round runs with mostly empty warps.  With the
 // option on, the grid is shrunk so that pixels / lanes is just under a whole number k = ceil(pixels / maxLanes): the same k
@@ -565,6 +590,11 @@ inline cudaError_t wave_configure()
     if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(k_raytrace_wave_tlas_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
     return wave_configure_one<true, true>();
 }
 
@@ -626,6 +656,37 @@ inline cudaError_t wave_launch(const DevParams& P, int numSMs, cudaStream_t stre
     if (P.tlas && P.modelSkip) return wave_launch_one<false, true, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
     return ext ? wave_launch_one<false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
                : wave_launch_one<false, false>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
+}
+
+// rtDispatchAdaptive: kernel 1 over the `count` pixels of P.pixelList, sized and chosen like wave_launch's whole-pixel kernels
+template <bool S, bool X, bool T> inline cudaError_t wave_launch_list_one(const DevParams& P, int numSMs, size_t smemBytes, unsigned count,
+                                                                          cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
+{
+    int ctasPerSM = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_list<S, X, T>, WAVE_THREADS, smemBytes);
+    if (e != cudaSuccess) return e;
+    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
+    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);
+    const unsigned int warpsNeeded = (count + 31u) / 32u;
+    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
+    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
+    grid = fit_persistent_grid(P.gridFit, grid, WAVE_THREADS, count);
+    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
+    if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
+    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_raytrace_wave_list<S, X, T>), P, count);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return cudaEventRecord(evB, stream);
+}
+
+inline cudaError_t wave_launch_list(const DevParams& P, int numSMs, unsigned count, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
+{
+    const size_t smemBytes = sizeof(WaveSmemHeader) + (size_t)P.smemPairs * sizeof(NodePair) + (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
+    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;
+    if (P.countStats) return ext ? wave_launch_list_one<true, true, false>(P, numSMs, smemBytes, count, stream, evA, evB)
+                                 : wave_launch_list_one<true, false, false>(P, numSMs, smemBytes, count, stream, evA, evB);
+    if (P.tlas && P.modelSkip) return wave_launch_list_one<false, true, true>(P, numSMs, smemBytes, count, stream, evA, evB);
+    return ext ? wave_launch_list_one<false, true, false>(P, numSMs, smemBytes, count, stream, evA, evB)
+               : wave_launch_list_one<false, false, false>(P, numSMs, smemBytes, count, stream, evA, evB);
 }
 
 } // namespace rtd

@@ -31,6 +31,14 @@ class RayTraceDisplay:
     def save_denoised(self, path: str) -> None:
         write_png(path, self.DenoisedImage()[..., :3])
 
+    def MeanImage(self) -> np.ndarray:
+        """The per-pixel mean of the accumulated image (rtDisplayMean): what an adaptively sampled render (RenderFrameAdaptive), whose
+        pixels have different frame counts, looks like.  (H, W, 4) uint8, top row first."""
+        return self.raytracer.display_mean()[::-1]
+
+    def save_mean(self, path: str) -> None:
+        write_png(path, self.MeanImage()[..., :3])
+
     def DebugView(self, visMode: int, debugVisScale: float) -> np.ndarray:
         """The reference's debug view (visMode / debugVisScale, RayCommon.hlsl:24-26): heat map of the per-pixel traversal counters
         of the counting launches, (H, W, 4) uint8, top row first.  See RayComputeManager.debug_view."""

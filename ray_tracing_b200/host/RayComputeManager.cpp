@@ -36,6 +36,8 @@ std::string RtApi::Load(const char* path)
     CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
     DenoiseFn = reinterpret_cast<decltype(DenoiseFn)>(dlsym(dl, "rtDenoise"));
     DenoiseTemporalFn = reinterpret_cast<decltype(DenoiseTemporalFn)>(dlsym(dl, "rtDenoiseTemporal"));
+    DispatchAdaptiveFn = reinterpret_cast<decltype(DispatchAdaptiveFn)>(dlsym(dl, "rtDispatchAdaptive"));
+    DisplayMeanFn = reinterpret_cast<decltype(DisplayMeanFn)>(dlsym(dl, "rtDisplayMean"));
     return "";
 }
 
@@ -116,6 +118,27 @@ int RayComputeManager::RenderFrames(int n)
     if (rc != RT_OK) return rc;
     TRY(api.DispatchFrames(ctx, (texWidth + 7) / 8, (texHeight + 7) / 8, 1, n));
     numAccumulatedFrames += n;
+    return RT_OK;
+}
+
+int RayComputeManager::RenderFrameAdaptive(float threshold, int minFrames, int maxFrames, int64_t* activePixels)
+{
+    if (activePixels) *activePixels = 0;
+    if (!ctx) return RT_E_STATE;
+    if (!IsRendering()) return RT_OK;
+    if (!api.DispatchAdaptiveFn) { lastError = "the library does not export rtDispatchAdaptive"; return RT_E_STATE; }
+    int rc = InitFrame();
+    if (rc != RT_OK) return rc;
+    TRY(api.DispatchAdaptiveFn(ctx, (texWidth + 7) / 8, (texHeight + 7) / 8, 1, threshold, minFrames, maxFrames, activePixels));
+    numAccumulatedFrames++;                      // accumulate is on (the call refuses otherwise)
+    return RT_OK;
+}
+
+int RayComputeManager::DisplayMean(uint8_t* dst, size_t bytes)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.DisplayMeanFn) { lastError = "the library does not export rtDisplayMean"; return RT_E_STATE; }
+    TRY(api.DisplayMeanFn(ctx, dst, bytes));
     return RT_OK;
 }
 

@@ -64,6 +64,8 @@ struct RtApi
     decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
     decltype(&rtDenoise) DenoiseFn = nullptr;               // optional: the a-trous denoiser (Denoise)
     decltype(&rtDenoiseTemporal) DenoiseTemporalFn = nullptr;  // optional: the temporal denoiser (DenoiseTemporal)
+    decltype(&rtDispatchAdaptive) DispatchAdaptiveFn = nullptr;  // optional: adaptive sampling (RenderFrameAdaptive)
+    decltype(&rtDisplayMean) DisplayMeanFn = nullptr;       // optional: the per-pixel mean on screen (DisplayMean)
     std::string Load(const char* path);        // returns "" on success, else the error text
     void Unload();
 };
@@ -120,6 +122,12 @@ public:
     // not in the reference: n RenderFrame() calls of a still image in one batch (rtDispatchFrames) — InitFrame, one launch of frames
     // numAccumulatedFrames .. + n - 1, numAccumulatedFrames += n.  With accumulate off, n RenderFrame() calls.
     int RenderFrames(int n);
+    // not in the reference: the next frame only where the estimated error is still above `threshold` (rtDispatchAdaptive over the
+    // whole image): the upload sequence and InitFrame of RenderFrame, then the adaptive dispatch, numAccumulatedFrames++.
+    // *activePixels (may be NULL) receives the number of pixels traced; 0 = converged.  Needs accumulate.  The defaults are capi.py's,
+    // chosen by the quality sweep of DESIGN.md section 7d.  DisplayMean: rtDisplayMean, the per-pixel mean as RGBA8.
+    int RenderFrameAdaptive(float threshold = 0.2f, int minFrames = 8, int maxFrames = 64, int64_t* activePixels = nullptr);
+    int DisplayMean(uint8_t* dst, size_t bytes);
     int OnDestroy();                             // :238-247
     void InvalidateBVH() { hasBVH = false; }     // meshes changed: rebuild on the next frame
 

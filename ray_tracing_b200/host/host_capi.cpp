@@ -229,6 +229,9 @@ int rcmOnEnable(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->m
 int rcmResetAccumulatedRender(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->ResetAccumulatedRender(); } CATCH_ALL(h) }
 int rcmRenderFrame(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFrame(); } CATCH_ALL(h) }
 int rcmRenderFrames(void* hv, int n) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFrames(n); } CATCH_ALL(h) }
+int rcmRenderFrameAdaptive(void* hv, float threshold, int minFrames, int maxFrames, int64_t* activePixels)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFrameAdaptive(threshold, minFrames, maxFrames, activePixels); } CATCH_ALL(h) }
+int rcmDisplayMean(void* hv, uint8_t* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->DisplayMean(dst, bytes); }
 int rcmReadFrame(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadFrame(dst, bytes); }
 int rcmReadAccumulated(void* hv, float* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadAccumulated(dst, bytes); }
 int rcmReadPixelStats(void* hv, RtPixelStats* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadPixelStats(dst, bytes); }

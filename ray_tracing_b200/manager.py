@@ -58,6 +58,8 @@ def host_lib() -> C.CDLL:
         for n in ("rcmOnEnable", "rcmResetAccumulatedRender", "rcmRenderFrame"):
             getattr(L, n).argtypes = [vp]
         L.rcmRenderFrames.argtypes = [vp, ci]
+        L.rcmRenderFrameAdaptive.argtypes = [vp, cf, ci, ci, C.POINTER(C.c_int64)]
+        L.rcmDisplayMean.argtypes = [vp, vp, C.c_size_t]
         L.rcmReadFrame.argtypes = [vp, vp, C.c_size_t]
         L.rcmReadAccumulated.argtypes = [vp, vp, C.c_size_t]
         L.rcmGetBVHStats.argtypes = [vp, vp, ci]
@@ -237,6 +239,15 @@ class RayComputeManager:
         With accumulate off it is n RenderFrame() calls."""
         self._ck(self._L.rcmRenderFrames(self._h, int(n)))
 
+    def RenderFrameAdaptive(self, threshold: float = capi.ADAPTIVE_THRESHOLD, min_frames: int = capi.ADAPTIVE_MIN_FRAMES,
+                            max_frames: int = capi.ADAPTIVE_MAX_FRAMES) -> int:
+        """The next frame only where the estimated error is still above `threshold` (rtDispatchAdaptive over the whole image): the
+        upload sequence and InitFrame of RenderFrame, then numAccumulatedFrames += 1.  Returns the number of pixels traced (0 =
+        converged).  Needs accumulate.  Show the result with mean_result / display_mean (each pixel has its own frame count)."""
+        active = C.c_int64(0)
+        self._ck(self._L.rcmRenderFrameAdaptive(self._h, float(threshold), int(min_frames), int(max_frames), C.byref(active)))
+        return int(active.value)
+
     def OnDestroy(self):
         if self._h:
             self._L.rcmDestroy(self._h)
@@ -263,6 +274,23 @@ class RayComputeManager:
     @property
     def accumulatedResult(self) -> np.ndarray:
         return self._read(self._L.rcmReadAccumulated, None)
+
+    @property
+    def mean_result(self) -> np.ndarray:
+        """(H, W, 4) float32, row 0 = bottom: the per-pixel mean accumulatedResult / accumulatedResult.w (0 where nothing was
+        accumulated) — the image of an adaptively sampled render, whose pixels have different frame counts."""
+        a = self.accumulatedResult
+        w = a[..., 3:4]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return np.where(w != 0, a / np.where(w != 0, w, 1), np.float32(0)).astype(np.float32)
+
+    def display_mean(self) -> np.ndarray:
+        """rtDisplayMean: the per-pixel mean encoded as the display encodes, (0, 0, 0, 255) where nothing was accumulated.
+        (H, W, 4) uint8, row 0 = bottom."""
+        w, h = self._size
+        out = np.empty((h, w, 4), dtype=np.uint8)
+        self._ck(self._L.rcmDisplayMean(self._h, out.ctypes.data, out.nbytes))
+        return out
 
     def read_accumulated_into(self, ptr: int, nbytes: int):
         self._ck(self._L.rcmReadAccumulated(self._h, C.c_void_p(ptr), nbytes))

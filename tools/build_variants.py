@@ -86,6 +86,9 @@ VARIANTS = {
     "temporal_taun80": ("RT_TEMPORAL_TAU_N=0.8f",),
     "temporal_taun95": ("RT_TEMPORAL_TAU_N=0.95f",),
     "temporal_taun50": ("RT_TEMPORAL_TAU_N=0.5f",),
+    # rtDispatchAdaptive's absolute floor for dark pixels, 2^-4 and 2^-12 against the default 2^-8 (tools/adaptive_bench.py --sweep)
+    "adaptive_eps4": ("RT_ADAPTIVE_EPSILON=0.0625f",),
+    "adaptive_eps12": ("RT_ADAPTIVE_EPSILON=0.000244140625f",),
 }
 OUT_DIR = os.path.join(build.PKG_DIR, "variants")
 

@@ -5,7 +5,7 @@ resizes, accumulation resets, settings and kernel options that change between fr
 manager against the oracle and against the kernels, compared bit for bit after every frame.  What it exercises is the host-side
 state of csrc/rt_api.cu: dirty flags, cached repacks, the regions the padded boxes were built for, kernel selection.
 
-    python tools/simt_fuzz_session.py [--cases 100] [--seed 1] [--steps 8] [--pixel-stats] [--frames]
+    python tools/simt_fuzz_session.py [--cases 100] [--seed 1] [--steps 8] [--pixel-stats] [--frames] [--queries] [--adaptive]
 
 --pixel-stats: both sides count from the start ("countStats" = 1, and the script's countStats switches reach the oracle too), and after
 every frame the per-pixel counters (PixelStats rays, box and triangle tests) are compared as well: accumulation across frames, resizes,
@@ -13,6 +13,11 @@ partial state changes.
 
 --frames: a step may render a batch of 2-6 frames as one call (RenderFrames: rtDispatchFrames) instead of one frame, on both sides.
 Where the kernels' side refuses the batch because "sampleChunks" is forced to 2 or more, it renders the frames one by one instead.
+
+--adaptive: a step may render an adaptive frame (RenderFrameAdaptive: rtDispatchAdaptive over the whole image) with a random threshold
+and min / max frames, or an adaptive call over a random partial region at a random Frame straight on the context, on both sides; the
+active counts, the images and "AdaptiveMoments" are compared after it, and refusals must agree.  Where the kernels' side would refuse
+because "sampleChunks" is forced to 2 or more, the step renders a plain frame on both sides instead.
 
 --queries: query steps anywhere in the script — before OnEnable, between a scene change and the next frame, right after a raw
 dispatch, between frames: rtTraceRays, rtTraceOcclusion or rtTracePaths of 0, 1, 31, 32, 33 or a few hundred rays (the ray sets of
@@ -148,7 +153,17 @@ def random_spheres(rng, n):
     return sph
 
 
-def make_script(rng, sc, steps, frames=False, queries=False):
+def random_adaptive(rng):
+    """('adaptive', (threshold, minFrames, maxFrames)) or ('adaptive_partial', (threshold, minFrames, maxFrames, gx, gy, Frame))"""
+    thr = float(rng.choice([0.0, 0.05, 0.2, 0.5, 1.0, float(rng.uniform(0, 2))]))
+    mn = int(rng.randint(2, 6))
+    mx = int(rng.choice([mn, mn + int(rng.randint(0, 6)), 1 << 24]))
+    if rng.rand() < 0.3:
+        return ("adaptive_partial", (thr, mn, mx, int(rng.randint(0, 9)), int(rng.randint(0, 6)), int(rng.randint(1, 1000))))
+    return ("adaptive", (thr, mn, mx))
+
+
+def make_script(rng, sc, steps, frames=False, queries=False, adaptive=False):
     """A list of (action, arguments) — applied to both managers; ('option', ...) only to the kernels' side.  frames: a step may end in
     ('frames', (n,)), a batch of n frames, instead of ('frame', ()).  queries: ('query', ...) steps (random_query) before OnEnable,
     among the scene changes, after raw dispatches and after frames."""
@@ -187,7 +202,9 @@ def make_script(rng, sc, steps, frames=False, queries=False):
                 value = {"kernel": [0, 1, 2, -1], "tlas": [-1, 0, 1], "modelSkip": [0, 1], "poolSlots": [0, 32, 64, 96], "pairOrder": [0, 1, 3], "smemNodes": [0, 9, 200, -1],
                          "tailLanes": [0, 5, 16, 31], "sortRays": [0, 1], "gridFit": [0, 1], "extInstantiation": [0, 1], "countStats": [0, 1], "sampleChunks": [-1, 0, 2, 3]}[name]
                 script.append(("option", (name, int(rng.choice(value)))))
-        if frames and rng.rand() < 0.5:
+        if adaptive and rng.rand() < 0.6:
+            script.append(random_adaptive(rng))
+        elif frames and rng.rand() < 0.5:
             script.append(("frames", (int(rng.randint(2, 7)),)))
         else:
             script.append(("frame", ()))
@@ -226,6 +243,25 @@ def read_pixel_stats(mgr):
         return e.code
 
 
+def run_adaptive(mgr, action, a):
+    """One adaptive step on one side: the active count, or the RT_E_* code of a refusal."""
+    try:
+        if action == "adaptive":
+            return mgr.RenderFrameAdaptive(*a)
+        thr, mn, mx, gx, gy, frame = a
+        mgr.context.set_int("Frame", frame)
+        return mgr.context.dispatch_adaptive(thr, mn, mx, gx, gy, 1)
+    except rt.capi.RtError as e:
+        return e.code
+
+
+def read_moments(mgr):
+    try:
+        return mgr.context.adaptive_moments()
+    except rt.capi.RtError as e:
+        return e.code
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--cases", type=int, default=100)
@@ -235,15 +271,16 @@ def main():
     ap.add_argument("--pixel-stats", action="store_true", help="also compare the per-pixel counters after every frame")
     ap.add_argument("--frames", action="store_true", help="steps may render a batch of 2-6 frames in one call (RenderFrames)")
     ap.add_argument("--queries", action="store_true", help="query steps (rtTraceRays / rtTraceOcclusion / rtTracePaths) anywhere in the script")
+    ap.add_argument("--adaptive", action="store_true", help="steps may render an adaptive frame (RenderFrameAdaptive / rtDispatchAdaptive)")
     args = ap.parse_args()
     lib = args.lib or simt_build.build()
     device = DeviceMemory(lib) if args.queries else None
-    bad, query_steps = 0, {k: 0 for k in QUERY_KINDS + QUERY_FORMS}
+    bad, query_steps, adaptive_steps = 0, {k: 0 for k in QUERY_KINDS + QUERY_FORMS}, 0
     for case in range(args.cases):
         seed = args.seed * 100003 + case
         rng = np.random.RandomState(seed)
         sc = random_scene(rng, odd=0.0)
-        script = make_script(rng, sc, args.steps, args.frames, args.queries)
+        script = make_script(rng, sc, args.steps, args.frames, args.queries, args.adaptive)
         pool = np.concatenate(list(ray_sets(sc, seed=seed, n=48).values())) if args.queries else None
         mgrs = []
         for backend in (ORACLE_LIB, lib):
@@ -276,15 +313,34 @@ def main():
                     spheres = len(a[0])
                 if action == "screen":
                     resized = True                      # the textures follow at the next RenderFrame (InitFrame): no raw dispatch in between
-                if action == "rawframe" and resized:
+                if action in ("rawframe", "adaptive_partial") and resized:
                     continue
-                if action in ("frame", "frames"):
+                if action in ("adaptive", "adaptive_partial") and chunks >= 2:
+                    action = "frame"                    # refused on the kernels' side only (a pixel list runs whole pixels)
+                if action in ("frame", "frames", "adaptive"):
                     resized = False
                 if action == "option" and a[0] == "sampleChunks":
                     chunks = a[1]
-                if action in ("frame", "frames", "rawframe"):
+                if action in ("adaptive", "adaptive_partial"):
+                    counts = [run_adaptive(m, action, a) for m in mgrs]
+                    frame_no += 1
+                    if counts[0] != counts[1]:
+                        failed = f"{action} {a} after {frame_no - 1} frames: {counts[1]} vs the oracle's {counts[0]}"
+                        break
+                    adaptive_steps += 1
+                    mo, mg = (read_moments(m) for m in mgrs)
+                    if isinstance(mo, int) or isinstance(mg, int):
+                        if not (isinstance(mo, int) and isinstance(mg, int) and mo == mg):
+                            failed = f"AdaptiveMoments readable on one side only after {action} {a}"
+                            break
+                    elif mo.shape != mg.shape or ((mo.view(np.uint32) != mg.view(np.uint32)) & ~(np.isnan(mo) & np.isnan(mg))).any():
+                        failed = f"AdaptiveMoments differ after {action} {a}"
+                        break
+                if action in ("frame", "frames", "rawframe", "adaptive", "adaptive_partial"):
                     for i, m in enumerate(mgrs):
-                        if action == "frame":
+                        if action in ("adaptive", "adaptive_partial"):
+                            pass
+                        elif action == "frame":
                             m.RenderFrame()
                         elif action == "frames":
                             try:
@@ -326,11 +382,11 @@ def main():
             m.OnDestroy()
         if failed:
             bad += 1
-            brief = [(act, a if act in ("option", "setting", "screen", "query") else "...") for act, a in script]
+            brief = [(act, a if act in ("option", "setting", "screen", "query", "adaptive", "adaptive_partial") else "...") for act, a in script]
             print(f"case seed {seed}: {failed}; {len(sc.models)} models, {len(sc.spheres)} spheres; script {brief}", flush=True)
         if (case + 1) % 25 == 0:
             print(f"  {case + 1} cases, {bad} findings", flush=True)
-    print(f"{args.cases} cases, {bad} findings" +
+    print(f"{args.cases} cases, {bad} findings" + (f"; adaptive steps equal: {adaptive_steps}" if args.adaptive else "") +
           (f"; query steps equal: {sum(query_steps[k] for k in QUERY_KINDS)} (" + ", ".join(f"{k} {v}" for k, v in query_steps.items()) + ")" if args.queries else ""))
     return 1 if bad else 0
 
