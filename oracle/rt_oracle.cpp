@@ -1253,6 +1253,7 @@ extern "C" int rtBuildBVH(RtContext* ctx, const float* verts, int vertCount, con
     b.nodes.push_back(BvhCs::Builder::Node(lo[0], lo[1], lo[2], hi[0], hi[1], hi[2], -1, -1));     // BC:61
     if (quality == 2) { b.nodes[0].startIndex = 0; b.nodes[0].triangleCount = triCount; }
     else b.Split(0, 0, triCount, 0);
+    if ((int)b.nodes.size() > nodeCapacity) return RT_E_INVALID;               // chains of empty children can exceed 2n + 1 nodes
     for (int i = 0; i < triCount; i++)                                           // BC:69-80
     {
         const int base = b.buildTriangles[i].Index;

@@ -130,9 +130,10 @@ BVH::BVH(const Vector3* verts, int vertCount, const int* indices, int indexCount
     {
         // the same recursion, its independent subtrees built by different threads and concatenated in the reference's order
         Block blk;
-        RtNode root = BuildBlock(Nodes[0], 0, triCount, 0, blk, threads);
-        if (root.triangleCount <= 0) root.startIndex = 1;                 // B(root) starts right after the root
-        for (RtNode& n : blk.nodes) if (n.triangleCount <= 0) n.startIndex += 1;
+        bool rootInner = false;
+        RtNode root = BuildBlock(Nodes[0], 0, triCount, 0, blk, threads, rootInner);
+        if (rootInner) root.startIndex = 1;                               // B(root) starts right after the root
+        for (size_t k = 0; k < blk.nodes.size(); k++) if (blk.inner[k]) blk.nodes[k].startIndex += 1;
         Nodes[0] = root;
         Nodes.insert(Nodes.end(), blk.nodes.begin(), blk.nodes.end());
         mergeStats(stats, blk.stats);
@@ -274,7 +275,7 @@ BVH::SplitChoice BVH::ChooseSplit(const RtNode& node, int start, int count, int 
     return best;
 }
 
-void BVH::Split(std::vector<RtNode>& Nodes, BuildStats& stats, int parentIndex, int triGlobalStart, int triNum, int depth)           // BVH.cs:89-181
+void BVH::Split(std::vector<RtNode>& Nodes, BuildStats& stats, int parentIndex, int triGlobalStart, int triNum, int depth, std::vector<char>* inner)   // BVH.cs:89-181
 {
     const int MaxDepth = 32;
     const RtNode parent = Nodes[parentIndex];
@@ -307,9 +308,10 @@ void BVH::Split(std::vector<RtNode>& Nodes, BuildStats& stats, int parentIndex, 
         Nodes.push_back(makeNode(right, triGlobalStart + numOnLeft, 0));
         const int childIndexRight = childIndexLeft + 1;
         Nodes[parentIndex].startIndex = childIndexLeft;
+        if (inner) { inner->resize(Nodes.size(), 0); (*inner)[parentIndex] = 1; }
         stats.RecordNode(depth, false);
-        Split(Nodes, stats, childIndexLeft, triGlobalStart, numOnLeft, depth + 1);
-        Split(Nodes, stats, childIndexRight, triGlobalStart + numOnLeft, numOnRight, depth + 1);
+        Split(Nodes, stats, childIndexLeft, triGlobalStart, numOnLeft, depth + 1, inner);
+        Split(Nodes, stats, childIndexRight, triGlobalStart + numOnLeft, numOnRight, depth + 1, inner);
     }
     else
     {
@@ -321,19 +323,24 @@ void BVH::Split(std::vector<RtNode>& Nodes, BuildStats& stats, int parentIndex, 
 
 // The subtree below `node` (its triangles are buildTris[triGlobalStart .. +triNum)), built with up to `threads` threads.
 // Takes exactly the decisions Split() takes — same ChooseSplit, same in-place partition — and returns the node with its leaf
-// range or, for an inner node, startIndex = 0 (block-relative); blk receives B(node).
-RtNode BVH::BuildBlock(RtNode node, int triGlobalStart, int triNum, int depth, Block& blk, int threads)
+// range or, for an inner node, startIndex = 0 (block-relative); blk receives B(node), isInner whether Split split the node.
+// Only inner nodes' startIndex is a child index to rebase.  triangleCount cannot tell: an empty leaf (a split that put every
+// triangle on one side, e.g. when every cost is inf) has triangleCount 0 like an inner node, and startIndex = its triangle start.
+RtNode BVH::BuildBlock(RtNode node, int triGlobalStart, int triNum, int depth, Block& blk, int threads, bool& isInner)
 {
     if (threads <= 1 || triNum < kParallelMinTris)
     {
         std::vector<RtNode> local;
+        std::vector<char> localInner(1, 0);
         local.reserve((size_t)triNum / 2 + 16);
         local.push_back(node);
-        Split(local, blk.stats, 0, triGlobalStart, triNum, depth);
+        Split(local, blk.stats, 0, triGlobalStart, triNum, depth, &localInner);
         node = local[0];
+        isInner = localInner[0] != 0;
         blk.nodes.assign(local.begin() + 1, local.end());
-        for (RtNode& n : blk.nodes) if (n.triangleCount <= 0) n.startIndex -= 1;      // local index -> block-relative
-        if (node.triangleCount <= 0) node.startIndex = 0;
+        blk.inner.assign(localInner.begin() + 1, localInner.end());
+        for (size_t k = 0; k < blk.nodes.size(); k++) if (blk.inner[k]) blk.nodes[k].startIndex -= 1;    // local index -> block-relative
+        if (isInner) node.startIndex = 0;
         return node;
     }
     const int MaxDepth = 32;
@@ -343,6 +350,7 @@ RtNode BVH::BuildBlock(RtNode node, int triGlobalStart, int triNum, int depth, B
     {
         node.startIndex = triGlobalStart; node.triangleCount = triNum;
         blk.stats.RecordNode(depth, true, triNum);
+        isInner = false;
         return node;
     }
     Box left, right;
@@ -368,19 +376,23 @@ RtNode BVH::BuildBlock(RtNode node, int triGlobalStart, int triNum, int depth, B
     if (threadsL < 1) threadsL = 1;
     if (threadsL > threads - 1) threadsL = threads - 1;
     Block bl, br;
-    std::thread worker([&]() { childL = BuildBlock(childL, triGlobalStart, numOnLeft, depth + 1, bl, threadsL); });
-    childR = BuildBlock(childR, triGlobalStart + numOnLeft, numOnRight, depth + 1, br, threads - threadsL);
+    bool innerL = false, innerR = false;
+    std::thread worker([&]() { childL = BuildBlock(childL, triGlobalStart, numOnLeft, depth + 1, bl, threadsL, innerL); });
+    childR = BuildBlock(childR, triGlobalStart + numOnLeft, numOnRight, depth + 1, br, threads - threadsL, innerR);
     worker.join();
     // B(node) = [L, R] + B(L) + B(R)
     const int offL = 2, offR = 2 + (int)bl.nodes.size();
-    if (childL.triangleCount <= 0) childL.startIndex = offL;
-    if (childR.triangleCount <= 0) childR.startIndex = offR;
+    if (innerL) childL.startIndex = offL;
+    if (innerR) childR.startIndex = offR;
     blk.nodes.reserve(2 + bl.nodes.size() + br.nodes.size());
+    blk.inner.reserve(2 + bl.inner.size() + br.inner.size());
     blk.nodes.push_back(childL); blk.nodes.push_back(childR);
-    for (RtNode& n : bl.nodes) { if (n.triangleCount <= 0) n.startIndex += offL; blk.nodes.push_back(n); }
-    for (RtNode& n : br.nodes) { if (n.triangleCount <= 0) n.startIndex += offR; blk.nodes.push_back(n); }
+    blk.inner.push_back(innerL); blk.inner.push_back(innerR);
+    for (size_t k = 0; k < bl.nodes.size(); k++) { if (bl.inner[k]) bl.nodes[k].startIndex += offL; blk.nodes.push_back(bl.nodes[k]); blk.inner.push_back(bl.inner[k]); }
+    for (size_t k = 0; k < br.nodes.size(); k++) { if (br.inner[k]) br.nodes[k].startIndex += offR; blk.nodes.push_back(br.nodes[k]); blk.inner.push_back(br.inner[k]); }
     mergeStats(blk.stats, bl.stats); mergeStats(blk.stats, br.stats);
     node.startIndex = 0;
+    isInner = true;
     return node;
 }
 

@@ -55,12 +55,14 @@ private:
     Quality quality;
 
     // B(n) of a node n: everything Split(n) appends to Nodes — [left child, right child] + B(left) + B(right) — with child
-    // indices relative to the first entry of the block, so that independently built blocks concatenate by adding offsets
-    struct Block { std::vector<RtNode> nodes; BuildStats stats; };
+    // indices relative to the first entry of the block, so that independently built blocks concatenate by adding offsets.
+    // inner[k] says whether nodes[k] was split (its startIndex is a child index) or is a leaf, empty leaves included.
+    struct Block { std::vector<RtNode> nodes; std::vector<char> inner; BuildStats stats; };
 
     int  AddNode(const RtNode& n);
-    void Split(std::vector<RtNode>& nodes, BuildStats& st, int parentIndex, int triGlobalStart, int triNum, int depth);
-    RtNode BuildBlock(RtNode node, int triGlobalStart, int triNum, int depth, Block& blk, int threads);
+    // inner (optional): set to 1 at every node Split splits, grown with the node list
+    void Split(std::vector<RtNode>& nodes, BuildStats& st, int parentIndex, int triGlobalStart, int triNum, int depth, std::vector<char>* inner = nullptr);
+    RtNode BuildBlock(RtNode node, int triGlobalStart, int triNum, int depth, Block& blk, int threads, bool& isInner);
     SplitChoice ChooseSplit(const RtNode& node, int start, int count, int threads = 1) const;
     float EvaluateSplit(int splitAxis, float splitPos, int start, int count) const;
     static float NodeCost(float x, float y, float z, int numTriangles);

@@ -1,4 +1,4 @@
-"""The randomised searches of tools/ (simt_fuzz.py: scenes against the oracle; simt_fuzz_session.py: sequences of host calls; simt_fuzz_bvh.py: rtBuildBVH against the host builder) run
+"""The randomised searches of tools/ (simt_fuzz.py: scenes against the oracle; simt_fuzz_session.py: sequences of host calls; simt_fuzz_bvh.py: rtBuildBVH and the host builder against the oracle's recursion) run
 for a few dozen cases each, so that the tools keep working and a regression in what they once found shows up in the CPU suite.  The
 long campaigns are run by hand (DESIGN.md 3b)."""
 import os
@@ -15,7 +15,10 @@ from conftest import REPO
                                        ("simt_fuzz.py", ["--cases", "4", "--seed", "5", "--far", "1.0"]),
                                        ("simt_fuzz.py", ["--cases", "20", "--seed", "7", "--far", "0", "--odd", "1.0"]),
                                        ("simt_fuzz_session.py", ["--cases", "12", "--seed", "3", "--steps", "6"]),
-                                       ("simt_fuzz_bvh.py", ["--cases", "30", "--seed", "11"])])
+                                       ("simt_fuzz_bvh.py", ["--cases", "30", "--seed", "11"]),
+                                       # 16,383..150,000 triangles: the host builder's multi-threaded path against the oracle's recursion
+                                       # (device builds of this size are left to the GPU suite: minutes each on the interpreter)
+                                       ("simt_fuzz_bvh.py", ["--cases", "40", "--seed", "12", "--large", "--host-only", "--odd", "0.5"])])
 def test_randomised_search_finds_nothing(tool, args):
     r = subprocess.run([sys.executable, os.path.join(REPO, "tools", tool)] + args, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]

@@ -74,23 +74,125 @@ def test_bvh_is_deterministic_and_splits_reduce_cost():
     assert a[2]["LeafMaxTriCount"] < 64 and a[2]["LeafNodeCount"] > m.triangle_count // 16
 
 
+def _triangle_mesh(tri, seed=0):
+    """MeshDesc of an (n, 3, 3) array of triangle corners: unshared vertices, random normals."""
+    v = np.ascontiguousarray(np.asarray(tri).reshape(-1, 3), dtype=np.float32)
+    nrm = np.ascontiguousarray(np.random.RandomState(seed).uniform(-1, 1, v.shape), dtype=np.float32)
+    return scenes.MeshDesc(v, np.arange(len(v), dtype=np.int32), nrm)
+
+
+def large_adversarial_meshes():
+    """(name, MeshDesc) pairs at and above the host builder's parallel threshold (16,384 triangles, host/BVH.cpp kParallelMinTris):
+    the classes of tools/simt_fuzz_bvh.py, non-finite vertices and extents whose surface area overflows FP32 (every split costs inf,
+    ChooseSplit falls back to 'axis 0, position 0' and Split still splits, so the tree has empty leaves), and a first split that
+    leaves one triangle on one side.  Also used by the device build's tests on the GPU."""
+    rng = np.random.RandomState(2024)
+
+    def soup(n, scale=1.0):
+        return (rng.uniform(-1, 1, (n, 1, 3)) + rng.uniform(-0.05, 0.05, (n, 3, 3))) * scale
+
+    def grid(n):
+        k = int(np.ceil(np.sqrt(n))); gx, gy = np.meshgrid(np.arange(k), np.arange(k))
+        g = np.stack([gx.ravel(), gy.ravel(), np.zeros(k * k)], 1)[:n]
+        return g[:, None, :] + np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], dtype=np.float64)[None]
+
+    def degenerate(n):
+        t = soup(n); t[::3, 1] = t[::3, 0]; t[::5, 2] = t[::5, 0]
+        return t
+
+    def line(n):
+        t = np.zeros((n, 3, 3)); t[:, :, 0] = np.arange(n)[:, None] + rng.uniform(0, 0.9, (n, 3))
+        return t
+
+    def far_clusters(n):
+        c = rng.choice([-100.0, 0.0, 100.0], (n, 1, 3)) + rng.uniform(-1, 1, (n, 1, 3))
+        return c + rng.uniform(-0.2, 0.2, (n, 3, 3))
+
+    def special(t, value, at):
+        t = t.copy(); t[at] = value
+        return t
+
+    def lone_first(n):                                                  # the root's split puts one triangle left, n - 1 right
+        t = soup(n) * 0.5 + 0.5
+        t[0] -= 1000.0
+        return t
+
+    meshes = [("soup 16383", soup(16383)), ("equal-cost grid 16384", grid(16384)),
+              ("coincident 16385", np.repeat(rng.uniform(-1, 1, (1, 3, 3)), 16385, axis=0)),
+              ("degenerate 16383", degenerate(16383)), ("+-0 planes 16384", rng.choice([-1.0, -0.0, 0.0, 1.0, 0.5], (16384, 3, 3))),
+              ("line 16385", line(16385)), ("far clusters 16384", far_clusters(16384)),
+              ("NaN vertex 16385", special(soup(16385), np.nan, (9000, 1, 0))),
+              ("+inf vertex 16384", special(soup(16384), np.inf, (123, 2, 1))),
+              ("-inf vertex 16383", special(soup(16383), -np.inf, (16000, 0, 2))),
+              ("extents 1e19 16385", soup(16385, 1e19)), ("extents 1e20 16384", soup(16384, 1e20)),
+              ("one triangle split off first 16385", lone_first(16385)),
+              ("far clusters with a +inf vertex 100003", special(far_clusters(100003), np.inf, (50000, 0, 0))),
+              # regressions: the multi-threaded build once rebased the empty leaves' startIndex as if it were a child index
+              ("overflow soup 20000", soup(20000, 1e19)),
+              ("+inf vertex 30000", special(soup(30000), np.inf, (7777, 1, 1)))]
+    return [(name, _triangle_mesh(t, seed=k)) for k, (name, t) in enumerate(meshes)]
+
+
+def _same_bytes(a, b):
+    return len(a) == len(b) and np.array_equal(a.view(np.uint8), b.view(np.uint8))
+
+
 def test_bvh_build_does_not_depend_on_the_thread_count():
     """The multi-threaded build (independent subtrees on different threads, slices of a large node evaluated in parallel) returns the
-    single-threaded recursion's buffers byte for byte: same node order, same bounds, same triangle order, same statistics."""
+    single-threaded recursion's buffers byte for byte: same node order, same bounds, same triangle order, same statistics.  The nodes
+    and the triangle order are also those of the oracle's plain restatement of the reference's recursion (oracle/rt_oracle.cpp), on
+    benign meshes and on the adversarial ones above."""
     knot = scenes.knot_mesh(nu=400, nv=24)                                          # 19,200 triangles: above the parallel threshold
     soup = max(scenes.random_soup(16, 16, 2, 1, triangles=60000, spheres=1).meshes, key=lambda m: m.triangle_count)
+    orc = capi.RtLib(ORACLE_LIB).create(0)
     try:
-        for mesh in (knot, soup):
+        for name, mesh in [("knot 19200", knot), ("soup", soup)] + large_adversarial_meshes():
             for q in ("High", "Low", "Disabled"):
+                to, no = orc.build_bvh(mesh.vertices, mesh.indices, mesh.normals, rt.manager.QUALITY[q])
                 rt.set_build_threads(1)
                 t1, n1, s1 = rt.build_bvh(mesh.vertices, mesh.indices, mesh.normals, q)
-                for threads in (2, 5, 16):
+                assert _same_bytes(n1, no) and _same_bytes(t1, to), f"{name} {q}: 1 thread vs the oracle"
+                assert q == "Disabled" or (s1["TotalNodeCount"] == len(n1) and s1["TriangleCount"] == mesh.triangle_count)
+                for threads in (2, 3, 5, 16, 0):
                     rt.set_build_threads(threads)
                     t, n, st = rt.build_bvh(mesh.vertices, mesh.indices, mesh.normals, q)
-                    assert np.array_equal(n.view(np.uint8), n1.view(np.uint8)) and np.array_equal(t.view(np.uint8), t1.view(np.uint8)), (q, threads)
-                    assert {k: v for k, v in st.items() if k != "TimeMs"} == {k: v for k, v in s1.items() if k != "TimeMs"}
+                    assert _same_bytes(n, no) and _same_bytes(t, to), f"{name} {q}: {threads or 'all'} threads vs the oracle"
+                    assert {k: v for k, v in st.items() if k != "TimeMs"} == {k: v for k, v in s1.items() if k != "TimeMs"}, (name, q, threads)
     finally:
         rt.set_build_threads(0)
+        orc.destroy()
+
+
+def test_large_adversarial_meshes_have_empty_leaves():
+    """The meshes above reach what they are there for: trees with empty leaves (triangleCount 0 and a startIndex that is a triangle
+    index, not a child index) built by the multi-threaded path."""
+    empty = {}
+    for name, mesh in large_adversarial_meshes():
+        _, nodes, st = rt.build_bvh(mesh.vertices, mesh.indices, mesh.normals, "High")
+        empty[name] = st["LeafMinTriCount"] == 0
+    assert empty["overflow soup 20000"] and empty["+inf vertex 30000"] and empty["extents 1e20 16384"], empty
+    assert not empty["soup 16383"] and not empty["equal-cost grid 16384"], empty
+
+
+def test_infinite_vertex_knot_renders_the_same_at_every_thread_count(oracle_path):
+    """A 38,400-triangle knot with one vertex coordinate at +inf, rendered through the oracle: the default (all threads) host build
+    gives the single-threaded recursion's tree, so the frame is the same bits (the multi-threaded build once produced child indices
+    out of range, which rtDispatch refuses)."""
+    sc = scenes.knot_room(32, 18, 2, 1, nu=400, nv=48)
+    knot = max(range(len(sc.meshes)), key=lambda i: sc.meshes[i].triangle_count)
+    sc.meshes[knot].vertices = sc.meshes[knot].vertices.copy()
+    sc.meshes[knot].vertices[1234, 0] = np.inf
+    assert sc.meshes[knot].triangle_count == 38400
+    try:
+        rt.set_build_threads(1)
+        f1, a1 = render(oracle_path, sc)
+        rt.set_build_threads(0)
+        f0, a0 = render(oracle_path, sc)
+    finally:
+        rt.set_build_threads(0)
+    assert_bit_equal(f0, f1, "all threads vs 1 thread")
+    assert_bit_equal(a0, a1, "all threads vs 1 thread (accumulated)")
+    assert np.isfinite(f1).all() and f1[..., :3].sum() > 0
 
 
 def test_bvh_vs_brute_force_image(oracle_path):

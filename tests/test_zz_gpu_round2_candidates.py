@@ -30,19 +30,59 @@ def test_grid_fit_is_schedule_only_on_gpu(kernel):
     assert_bit_equal(ag, ao, f"gridFit kernel={kernel}")
 
 
+def _bvh_production_meshes():
+    """The meshes the renders build: the 87k-triangle knot, the 871k-triangle cluster (one mesh) and the 900k-triangle mesh of the
+    1M-triangle soup (the bench's big scene)."""
+    biggest = lambda sc: max(sc.meshes, key=lambda m: m.triangle_count)          # noqa: E731
+    return [("knot 87k", scenes.knot_mesh()), ("cluster 871k", biggest(scenes.knot_cluster(64, 36, 2, 1))),
+            ("soup 900k", biggest(scenes.random_soup(16, 16, 2, 1)))]
+
+
 def test_device_bvh_build_equals_the_host_builder_on_gpu():
-    """rtBuildBVH on the H100 against host/BVH.cpp: Nodes and Triangles byte for byte (87k-triangle knot, 100k random triangles)."""
+    """rtBuildBVH on the H100 against the oracle's single-threaded restatement of the reference's recursion (oracle/rt_oracle.cpp), and
+    host/BVH.cpp at all threads against the same: Nodes and Triangles byte for byte.  The production meshes, and the large adversarial
+    meshes of tests/test_host.py (16,383 to 100,003 triangles: the host's multi-threaded path, empty leaves from non-finite vertices and
+    overflowing extents) at all three qualities."""
     import numpy as np
     import ray_tracing_b200 as rt
     from ray_tracing_b200 import capi
-    gpu = capi.RtLib(CUDA_LIB).create(0)
-    soup = max(scenes.random_soup(16, 16, 2, 1, triangles=300000, spheres=1).meshes, key=lambda m: m.triangle_count)
-    for m in (scenes.knot_mesh(), soup):
-        for q in (1, 0):
+    from test_host import large_adversarial_meshes
+    same = lambda a, b: len(a) == len(b) and np.array_equal(a.view(np.uint8), b.view(np.uint8))    # noqa: E731
+    gpu, orc = capi.RtLib(CUDA_LIB).create(0), capi.RtLib(ORACLE_LIB).create(0)
+    rt.set_build_threads(0)
+    cases = [(name, m, (1, 0)) for name, m in _bvh_production_meshes()] + [(name, m, (1, 0, 2)) for name, m in large_adversarial_meshes()]
+    for name, m, qualities in cases:
+        for q in qualities:
+            to, no = orc.build_bvh(m.vertices, m.indices, m.normals, q)
             th, nh, _ = rt.build_bvh(m.vertices, m.indices, m.normals, q)
             tg, ng = gpu.build_bvh(m.vertices, m.indices, m.normals, q)
-            assert len(ng) == len(nh) and np.array_equal(ng.view(np.uint8), nh.view(np.uint8)) and np.array_equal(tg.view(np.uint8), th.view(np.uint8))
-    gpu.destroy()
+            assert same(nh, no) and same(th, to), f"host vs oracle: {name} q={q}"
+            assert same(ng, no), f"device nodes vs oracle: {name} q={q} ({len(ng)} vs {len(no)} nodes)"
+            assert same(tg, to), f"device triangle order vs oracle: {name} q={q}"
+    gpu.destroy(); orc.destroy()
+
+
+def test_device_bvh_build_through_the_manager_on_an_infinite_vertex_knot():
+    """buildBVHOnDevice = 1 on the 38,400-triangle knot room with one vertex at +inf (a tree with empty leaves): the manager's frames
+    are those of the host-built tree, on the H100 and through the oracle."""
+    sc = scenes.knot_room(32, 18, 2, 1, nu=400, nv=48)
+    knot = max(range(len(sc.meshes)), key=lambda i: sc.meshes[i].triangle_count)
+    sc.meshes[knot].vertices = sc.meshes[knot].vertices.copy()
+    sc.meshes[knot].vertices[1234, 0] = float("inf")
+
+    def run(lib, on_device):
+        import ray_tracing_b200 as rt
+        mgr = rt.RayComputeManager(lib)
+        scenes.apply(sc, mgr)
+        mgr.buildBVHOnDevice = on_device
+        mgr.OnEnable(); mgr.RenderFrame(); mgr.RenderFrame()
+        out = mgr.accumulatedResult.copy()
+        mgr.OnDestroy()
+        return out
+
+    ref = run(ORACLE_LIB, 0)
+    assert_bit_equal(run(CUDA_LIB, 0), ref, "host-built tree")
+    assert_bit_equal(run(CUDA_LIB, 1), ref, "device-built tree")
 
 
 def test_l2_persistence_window_changes_nothing_but_caching():
@@ -252,14 +292,16 @@ def test_moving_the_camera_out_of_the_padded_region_rebuilds_the_model_boxes():
 
 
 def test_model_free_device_bvh_build_on_degenerate_and_non_finite_input():
-    """rtBuildBVH against host/BVH.cpp, byte for byte, where a level-synchronous build can go wrong (all found by tools/simt_fuzz_bvh.py):
-    bounds that see +0 and -0 (the reference's sequential strict comparison keeps the first), NaN vertices (never replace a running
-    bound), an infinite vertex and extents whose surface area overflows FP32 (every candidate costs inf, ChooseSplit returns its
-    defaults 'axis 0, position 0' and Split still splits — the first version of the device build never finished on that)."""
+    """rtBuildBVH against the oracle's restatement of the reference's recursion (and host/BVH.cpp against the same), byte for byte, where
+    a level-synchronous build can go wrong (all found by tools/simt_fuzz_bvh.py): bounds that see +0 and -0 (the reference's sequential
+    strict comparison keeps the first), NaN vertices (never replace a running bound), an infinite vertex and extents whose surface area
+    overflows FP32 (every candidate costs inf, ChooseSplit returns its defaults 'axis 0, position 0' and Split still splits — the first
+    version of the device build never finished on that).  Small meshes only: tests/test_simt_kernels.py runs this body on the
+    interpreter; the large ones are in test_device_bvh_build_equals_the_host_builder_on_gpu."""
     import numpy as np
     import ray_tracing_b200 as rt
     from ray_tracing_b200 import capi
-    gpu = capi.RtLib(CUDA_LIB).create(0)
+    gpu, orc = capi.RtLib(CUDA_LIB).create(0), capi.RtLib(ORACLE_LIB).create(0)
     rng = np.random.RandomState(4)
     cases = []
     cases.append(rng.choice([-1.0, -0.0, 0.0, 1.0, 0.5], (300, 3, 3)))                                        # exact zeros of both signs
@@ -275,14 +317,18 @@ def test_model_free_device_bvh_build_on_degenerate_and_non_finite_input():
         idx = np.arange(len(v), dtype=np.int32)
         nrm = np.ascontiguousarray(rng.uniform(-1, 1, v.shape), dtype=np.float32)
         for q in (1, 0, 2):
+            to, no = orc.build_bvh(v, idx, nrm, q)
             th, nh, _ = rt.build_bvh(v, idx, nrm, q)
             tg, ng = gpu.build_bvh(v, idx, nrm, q)
-            assert len(ng) == len(nh) and np.array_equal(ng.view(np.uint8), nh.view(np.uint8)) and np.array_equal(tg.view(np.uint8), th.view(np.uint8))
-    # a tree with more than 2n + 1 nodes (chains of empty children below an infinite box): both builders refuse, neither hangs
+            assert len(nh) == len(no) and np.array_equal(nh.view(np.uint8), no.view(np.uint8)) and np.array_equal(th.view(np.uint8), to.view(np.uint8))
+            assert len(ng) == len(no) and np.array_equal(ng.view(np.uint8), no.view(np.uint8)) and np.array_equal(tg.view(np.uint8), to.view(np.uint8))
+    # a tree with more than 2n + 1 nodes (chains of empty children below an infinite box): every builder refuses, none hangs
     t = soup[:20].copy(); t[17, 1, 0] = np.inf
     v = np.ascontiguousarray(t.reshape(-1, 3), dtype=np.float32); idx = np.arange(len(v), dtype=np.int32)
     with pytest.raises(ValueError):
         rt.build_bvh(v, idx, v, 1)
     with pytest.raises(capi.RtError):
+        orc.build_bvh(v, idx, v, 1)
+    with pytest.raises(capi.RtError):
         gpu.build_bvh(v, idx, v, 1)
-    gpu.destroy()
+    gpu.destroy(); orc.destroy()

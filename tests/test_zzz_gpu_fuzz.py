@@ -1,5 +1,5 @@
 """The randomised searches of tools/ against the real kernels (librt_b200.so on the H100): random scenes, random sessions of host calls and
-random meshes for rtBuildBVH, compared bit for bit with the oracle / the host builder.  Sorts last, so that `pytest -x -m gpu` reaches it
+random meshes for rtBuildBVH and the host builder, compared bit for bit with the oracle.  Sorts last, so that `pytest -x -m gpu` reaches it
 after every hand-made case.  On the CPU the same searches run against the SIMT interpreter build (tests/test_fuzz_smoke.py)."""
 import os
 import subprocess
@@ -15,7 +15,8 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("tool,args", [("simt_fuzz.py", ["--cases", "250", "--seed", "301", "--far", "0.03", "--spheres", "0.06", "--odd", "0.1"]),
                                        ("simt_fuzz_session.py", ["--cases", "50", "--seed", "302"]),
-                                       ("simt_fuzz_bvh.py", ["--cases", "150", "--seed", "303"])])
+                                       ("simt_fuzz_bvh.py", ["--cases", "150", "--seed", "303"]),
+                                       ("simt_fuzz_bvh.py", ["--cases", "60", "--seed", "304", "--large", "--odd", "0.5"])])
 def test_randomised_search_on_the_gpu_finds_nothing(tool, args):
     r = subprocess.run([sys.executable, os.path.join(REPO, "tools", tool), "--lib", CUDA_LIB] + args, capture_output=True, text=True, timeout=1200)
     assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
