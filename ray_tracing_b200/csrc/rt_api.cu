@@ -25,6 +25,8 @@
 #include <cstring>
 #include <string>
 #include <thread>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 using namespace rtd;
@@ -134,6 +136,104 @@ static int failCuda(RtContext* c, cudaError_t e, const char* what)
     return fail(c, RT_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 
+// The calls that work on one GPU's images only refuse every context of a group (rtCreateMulti); the calls a group makes on all its
+// GPUs refuse the contexts it made for its followers
+static int refuseGroup(RtContext* c, const char* what)
+{
+    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, std::string(what) + ": not available on a group context (rtCreateMulti)");
+    return RT_OK;
+}
+static int refuseMember(RtContext* c, const char* what)
+{
+    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; call it on the context rtCreateMulti returned");
+    return RT_OK;
+}
+
+// `one` on the context, then on each follower of its group; a follower's failure is reported on the context
+template <class F> static int forGroup(RtContext* c, F one)
+{
+    int rc = one(c);
+    if (rc != RT_OK || !c) return rc;
+    for (RtContext* m : c->followers) if ((rc = one(m)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
+    return RT_OK;
+}
+
+// ---- the named per-pixel images: one W x H DevBuf each, served by name to rtReadback and rtGetDevicePointer -----------------------
+template <class T> static int allocateZeroed(RtContext* c, DevBuf<T>& b, size_t n)
+{
+    CK(b.ensure(n));
+    CK(cudaMemsetAsync(b.p, 0, n * sizeof(T), c->stream));
+    return RT_OK;
+}
+
+// An image's DevBuf field of RtContext, whatever its element type
+struct ImageBuf
+{
+    size_t element;                                  // bytes per pixel
+    void* (*p)(const RtContext*);
+    size_t (*count)(const RtContext*);
+    int (*allocateZeroed)(RtContext*, size_t n);
+    void (*release)(RtContext*);
+};
+template <auto F> static constexpr ImageBuf imageBuf()
+{
+    using T = std::remove_reference_t<decltype(*(std::declval<RtContext&>().*F).p)>;
+    return {sizeof(T), [](const RtContext* c) -> void* { return (c->*F).p; }, [](const RtContext* c) { return (c->*F).count; },
+            [](RtContext* c, size_t n) { return allocateZeroed(c, c->*F, n); }, [](RtContext* c) { (c->*F).release(); }};
+}
+
+struct NamedImage
+{
+    const char* name;
+    ImageBuf buf;
+    const char* producer;                            // the call that allocates it, for the "no ... yet" refusal
+    bool resizeAlways;                               // rtResize allocates it; the others follow a new size only once allocated
+    bool resetAccumulated;                           // RT_KERNEL_RESET_ACCUMULATED zeroes its region: it accumulates over the same frames
+    bool readback;                                   // rtReadback serves it (PixelStats has rtReadbackPixelStats)
+    bool refuseGroup;                                // rtReadback / rtGetDevicePointer refuse a group context
+};
+
+// A new size zeroes every allocated image; the producers that do not write every pixel allocate theirs zero-filled (allocateZeroed)
+static const NamedImage kImages[] = {
+    // name                buffer                                  producer                                            resize reset  read   group
+    {"FrameRender",       imageBuf<&RtContext::frame>(),         "rtResize",                                         true,  false, true,  false},
+    {"AccumulatedRender", imageBuf<&RtContext::accum>(),         "rtResize",                                         true,  true,  true,  false},
+    {"PixelStats",        imageBuf<&RtContext::pixelStats>(),    "counting dispatch (rtSetOption(\"countStats\", 1))", false, false, false, false},
+    {"FeatureFrame",      imageBuf<&RtContext::featureFrame>(),  "rtDispatchFeatures",                               false, false, true,  true},
+    {"AccumulatedAlbedo", imageBuf<&RtContext::accumAlbedo>(),   "rtDispatchFeatures",                               false, true,  true,  true},
+    {"AccumulatedNormal", imageBuf<&RtContext::accumNormal>(),   "rtDispatchFeatures",                               false, true,  true,  true},
+    {"DenoisedRender",    imageBuf<&RtContext::denoised>(),      "rtDenoise",                                        false, false, true,  true},
+    {"TemporalFrame",     imageBuf<&RtContext::temporalFrame>(), "rtDenoiseTemporal",                                false, false, true,  true},
+    {"AdaptiveMoments",   imageBuf<&RtContext::moments>(),       "rtDispatchAdaptive",                               false, true,  true,  true},
+};
+
+static const NamedImage* findImage(const char* name)
+{
+    for (const NamedImage& img : kImages) if (strcmp(img.name, name) == 0) return &img;
+    return nullptr;
+}
+
+static int imageReady(RtContext* c, const NamedImage& img, const char* what)
+{
+    if (img.refuseGroup) { int rc = refuseGroup(c, what); if (rc != RT_OK) return rc; }
+    if (!img.buf.p(c)) return fail(c, RT_E_STATE, std::string(what) + ": no " + img.producer + " yet");
+    return RT_OK;
+}
+
+// The synchronous display calls: wait for a pipelined copy (it may still read `display`), `encode` n pixels into `display`, copy it to dst
+template <class Encode> static int displayTo(RtContext* c, Encode encode, uint8_t* dst, size_t bytes)
+{
+    const size_t n = bytes / 4;
+    CK(cudaSetDevice(c->device));
+    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
+    CK(c->display.ensure(n));
+    int rc = encode(n); if (rc != RT_OK) return rc;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
 static int drainEvents(RtContext* c)
 {
     for (auto& ev : c->pending)
@@ -227,11 +327,11 @@ int rtDestroy(RtContext* c)
     c->snap.release();
     c->buildArena.release(); c->handoff.release(); c->poolCold.release();
     for (int k = 0; k < 2; k++) { if (c->stageBuf[k]) cudaFreeHost(c->stageBuf[k]); if (c->stageEv[k]) cudaEventDestroy(c->stageEv[k]); }
-    c->frame.release(); c->accum.release(); c->tileSend.release(); c->tileRecv.release(); c->display.release();
-    c->pixelStats.release(); c->queryRays.release(); c->queryHits.release();
-    c->featureFrame.release(); c->accumAlbedo.release(); c->accumNormal.release(); c->cameraRays.release();
-    c->denoised.release(); c->denoiseScratch.release(); c->temporalFrame.release(); c->temporalHist.release();
-    c->moments.release(); c->adaptiveList.release(); c->adaptiveScratch.release();
+    for (const NamedImage& img : kImages) img.buf.release(c);
+    c->tileSend.release(); c->tileRecv.release(); c->display.release();
+    c->queryRays.release(); c->queryHits.release(); c->cameraRays.release();
+    c->denoiseScratch.release(); c->temporalHist.release();
+    c->adaptiveList.release(); c->adaptiveScratch.release();
     if (c->adaptiveCount) cudaFreeHost(c->adaptiveCount);
     c->repack.release();
     closePeers(c);
@@ -387,38 +487,11 @@ static int one_rtResize(RtContext* c, int w, int h)
     {
         if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
         const size_t n = (size_t)w * h;
-        CK(c->frame.ensure(n)); CK(c->accum.ensure(n));
-        CK(cudaMemsetAsync(c->frame.p, 0, n * 16, c->stream));
-        CK(cudaMemsetAsync(c->accum.p, 0, n * 16, c->stream));
-        if (c->pixelStats.p)                                // the per-pixel counters follow the image size, zero-filled
-        {
-            CK(c->pixelStats.ensure(n));
-            CK(cudaMemsetAsync(c->pixelStats.p, 0, n * sizeof(RtPixelStats), c->stream));
-        }
-        if (c->featureFrame.p)                              // so do the feature images
-        {
-            CK(c->featureFrame.ensure(n)); CK(c->accumAlbedo.ensure(n)); CK(c->accumNormal.ensure(n));
-            CK(cudaMemsetAsync(c->featureFrame.p, 0, n * sizeof(RtPixelFeatures), c->stream));
-            CK(cudaMemsetAsync(c->accumAlbedo.p, 0, n * 16, c->stream));
-            CK(cudaMemsetAsync(c->accumNormal.p, 0, n * 16, c->stream));
-        }
-        if (c->denoised.p)                                  // the denoised image is zeroed, its scratch freed
-        {
-            CK(c->denoised.ensure(n));
-            CK(cudaMemsetAsync(c->denoised.p, 0, n * 16, c->stream));
-        }
+        for (const NamedImage& img : kImages)
+            if (img.resizeAlways || img.buf.p(c)) { int rc = img.buf.allocateZeroed(c, n); if (rc != RT_OK) return rc; }
+        // the scratch images are freed: the denoiser's, the temporal history (discarded), the adaptive pixel list, the camera's rays
         c->denoiseScratch.release();
-        if (c->temporalFrame.p)                             // TemporalFrame is zeroed, the temporal history discarded
-        {
-            CK(c->temporalFrame.ensure(n));
-            CK(cudaMemsetAsync(c->temporalFrame.p, 0, n * 16, c->stream));
-        }
         c->temporalHist.release(); c->temporalHistory = false;
-        if (c->moments.p)                                   // the moments start again from zero
-        {
-            CK(c->moments.ensure(n));
-            CK(cudaMemsetAsync(c->moments.p, 0, n * 16, c->stream));
-        }
         c->adaptiveList.release(); c->adaptiveScratch.release();
         c->cameraRays.release();
         c->width = w; c->height = h;
@@ -483,75 +556,16 @@ static int one_rtSetOption(RtContext* c, const char* name, int value)
 // ---- the setters of a context that leads a group (rtCreateMulti) reach every GPU of the group ----
 int rtSetBuffer(RtContext* c, const char* name, const void* data, int count, int stride)
 {
-    int rc = one_rtSetBuffer(c, name, data, count, stride);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetBuffer(m, name, data, count, stride)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
+    return forGroup(c, [&](RtContext* m) { return one_rtSetBuffer(m, name, data, count, stride); });
 }
-
-int rtSetInt(RtContext* c, const char* name, int v)
-{
-    int rc = one_rtSetInt(c, name, v);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetInt(m, name, v)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtSetInts(RtContext* c, const char* name, const int* v, int n)
-{
-    int rc = one_rtSetInts(c, name, v, n);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetInts(m, name, v, n)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtSetFloat(RtContext* c, const char* name, float v)
-{
-    int rc = one_rtSetFloat(c, name, v);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetFloat(m, name, v)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtSetVector(RtContext* c, const char* name, const float v[4])
-{
-    int rc = one_rtSetVector(c, name, v);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetVector(m, name, v)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtSetMatrix(RtContext* c, const char* name, const float v[16])
-{
-    int rc = one_rtSetMatrix(c, name, v);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetMatrix(m, name, v)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtSetBool(RtContext* c, const char* name, int v)
-{
-    int rc = one_rtSetBool(c, name, v);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetBool(m, name, v)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtResize(RtContext* c, int w, int h)
-{
-    int rc = one_rtResize(c, w, h);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtResize(m, w, h)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
-
-int rtSetOption(RtContext* c, const char* name, int value)
-{
-    int rc = one_rtSetOption(c, name, value);
-    if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtSetOption(m, name, value)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    return RT_OK;
-}
+int rtSetInt(RtContext* c, const char* name, int v) { return forGroup(c, [&](RtContext* m) { return one_rtSetInt(m, name, v); }); }
+int rtSetInts(RtContext* c, const char* name, const int* v, int n) { return forGroup(c, [&](RtContext* m) { return one_rtSetInts(m, name, v, n); }); }
+int rtSetFloat(RtContext* c, const char* name, float v) { return forGroup(c, [&](RtContext* m) { return one_rtSetFloat(m, name, v); }); }
+int rtSetVector(RtContext* c, const char* name, const float v[4]) { return forGroup(c, [&](RtContext* m) { return one_rtSetVector(m, name, v); }); }
+int rtSetMatrix(RtContext* c, const char* name, const float v[16]) { return forGroup(c, [&](RtContext* m) { return one_rtSetMatrix(m, name, v); }); }
+int rtSetBool(RtContext* c, const char* name, int v) { return forGroup(c, [&](RtContext* m) { return one_rtSetBool(m, name, v); }); }
+int rtResize(RtContext* c, int w, int h) { return forGroup(c, [&](RtContext* m) { return one_rtResize(m, w, h); }); }
+int rtSetOption(RtContext* c, const char* name, int value) { return forGroup(c, [&](RtContext* m) { return one_rtSetOption(m, name, value); }); }
 
 // Automatic choice: with meshes the pooled wavefront kernel wins (BVH traversal needs the ray queue);
 // for sphere-only scenes every ray costs the same and one path per lane avoids the pool's shared-memory round trips.
@@ -728,6 +742,52 @@ static void bindScene(const RtContext* c, DevParams& P)
     P.tlasRootStart = c->repack.tlasRootStart; P.tlasRootCount = c->repack.tlasRootCount;
 }
 
+// The parameter block of a launch that is not a camera render (queries, paths, features): the scene and the counters, no images, no peers
+static DevParams queryParams(const RtContext* c)
+{
+    DevParams P = c->P;
+    bindScene(c, P);
+    P.countStats = c->optCountStats;
+    P.smemPairs = 0;                                 // no tree-top staging: every record from global memory
+    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    return P;
+}
+
+// The boxes the models' and the spheres' padding was computed for (QueryParams, PathParams)
+static void sceneBounds(const RtContext* c, float modelLo[3], float modelHi[3], float sphLo[3], float sphHi[3])
+{
+    for (int a = 0; a < 3; a++)
+    {
+        modelLo[a] = c->repack.modelBoundLo[a]; modelHi[a] = c->repack.modelBoundHi[a];
+        sphLo[a] = c->repack.sphBoundLo[a]; sphHi[a] = c->repack.sphBoundHi[a];
+    }
+}
+
+// The pixels groups of 8 x 8 cover: limX x limY, none when gz = 0
+static void groupLimits(int gx, int gy, int gz, unsigned W, unsigned H, unsigned& limX, unsigned& limY)
+{
+    limX = (unsigned long long)gx * 8ull < W ? (unsigned)gx * 8u : W;
+    limY = (unsigned long long)gy * 8ull < H ? (unsigned)gy * 8u : H;
+    if (gz == 0) limX = limY = 0;
+}
+
+// The rows among the first limY that the bands of bandRows rows, dealt round-robin to tileWorld ranks, give to `rank`
+static unsigned ownedRows(unsigned limY, int bandRows, int tileWorld, int rank)
+{
+    unsigned rows = 0;
+    for (unsigned y0 = 0, b = 0; y0 < limY; y0 += (unsigned)bandRows, b++)
+        if ((int)(b % (unsigned)tileWorld) == rank) rows += limY - y0 < (unsigned)bandRows ? limY - y0 : (unsigned)bandRows;
+    return rows;
+}
+
+// A pair of timing events: one the context timed before and has read, or a new one
+static int takeEventPair(RtContext* c, EventPair& ev)
+{
+    if (!c->freeEvents.empty()) { ev = c->freeEvents.back(); c->freeEvents.pop_back(); }
+    else { CK(cudaEventCreate(&ev.a)); CK(cudaEventCreate(&ev.b)); }
+    return RT_OK;
+}
+
 // rtDispatchAdaptive's arguments (dispatchLocal); `active` receives the number of pixels traced
 struct AdaptiveCall { float threshold; int minFrames, maxFrames; long long active; };
 
@@ -743,21 +803,17 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     if ((int)c->P.W != c->width || (int)c->P.H != c->height) return fail(c, RT_E_STATE, "rtDispatch: Resolution does not match the render textures");
     CK(cudaSetDevice(c->device));
     const unsigned W = c->P.W, H = c->P.H;
-    unsigned limX = (unsigned long long)gx * 8ull < W ? (unsigned)gx * 8u : W;
-    unsigned limY = (unsigned long long)gy * 8ull < H ? (unsigned)gy * 8u : H;
-    if (gz == 0) limX = limY = 0;
+    unsigned limX, limY;
+    groupLimits(gx, gy, gz, W, H, limX, limY);
 
     if (kernelIndex == RT_KERNEL_RESET_ACCUMULATED)            // RC:26-32
     {
         if (limX == 0 || limY == 0) return RT_OK;
-        CK(cudaMemset2DAsync(c->accum.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
-        if (c->accumAlbedo.p)                                  // the guides are averaged over the same frames as the colour
+        for (const NamedImage& img : kImages)
         {
-            CK(cudaMemset2DAsync(c->accumAlbedo.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
-            CK(cudaMemset2DAsync(c->accumNormal.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
+            void* p = img.resetAccumulated ? img.buf.p(c) : nullptr;
+            if (p) CK(cudaMemset2DAsync(p, (size_t)W * img.buf.element, 0, (size_t)limX * img.buf.element, limY, c->stream));
         }
-        if (c->moments.p)                                      // so are the adaptive moments
-            CK(cudaMemset2DAsync(c->moments.p, (size_t)W * 16, 0, (size_t)limX * 16, limY, c->stream));
         return RT_OK;
     }
     if (kernelIndex != RT_KERNEL_RAYTRACE) return fail(c, RT_E_INVALID, "rtDispatch: kernelIndex must be 0 (RayTrace) or 1 (ResetAccumulated)");
@@ -766,12 +822,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     if (c->P.MaxBounceCount > 200 || W > 65535u || H > 65535u) return fail(c, RT_E_STATE, "rtDispatch: MaxBounceCount > 200 or a resolution above 65535 is not supported");
     if (c->P.MaxBounceCount < 0) return fail(c, RT_E_STATE, "rtDispatch: MaxBounceCount is negative (the reference clamps it to [0, 32], RCM:15)");
 
-    {
-        unsigned long long rows = 0;
-        for (unsigned int y0 = 0, b = 0; y0 < limY; y0 += (unsigned int)c->bandRows, b++)
-            if ((int)(b % (unsigned int)c->tileWorld) == c->tileRank) rows += (limY - y0) < (unsigned int)c->bandRows ? (limY - y0) : (unsigned int)c->bandRows;
-        c->dispatchPixels = rows * limX;
-    }
+    c->dispatchPixels = (unsigned long long)ownedRows(limY, c->bandRows, c->tileWorld, c->tileRank) * limX;
     c->dispatchFrames = frames;
     int rc = RT_OK;
     if (ad)
@@ -785,19 +836,9 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     }
     rc = prepareScene(c);
     if (rc != RT_OK) return rc;
-    if (ad && !c->moments.p)                               // the first traced call allocates the moments, zero-filled
-    {
-        const size_t n = (size_t)W * H;
-        CK(c->moments.ensure(n));
-        CK(cudaMemsetAsync(c->moments.p, 0, n * 16, c->stream));
-    }
+    if (ad && !c->moments.p && (rc = allocateZeroed(c, c->moments, (size_t)W * H)) != RT_OK) return rc;       // the first traced call allocates the moments
     applyL2Persistence(c);
-    if (c->optCountStats && !c->pixelStats.p)              // the first counting dispatch allocates the per-pixel counters
-    {
-        const size_t n = (size_t)W * H;
-        CK(c->pixelStats.ensure(n));
-        CK(cudaMemsetAsync(c->pixelStats.p, 0, n * sizeof(RtPixelStats), c->stream));
-    }
+    if (c->optCountStats && !c->pixelStats.p && (rc = allocateZeroed(c, c->pixelStats, (size_t)W * H)) != RT_OK) return rc;     // so does the first counting dispatch the per-pixel counters
 
     DevParams P = c->P;
     P.limX = limX; P.limY = limY;
@@ -821,8 +862,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     for (int k = 0; k < c->nPeers; k++) { P.peerFrame[k] = c->peerFrame[k]; P.peerAccum[k] = c->peerAccum[k]; }
 
     EventPair ev;
-    if (!c->freeEvents.empty()) { ev = c->freeEvents.back(); c->freeEvents.pop_back(); }
-    else { CK(cudaEventCreate(&ev.a)); CK(cudaEventCreate(&ev.b)); }
+    if ((rc = takeEventPair(c, ev)) != RT_OK) return rc;
     if (c->pending.size() >= 512) { rc = drainEvents(c); if (rc != RT_OK) return rc; }
 
     int kernel = effectiveKernel(c);
@@ -847,106 +887,64 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
         }
         P.handoff = c->handoff.p; P.chunkSerial = (int)c->chunkSerial;
     }
-    if (ad)
+    if (kernel == 2 && POOL_COLD_WORDS > 0)
     {
-        const unsigned count = (unsigned)ad->active;
-        cudaError_t e = cudaSuccess;
-        if (kernel == 0)
-        {
-            CK(cudaEventRecord(ev.a, c->stream));
-            RT_LAUNCH((count + 63u) / 64u, 64, 0, c->stream, k_raytrace_mega_list<64>, P, count, c->adaptiveList.p, c->moments.p);
-            CK(cudaEventRecord(ev.b, c->stream));
-        }
-        else if (kernel == 1)
-        {
-            P.pixelList = c->adaptiveList.p; P.adaptiveMoments = c->moments.p;       // (the hand-off's and the cold pool's slots: unused here)
-            e = wave_launch_list(P, c->numSMs, count, c->stream, ev.a, ev.b);
-        }
-        else
-        {
-            if (POOL_COLD_WORDS > 0)
-            {
-                CK(c->poolCold.ensure((size_t)c->numSMs * POOL_WARPS * POOL_COLD_WORDS * 96));
-                P.poolCold = c->poolCold.p;
-            }
-            e = pool_launch_list(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b, count, c->adaptiveList.p, c->moments.p);
-        }
-        if (e != cudaSuccess) return failCuda(c, e, "adaptive launch");
+        CK(c->poolCold.ensure((size_t)c->numSMs * POOL_WARPS * POOL_COLD_WORDS * 96));      // sized for the largest pools
+        P.poolCold = c->poolCold.p;
     }
-    else if (kernel == 0)
+    // ad: the same kernels over the selected pixels only (adaptiveList, count long), with their moments
+    const unsigned count = ad ? (unsigned)ad->active : 0u;
+    cudaError_t e = cudaSuccess;
+    if (kernel == 0)
     {
         CK(cudaEventRecord(ev.a, c->stream));
         dim3 grid((limX + 7) / 8, (limY + 7) / 8, 1), block(8, 8, 1);
-        if (frames > 1) RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega_frames, P);
+        if (ad) RT_LAUNCH((count + 63u) / 64u, 64, 0, c->stream, k_raytrace_mega_list<64>, P, count, c->adaptiveList.p, c->moments.p);
+        else if (frames > 1) RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega_frames, P);
         else RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega, P);
         CK(cudaEventRecord(ev.b, c->stream));
     }
-    else if (kernel == 1)
+    else if (kernel == 1 && ad)
     {
-        cudaError_t e = wave_launch(P, c->numSMs, c->stream, ev.a, ev.b);
-        if (e != cudaSuccess) return failCuda(c, e, "wavefront launch");
+        P.pixelList = c->adaptiveList.p; P.adaptiveMoments = c->moments.p;       // (the hand-off's and the cold pool's slots: unused here)
+        e = wave_launch_list(P, c->numSMs, count, c->stream, ev.a, ev.b);
     }
-    else
-    {
-        if (POOL_COLD_WORDS > 0)
-        {
-            CK(c->poolCold.ensure((size_t)c->numSMs * POOL_WARPS * POOL_COLD_WORDS * 96));      // sized for the largest pools
-            P.poolCold = c->poolCold.p;
-        }
-        cudaError_t e = pool_launch(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b);
-        if (e != cudaSuccess) return failCuda(c, e, "pool wavefront launch");
-    }
+    else if (kernel == 1) e = wave_launch(P, c->numSMs, c->stream, ev.a, ev.b);
+    else if (ad) e = pool_launch_list(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b, count, c->adaptiveList.p, c->moments.p);
+    else e = pool_launch(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b);
+    if (e != cudaSuccess) return failCuda(c, e, ad ? "adaptive launch" : kernel == 1 ? "wavefront launch" : "pool wavefront launch");
     CK(cudaGetLastError());
     c->pending.push_back(ev);
     c->stats.dispatches += (unsigned long long)frames;
     return RT_OK;
 }
 
-// The feature images exist after the first rtDispatchFeatures, on a single context
-static int featuresReady(RtContext* c, const char* what)
-{
-    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, std::string(what) + ": the feature images are not available on a group context (rtCreateMulti)");
-    if (!c->featureFrame.p) return fail(c, RT_E_STATE, std::string(what) + ": no rtDispatchFeatures yet");
-    return RT_OK;
-}
-
 int rtReadback(RtContext* c, const char* tex, float* dst, size_t bytes)
 {
     if (!c || !tex || !dst) return fail(c, RT_E_INVALID, "rtReadback: bad argument");
-    const std::string n(tex);
-    const bool feature = n == "FeatureFrame" || n == "AccumulatedAlbedo" || n == "AccumulatedNormal";
-    if (feature) { int rc = featuresReady(c, "rtReadback"); if (rc != RT_OK) return rc; }
-    if (n == "DenoisedRender" && !c->denoised.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoise yet");
-    if (n == "TemporalFrame" && !c->temporalFrame.p) return fail(c, RT_E_STATE, "rtReadback: no rtDenoiseTemporal yet");
-    if (n == "AdaptiveMoments" && !c->moments.p) return fail(c, RT_E_STATE, "rtReadback: no rtDispatchAdaptive yet");
-    const void* src = n == "FrameRender" ? (const void*)c->frame.p : n == "AccumulatedRender" ? (const void*)c->accum.p : n == "FeatureFrame" ? (const void*)c->featureFrame.p :
-                      n == "AccumulatedAlbedo" ? (const void*)c->accumAlbedo.p : n == "AccumulatedNormal" ? (const void*)c->accumNormal.p :
-                      n == "DenoisedRender" ? (const void*)c->denoised.p : n == "TemporalFrame" ? (const void*)c->temporalFrame.p :
-                      n == "AdaptiveMoments" ? (const void*)c->moments.p : nullptr;
-    if (n != "FrameRender" && n != "AccumulatedRender" && n != "DenoisedRender" && n != "TemporalFrame" && n != "AdaptiveMoments" && !feature) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
-    if (!src) return fail(c, RT_E_STATE, "rtReadback: rtResize has not been called");
-    if (bytes != (size_t)c->width * c->height * (n == "FeatureFrame" ? sizeof(RtPixelFeatures) : 16))
-        return fail(c, RT_E_INVALID, n == "FeatureFrame" ? "rtReadback: bytes must equal W*H*32" : "rtReadback: bytes must equal W*H*16");
+    const NamedImage* img = findImage(tex);
+    if (!img || !img->readback) return fail(c, RT_E_UNKNOWN_NAME, std::string("rtReadback: unknown texture ") + tex);
+    int rc = imageReady(c, *img, "rtReadback"); if (rc != RT_OK) return rc;
+    if (bytes != (size_t)c->width * c->height * img->buf.element)
+        return fail(c, RT_E_INVALID, "rtReadback: bytes must equal W*H*" + std::to_string(img->buf.element));
     CK(cudaSetDevice(c->device));
-    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(dst, img->buf.p(c), bytes, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
     return RT_OK;
+}
+
+// rtDisplay's encode of n pixels of src into `display` (tex / Frame as the sRGB 8-bit back buffer)
+static void encodeDisplay(RtContext* c, const float4* src, size_t n, float frame)
+{
+    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, src, c->display.p, n, frame);
 }
 
 int rtDisplay(RtContext* c, int useAccumulated, int Frame, uint8_t* dst, size_t bytes)
 {
     if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplay: bad argument");
     if (!c->frame.p) return fail(c, RT_E_STATE, "rtDisplay: rtResize has not been called");
-    const size_t n = (size_t)c->width * c->height;
-    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplay: bytes must equal W*H*4");
-    CK(cudaSetDevice(c->device));
-    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
-    CK(c->display.ensure(n));
-    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, useAccumulated ? c->accum.p : c->frame.p, c->display.p, n, (float)Frame);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    if (bytes != (size_t)c->width * c->height * 4) return fail(c, RT_E_INVALID, "rtDisplay: bytes must equal W*H*4");
+    return displayTo(c, [&](size_t n) { encodeDisplay(c, useAccumulated ? c->accum.p : c->frame.p, n, (float)Frame); return RT_OK; }, dst, bytes);
 }
 
 // ---- pipelined readback -------------------------------------------------------------------------------------------------------
@@ -992,7 +990,7 @@ int rtDisplayAsync(RtContext* c, int useAccumulated, int Frame, uint8_t* dst, si
     CK(cudaSetDevice(c->device));
     int rc = copyPipeline(c); if (rc != RT_OK) return rc;
     CK(c->display.ensure(n));
-    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, useAccumulated ? c->accum.p : c->frame.p, c->display.p, n, (float)Frame);
+    encodeDisplay(c, useAccumulated ? c->accum.p : c->frame.p, n, (float)Frame);
     CK(cudaGetLastError());
     return copyOut(c, dst, c->display.p, bytes);
 }
@@ -1019,13 +1017,7 @@ int rtSynchronize(RtContext* c)
 
 // ---- multi-GPU tile staging -----------------------------------------------------------------------------------------------
 
-static size_t tileRows(const RtContext* c, int rank)
-{
-    size_t rows = 0;
-    for (int y0 = 0, b = 0; y0 < c->height; y0 += c->bandRows, b++)
-        if (b % c->tileWorld == rank) rows += (size_t)((c->height - y0) < c->bandRows ? (c->height - y0) : c->bandRows);
-    return rows;
-}
+static size_t tileRows(const RtContext* c, int rank) { return ownedRows((unsigned)c->height, c->bandRows, c->tileWorld, rank); }
 
 static int ensureTileBuffers(RtContext* c)
 {
@@ -1065,14 +1057,6 @@ int rtUnpackTiles(RtContext* c)
 // true when a RayTrace dispatch on this context is followed by the all-gather of the frame's tiles
 static bool exchanges(const RtContext* c) { return c->optExchange && c->tileWorld > 1 && (c->comm || !c->followers.empty() || c->leader); }
 
-static int beginExchangeTiming(RtContext* c, EventPair& ev)
-{
-    if (!c->freeEvents.empty()) { ev = c->freeEvents.back(); c->freeEvents.pop_back(); }
-    else { CK(cudaEventCreate(&ev.a)); CK(cudaEventCreate(&ev.b)); }
-    CK(cudaEventRecord(ev.a, c->stream));
-    return RT_OK;
-}
-
 static int ncclFail(RtContext* c, NcclApi* api, int r, const char* what)
 {
     return fail(c, RT_E_CUDA, std::string(what) + ": " + (api && api->GetErrorString ? api->GetErrorString(r) : "NCCL error") + " (" + std::to_string(r) + ")");
@@ -1088,7 +1072,8 @@ static int exchangeTiles(RtContext* const* cs, int n)
     {
         RtContext* c = cs[i];
         CK(cudaSetDevice(c->device));
-        int rc = beginExchangeTiming(c, evs[i]); if (rc != RT_OK) return rc;
+        int rc = takeEventPair(c, evs[i]); if (rc != RT_OK) return rc;
+        CK(cudaEventRecord(evs[i].a, c->stream));
         rc = rtPackTile(c); if (rc != RT_OK) return i ? fail(lead, rc, c->err) : rc;
     }
 #ifdef RT_SIMT_EMU
@@ -1122,53 +1107,49 @@ static int exchangeTiles(RtContext* const* cs, int n)
     return RT_OK;
 }
 
-int rtDispatch(RtContext* c, int kernelIndex, int gx, int gy, int gz)
+// The exchange over this context and the followers of its group
+static int exchangeGroup(RtContext* c)
 {
-    if (!c) return RT_E_INVALID;
-    if (c->leader) return fail(c, RT_E_STATE, "rtDispatch: this context belongs to a group; dispatch on the context rtCreateMulti returned");
-    int rc = dispatchLocal(c, kernelIndex, gx, gy, gz);
-    if (rc != RT_OK) return rc;
-    for (RtContext* m : c->followers)
-        if ((rc = dispatchLocal(m, kernelIndex, gx, gy, gz)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
-    if (!c->followers.empty()) CK(cudaSetDevice(c->device));
-    const bool traced = kernelIndex == RT_KERNEL_RAYTRACE && gz != 0 && gx > 0 && gy > 0;
-    if (!traced || !exchanges(c)) return RT_OK;
     std::vector<RtContext*> all(1, c);
     all.insert(all.end(), c->followers.begin(), c->followers.end());
     return exchangeTiles(all.data(), (int)all.size());
 }
 
+int rtDispatch(RtContext* c, int kernelIndex, int gx, int gy, int gz)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = refuseMember(c, "rtDispatch"); if (rc != RT_OK) return rc;
+    if ((rc = forGroup(c, [&](RtContext* m) { return dispatchLocal(m, kernelIndex, gx, gy, gz); })) != RT_OK) return rc;
+    if (!c->followers.empty()) CK(cudaSetDevice(c->device));
+    const bool traced = kernelIndex == RT_KERNEL_RAYTRACE && gz != 0 && gx > 0 && gy > 0;
+    if (!traced || !exchanges(c)) return RT_OK;
+    return exchangeGroup(c);
+}
+
 int rtDispatchFrames(RtContext* c, int gx, int gy, int gz, int frameCount)
 {
     if (!c) return RT_E_INVALID;
-    if (c->leader) return fail(c, RT_E_STATE, "rtDispatchFrames: this context belongs to a group; dispatch on the context rtCreateMulti returned");
+    int rc = refuseMember(c, "rtDispatchFrames"); if (rc != RT_OK) return rc;
     const long long chain = (long long)frameCount * (c->P.NumRaysPerPixel > 1 ? c->P.NumRaysPerPixel : 1);
     if (frameCount < 1 || chain > RT_MAX_BATCH_SAMPLES)
         return fail(c, RT_E_INVALID, "rtDispatchFrames: frameCount must be >= 1 and frameCount * max(1, NumRaysPerPixel) at most RT_MAX_BATCH_SAMPLES");
     if (!c->P.accumulate) return fail(c, RT_E_STATE, "rtDispatchFrames: needs accumulate = 1 (without accumulation only the last frame is observable)");
     if (frameCount == 1) return rtDispatch(c, RT_KERNEL_RAYTRACE, gx, gy, gz);
     if (c->optSampleChunks >= 2) return fail(c, RT_E_STATE, "rtDispatchFrames: a batch of frames runs whole pixels; sampleChunks is forced to 2 or more");
-    int rc = dispatchLocal(c, RT_KERNEL_RAYTRACE, gx, gy, gz, frameCount);
-    if (rc != RT_OK) return rc;
-    for (RtContext* m : c->followers)
-        if ((rc = dispatchLocal(m, RT_KERNEL_RAYTRACE, gx, gy, gz, frameCount)) != RT_OK) return fail(c, rc, "GPU " + std::to_string(m->device) + ": " + m->err);
+    if ((rc = forGroup(c, [&](RtContext* m) { return dispatchLocal(m, RT_KERNEL_RAYTRACE, gx, gy, gz, frameCount); })) != RT_OK) return rc;
     if (!c->followers.empty()) CK(cudaSetDevice(c->device));
     const bool traced = gz != 0 && gx > 0 && gy > 0;
     if (!traced || !exchanges(c)) return RT_OK;
-    std::vector<RtContext*> all(1, c);                      // one exchange for the whole batch: it carries the last frame and the sum
-    all.insert(all.end(), c->followers.begin(), c->followers.end());
-    return exchangeTiles(all.data(), (int)all.size());
+    return exchangeGroup(c);                                // one exchange for the whole batch: it carries the last frame and the sum
 }
 
 // rtDispatchAdaptive's selection over this context's covered pixels, in the camera kernels' job order: the list and its length, read
 // back into ad.active (the call's one synchronisation).  Before the first traced call the moments are all zero (none allocated yet).
 static int adaptiveSelect(RtContext* c, unsigned limX, unsigned limY, AdaptiveCall& ad)
 {
-    unsigned int ownedRows = 0;
-    for (unsigned int y0 = 0, b = 0; y0 < limY; y0 += (unsigned int)c->bandRows, b++)
-        if ((int)(b % (unsigned int)c->tileWorld) == c->tileRank) ownedRows += (limY - y0) < (unsigned int)c->bandRows ? (limY - y0) : (unsigned int)c->bandRows;
+    const unsigned int rows = ownedRows(limY, c->bandRows, c->tileWorld, c->tileRank);
     const unsigned int tilesX = (limX + 7u) / 8u;
-    const unsigned long long jobs = (unsigned long long)tilesX * ((ownedRows + 3u) / 4u) * 32ull;       // < 2^32: W, H <= 65535
+    const unsigned long long jobs = (unsigned long long)tilesX * ((rows + 3u) / 4u) * 32ull;       // < 2^32: W, H <= 65535
     const unsigned int nBlocks = (unsigned int)((jobs + ADAPTIVE_BLOCK - 1) / ADAPTIVE_BLOCK);
     const size_t n = (size_t)c->width * c->height;
     CK(c->adaptiveList.ensure(n));
@@ -1177,7 +1158,7 @@ static int adaptiveSelect(RtContext* c, unsigned limX, unsigned limY, AdaptiveCa
     AdaptiveParams A;
     A.moments = c->moments.p;
     A.masks = c->adaptiveScratch.p; A.partials = A.masks + jobs / 32; A.count = A.partials + nBlocks; A.list = c->adaptiveList.p;
-    A.W = c->P.W; A.limX = limX; A.ownedRows = ownedRows; A.tilesX = tilesX; A.totalJobs = (unsigned int)jobs; A.nBlocks = nBlocks;
+    A.W = c->P.W; A.limX = limX; A.ownedRows = rows; A.tilesX = tilesX; A.totalJobs = (unsigned int)jobs; A.nBlocks = nBlocks;
     A.tileRank = c->tileRank; A.tileWorld = c->tileWorld; A.bandRows = c->bandRows;
     A.threshold = ad.threshold; A.minFrames = (float)ad.minFrames; A.maxFrames = (float)ad.maxFrames;
     cudaError_t e = adaptive_select(A, c->stream);
@@ -1196,13 +1177,13 @@ int rtDispatchAdaptive(RtContext* c, int gx, int gy, int gz, float threshold, in
     if (minFrames < 2) return fail(c, RT_E_INVALID, "rtDispatchAdaptive: minFrames must be at least 2");
     if (maxFrames < minFrames || maxFrames > RT_ADAPTIVE_MAX_FRAMES)
         return fail(c, RT_E_INVALID, "rtDispatchAdaptive: maxFrames must lie in minFrames .. RT_ADAPTIVE_MAX_FRAMES");
-    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDispatchAdaptive: not available on a group context (rtCreateMulti)");
+    int rc = refuseGroup(c, "rtDispatchAdaptive"); if (rc != RT_OK) return rc;
     if (c->comm) return fail(c, RT_E_STATE, "rtDispatchAdaptive: not available on a context with a communicator (rtCommInit)");
     if (c->nPeers > 0) return fail(c, RT_E_STATE, "rtDispatchAdaptive: not available on a context with peers (rtSetPeers)");
     if (!c->P.accumulate) return fail(c, RT_E_STATE, "rtDispatchAdaptive: needs accumulate = 1 (the moments count accumulated frames)");
     if (c->optSampleChunks >= 2) return fail(c, RT_E_STATE, "rtDispatchAdaptive: a pixel list runs whole pixels; sampleChunks is forced to 2 or more");
     AdaptiveCall ad; ad.threshold = threshold; ad.minFrames = minFrames; ad.maxFrames = maxFrames; ad.active = 0;
-    const int rc = dispatchLocal(c, RT_KERNEL_RAYTRACE, gx, gy, gz, 1, &ad);
+    rc = dispatchLocal(c, RT_KERNEL_RAYTRACE, gx, gy, gz, 1, &ad);
     if (rc != RT_OK) return rc;
     if (activePixels) *activePixels = (int64_t)ad.active;
     return RT_OK;
@@ -1212,18 +1193,14 @@ int rtDisplayMean(RtContext* c, uint8_t* dst, size_t bytes)
 {
     if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplayMean: bad argument");
     if (!c->accum.p) return fail(c, RT_E_STATE, "rtDisplayMean: rtResize has not been called");
-    const size_t n = (size_t)c->width * c->height;
-    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplayMean: bytes must equal W*H*4");
-    CK(cudaSetDevice(c->device));
-    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
-    CK(c->display.ensure(n));
-    CK(c->snap.ensure(n));                                  // the pipelined readback's snapshot image is free here (the copy was waited for)
-    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_mean_image, c->accum.p, c->snap.p, n);
-    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, c->snap.p, c->display.p, n, 1.0f);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    if (bytes != (size_t)c->width * c->height * 4) return fail(c, RT_E_INVALID, "rtDisplayMean: bytes must equal W*H*4");
+    return displayTo(c, [&](size_t n) -> int
+    {
+        CK(c->snap.ensure(n));                              // the pipelined readback's snapshot image is free here (the copy was waited for)
+        RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_mean_image, c->accum.p, c->snap.p, n);
+        encodeDisplay(c, c->snap.p, n, 1.0f);
+        return RT_OK;
+    }, dst, bytes);
 }
 
 // ---- closest-hit and occlusion queries (rtTraceRays, rtTraceOcclusion, rt_kernel_query.cuh) -----------------------------------------
@@ -1232,7 +1209,7 @@ static int stagedD2H(RtContext* c, void* dst, const void* src, size_t bytes);
 
 static int traceArgs(RtContext* c, const char* what, const void* rays, const void* hits, int n, int flags)
 {
-    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; trace on the context rtCreateMulti returned");
+    int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
     if (n < 0 || (n > 0 && (!rays || !hits))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or rays / hits NULL)");
     if (flags != 0 && flags != RT_TRACE_NO_CULL) return fail(c, RT_E_INVALID, std::string(what) + ": flags must be 0 or RT_TRACE_NO_CULL");
     return RT_OK;
@@ -1244,17 +1221,9 @@ static int traceArgs(RtContext* c, const char* what, const void* rays, const voi
 static int queryLocal(RtContext* c, const char* what, QueryParams& Q, int n, int flags, bool occlusion)
 {
     int rc = prepareQueryScene(c, what); if (rc != RT_OK) return rc;
-    DevParams P = c->P;
-    bindScene(c, P);
-    P.countStats = c->optCountStats;
-    P.smemPairs = 0;                                 // no tree-top staging: every record from global memory
-    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    const DevParams P = queryParams(c);
     Q.n = (unsigned int)n; Q.noCull = flags & RT_TRACE_NO_CULL;
-    for (int a = 0; a < 3; a++)
-    {
-        Q.modelLo[a] = c->repack.modelBoundLo[a]; Q.modelHi[a] = c->repack.modelBoundHi[a];
-        Q.sphLo[a] = c->repack.sphBoundLo[a]; Q.sphHi[a] = c->repack.sphBoundHi[a];
-    }
+    sceneBounds(c, Q.modelLo, Q.modelHi, Q.sphLo, Q.sphHi);
     cudaError_t e = occlusion ? query_launch<true>(P, Q, c->numSMs, c->stream) : query_launch<false>(P, Q, c->numSMs, c->stream);
     if (e != cudaSuccess) return failCuda(c, e, occlusion ? "rtTraceOcclusion launch" : "rtTraceRays launch");
     return RT_OK;
@@ -1347,7 +1316,7 @@ int rtTraceOcclusionDevice(RtContext* c, const void* dSegs, void* dOccluded, int
 // ---- radiance along caller-supplied rays (rtTracePaths, k_trace_paths in rt_kernel_query.cuh) ------------------------------------------
 static int pathArgs(RtContext* c, const char* what, const void* rays, const void* out, int n, int samples)
 {
-    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; trace on the context rtCreateMulti returned");
+    int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
     if (n < 0 || (n > 0 && (!rays || !out))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or rays / out NULL)");
     if (samples < 1 || samples > RT_MAX_BATCH_SAMPLES) return fail(c, RT_E_INVALID, std::string(what) + ": samples must be 1 .. RT_MAX_BATCH_SAMPLES");
     return RT_OK;
@@ -1360,18 +1329,10 @@ static int pathsLocal(RtContext* c, const RtPathRay* dRays, RtPathRadiance* dOut
     // a kernel-1-style loop traces one segment even with a negative bound, where the reference's loop (HL:484) traces none
     if (c->P.MaxBounceCount < 0 || c->P.MaxBounceCount > 200) return fail(c, RT_E_STATE, "rtTracePaths: MaxBounceCount must be 0 .. 200 (as rtDispatch)");
     int rc = prepareQueryScene(c, "rtTracePaths"); if (rc != RT_OK) return rc;
-    DevParams P = c->P;
-    bindScene(c, P);
-    P.countStats = c->optCountStats;
-    P.smemPairs = 0;                                 // no tree-top staging: every record from global memory
-    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    const DevParams P = queryParams(c);
     PathParams Q = {};
     Q.rays = dRays; Q.out = dOut; Q.n = (unsigned int)n; Q.samples = samples;
-    for (int a = 0; a < 3; a++)
-    {
-        Q.modelLo[a] = c->repack.modelBoundLo[a]; Q.modelHi[a] = c->repack.modelBoundHi[a];
-        Q.sphLo[a] = c->repack.sphBoundLo[a]; Q.sphHi[a] = c->repack.sphBoundHi[a];
-    }
+    sceneBounds(c, Q.modelLo, Q.modelHi, Q.sphLo, Q.sphHi);
     cudaError_t e = paths_launch(P, Q, c->numSMs, c->stream);
     if (e != cudaSuccess) return failCuda(c, e, "rtTracePaths launch");
     return RT_OK;
@@ -1424,28 +1385,24 @@ int rtDispatchFeatures(RtContext* c, int gx, int gy, int gz)
 {
     if (!c) return RT_E_INVALID;
     if (gx < 0 || gy < 0 || gz < 0) return fail(c, RT_E_INVALID, "rtDispatchFeatures: bad argument");
-    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDispatchFeatures: not available on a group context (rtCreateMulti)");
-    int rc = cameraImage(c, "rtDispatchFeatures"); if (rc != RT_OK) return rc;
+    int rc = refuseGroup(c, "rtDispatchFeatures"); if (rc != RT_OK) return rc;
+    if ((rc = cameraImage(c, "rtDispatchFeatures")) != RT_OK) return rc;
     CK(cudaSetDevice(c->device));
     const unsigned W = c->P.W, H = c->P.H;
     if (!c->featureFrame.p)                                    // the first call allocates the three images, zero-filled
     {
         const size_t n = (size_t)W * H;
-        CK(c->featureFrame.ensure(n)); CK(c->accumAlbedo.ensure(n)); CK(c->accumNormal.ensure(n));
-        CK(cudaMemsetAsync(c->featureFrame.p, 0, n * sizeof(RtPixelFeatures), c->stream));
-        CK(cudaMemsetAsync(c->accumAlbedo.p, 0, n * 16, c->stream));
-        CK(cudaMemsetAsync(c->accumNormal.p, 0, n * 16, c->stream));
+        if ((rc = allocateZeroed(c, c->featureFrame, n)) != RT_OK || (rc = allocateZeroed(c, c->accumAlbedo, n)) != RT_OK ||
+            (rc = allocateZeroed(c, c->accumNormal, n)) != RT_OK) return rc;
     }
-    unsigned limX = (unsigned long long)gx * 8ull < W ? (unsigned)gx * 8u : W;
-    unsigned limY = (unsigned long long)gy * 8ull < H ? (unsigned)gy * 8u : H;
-    if (gz == 0 || limX == 0 || limY == 0) return RT_OK;
+    unsigned limX, limY;
+    groupLimits(gx, gy, gz, W, H, limX, limY);
+    if (limX == 0 || limY == 0) return RT_OK;
     if ((rc = prepareQueryScene(c, "rtDispatchFeatures")) != RT_OK) return rc;
-    DevParams P = c->P;
-    bindScene(c, P);
+    DevParams P = queryParams(c);
     P.limX = limX; P.limY = limY;
-    P.tileRank = c->tileRank; P.tileWorld = c->tileWorld; P.bandRows = c->bandRows; P.countStats = c->optCountStats;
-    P.smemPairs = 0; P.zeroDefocus = 0;                        // no tree-top staging: every record from global memory
-    P.FrameRender = P.AccumulatedRender = nullptr; P.pixelStats = nullptr; P.nPeers = 0;
+    P.tileRank = c->tileRank; P.tileWorld = c->tileWorld; P.bandRows = c->bandRows;
+    P.zeroDefocus = 0;
     FeatureParams F = {};
     F.features = c->featureFrame.p; F.accumAlbedo = c->accumAlbedo.p; F.accumNormal = c->accumNormal.p;
     cudaError_t e = features_launch(P, F, c->numSMs, c->stream);
@@ -1456,9 +1413,9 @@ int rtDispatchFeatures(RtContext* c, int gx, int gy, int gz)
 // What both forms of rtCameraRays check before anything is allocated or launched
 static int cameraRaysArgs(RtContext* c, const char* what, const void* rays, size_t bytes)
 {
-    if (c->leader) return fail(c, RT_E_STATE, std::string(what) + ": this context belongs to a group; call it on the context rtCreateMulti returned");
+    int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
     if (!rays) return fail(c, RT_E_INVALID, std::string(what) + ": rays is NULL");
-    int rc = cameraImage(c, what); if (rc != RT_OK) return rc;
+    if ((rc = cameraImage(c, what)) != RT_OK) return rc;
     if (bytes != (size_t)c->width * c->height * sizeof(RtPathRay)) return fail(c, RT_E_INVALID, std::string(what) + ": bytes must equal W*H*28");
     return RT_OK;
 }
@@ -1501,6 +1458,17 @@ int rtCameraRaysDevice(RtContext* c, void* dRays, size_t bytes)
 // ---- the a-trous denoiser (rtDenoise, rt_kernel_denoise.cuh) --------------------------------------------------------------------------
 static bool finiteAbove0(float v) { return v > 0.0f && v < INFINITY; }
 
+// The passes of the a-trous filter: pass k reads the image pass k - 1 wrote, 2^k pixels apart, with the colour weight cK0 * 4^k
+static void passSchedule(int iterations, float cK0, DenoisePass* passes)
+{
+    for (int k = 0; k < iterations; k++)
+    {
+        passes[k].cK = cK0 * (float)(1u << (2 * k));
+        passes[k].rd1 = 1.0f / (float)(1u << k); passes[k].rd2 = 1.0f / (float)(2u << k);
+        passes[k].step = 1 << k; passes[k].src = k & 1; passes[k].last = k == iterations - 1;
+    }
+}
+
 int rtDenoise(RtContext* c, int useAccumulated, int iterations, float sigmaColour, float sigmaNormal, float sigmaDepth)
 {
     if (!c) return RT_E_INVALID;
@@ -1510,16 +1478,11 @@ int rtDenoise(RtContext* c, int useAccumulated, int iterations, float sigmaColou
     // the constants of include/rt_b200.h, one binary32 operation each
     const float invC = 1.0f / (sigmaColour * sigmaColour), invN = 1.0f / (sigmaNormal * sigmaNormal), invZ = 1.0f / sigmaDepth;
     DenoisePass passes[RT_DENOISE_MAX_ITERATIONS];
-    for (int k = 0; k < iterations; k++)
-    {
-        passes[k].cK = invC * (float)(1u << (2 * k));
-        passes[k].rd1 = 1.0f / (float)(1u << k); passes[k].rd2 = 1.0f / (float)(2u << k);
-        passes[k].step = 1 << k; passes[k].src = k & 1; passes[k].last = k == iterations - 1;
-    }
+    passSchedule(iterations, invC, passes);
     if (!(passes[iterations - 1].cK < INFINITY) || !(invN < INFINITY) || !(invZ < INFINITY))
         return fail(c, RT_E_INVALID, "rtDenoise: a sigma too small: invC * 4^(iterations-1), 1 / sigmaNormal^2 or 1 / sigmaDepth is not finite");
-    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDenoise: not available on a group context (rtCreateMulti)");
-    int rc = cameraImage(c, "rtDenoise"); if (rc != RT_OK) return rc;
+    int rc = refuseGroup(c, "rtDenoise"); if (rc != RT_OK) return rc;
+    if ((rc = cameraImage(c, "rtDenoise")) != RT_OK) return rc;
     if (!c->featureFrame.p) return fail(c, RT_E_STATE, "rtDenoise: no rtDispatchFeatures yet");
     if (c->tileWorld > 1) return fail(c, RT_E_STATE, "rtDenoise: the images of a context with rtSetTile world > 1 hold its own bands only");
     CK(cudaSetDevice(c->device));
@@ -1565,8 +1528,8 @@ int rtDenoiseTemporal(RtContext* c, int iterations, float sigmaLuminance, float 
     const float invN = 1.0f / (sigmaNormal * sigmaNormal), invZ = 1.0f / sigmaDepth, invL = 1.0f / sigmaLuminance;
     if (!(invN < INFINITY) || !(invZ < INFINITY) || !(invL < INFINITY))
         return fail(c, RT_E_INVALID, "rtDenoiseTemporal: a sigma too small: 1 / sigmaNormal^2, 1 / sigmaDepth or 1 / sigmaLuminance is not finite");
-    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, "rtDenoiseTemporal: not available on a group context (rtCreateMulti)");
-    int rc = cameraImage(c, "rtDenoiseTemporal"); if (rc != RT_OK) return rc;
+    int rc = refuseGroup(c, "rtDenoiseTemporal"); if (rc != RT_OK) return rc;
+    if ((rc = cameraImage(c, "rtDenoiseTemporal")) != RT_OK) return rc;
     if (!c->featureFrame.p) return fail(c, RT_E_STATE, "rtDenoiseTemporal: no rtDispatchFeatures yet");
     if (c->tileWorld > 1) return fail(c, RT_E_STATE, "rtDenoiseTemporal: the images of a context with rtSetTile world > 1 hold its own bands only");
     CK(cudaSetDevice(c->device));
@@ -1574,12 +1537,7 @@ int rtDenoiseTemporal(RtContext* c, int iterations, float sigmaLuminance, float 
     if (!c->temporalHist.p) c->temporalHistory = false;
     CK(c->denoised.ensure(n)); CK(c->denoiseScratch.ensure(3 * n)); CK(c->temporalFrame.ensure(n)); CK(c->temporalHist.ensure(6 * n));
     DenoisePass passes[RT_DENOISE_MAX_ITERATIONS];
-    for (int k = 0; k < iterations; k++)
-    {
-        passes[k].cK = 0.0f;
-        passes[k].rd1 = 1.0f / (float)(1u << k); passes[k].rd2 = 1.0f / (float)(2u << k);
-        passes[k].step = 1 << k; passes[k].src = k & 1; passes[k].last = k == iterations - 1;
-    }
+    passSchedule(iterations, 0.0f, passes);                                        // no colour weight: the variance guides instead
     const int cur = c->temporalSet ^ 1;
     float4* const set[2] = {c->temporalHist.p, c->temporalHist.p + 3 * n};       // guide, moments, colour history
     TemporalParams T = {};
@@ -1618,16 +1576,8 @@ int rtDisplayDenoised(RtContext* c, uint8_t* dst, size_t bytes)
 {
     if (!c || !dst) return fail(c, RT_E_INVALID, "rtDisplayDenoised: bad argument");
     if (!c->denoised.p) return fail(c, RT_E_STATE, "rtDisplayDenoised: no rtDenoise yet");
-    const size_t n = (size_t)c->width * c->height;
-    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplayDenoised: bytes must equal W*H*4");
-    CK(cudaSetDevice(c->device));
-    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }
-    CK(c->display.ensure(n));
-    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_display, c->denoised.p, c->display.p, n, 1.0f);      // t / 1 is exact
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    if (bytes != (size_t)c->width * c->height * 4) return fail(c, RT_E_INVALID, "rtDisplayDenoised: bytes must equal W*H*4");
+    return displayTo(c, [&](size_t n) { encodeDisplay(c, c->denoised.p, n, 1.0f); return RT_OK; }, dst, bytes);      // t / 1 is exact
 }
 
 int rtExchangeTiles(RtContext* c)
@@ -1636,9 +1586,7 @@ int rtExchangeTiles(RtContext* c)
     if (c->leader) return fail(c, RT_E_STATE, "rtExchangeTiles: call it on the context rtCreateMulti returned");
     if (c->tileWorld <= 1) return RT_OK;
     if (!c->comm && c->followers.empty()) return fail(c, RT_E_STATE, "rtExchangeTiles: no communicator (rtCommInit / rtCreateMulti)");
-    std::vector<RtContext*> all(1, c);
-    all.insert(all.end(), c->followers.begin(), c->followers.end());
-    return exchangeTiles(all.data(), (int)all.size());
+    return exchangeGroup(c);
 }
 
 int rtGetUniqueId(void* id, size_t bytes)
@@ -1737,45 +1685,19 @@ int rtCreateMulti(RtContext** out, const int* devices, int nDevices)
 int rtGetDevicePointer(RtContext* c, const char* name, void** devPtr, size_t* bytes)
 {
     if (!c || !name || !devPtr || !bytes) return fail(c, RT_E_INVALID, "rtGetDevicePointer: bad argument");
-    const std::string n(name);
     CK(cudaSetDevice(c->device));
-    if (n == "FrameRender") { *devPtr = c->frame.p; *bytes = c->frame.count * 16; }
-    else if (n == "AccumulatedRender") { *devPtr = c->accum.p; *bytes = c->accum.count * 16; }
-    else if (n == "PixelStats")
+    if (const NamedImage* img = findImage(name))
     {
-        if (!c->pixelStats.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: PixelStats is allocated by the first counting dispatch");
-        *devPtr = c->pixelStats.p; *bytes = c->pixelStats.count * sizeof(RtPixelStats);
+        int rc = imageReady(c, *img, "rtGetDevicePointer"); if (rc != RT_OK) return rc;
+        *devPtr = img->buf.p(c); *bytes = img->buf.count(c) * img->buf.element;
+        return RT_OK;
     }
-    else if (n == "FeatureFrame" || n == "AccumulatedAlbedo" || n == "AccumulatedNormal")
-    {
-        int rc = featuresReady(c, "rtGetDevicePointer"); if (rc != RT_OK) return rc;
-        if (n == "FeatureFrame") { *devPtr = c->featureFrame.p; *bytes = c->featureFrame.count * sizeof(RtPixelFeatures); }
-        else if (n == "AccumulatedAlbedo") { *devPtr = c->accumAlbedo.p; *bytes = c->accumAlbedo.count * 16; }
-        else { *devPtr = c->accumNormal.p; *bytes = c->accumNormal.count * 16; }
-    }
-    else if (n == "DenoisedRender")
-    {
-        if (!c->denoised.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: DenoisedRender is allocated by the first rtDenoise");
-        *devPtr = c->denoised.p; *bytes = c->denoised.count * 16;
-    }
-    else if (n == "TemporalFrame")
-    {
-        if (!c->temporalFrame.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: TemporalFrame is allocated by the first rtDenoiseTemporal");
-        *devPtr = c->temporalFrame.p; *bytes = c->temporalFrame.count * 16;
-    }
-    else if (n == "AdaptiveMoments")
-    {
-        if (!c->moments.p) return fail(c, RT_E_STATE, "rtGetDevicePointer: AdaptiveMoments is allocated by the first rtDispatchAdaptive");
-        *devPtr = c->moments.p; *bytes = c->moments.count * 16;
-    }
-    else if (n == "TileSend" || n == "TileRecv")
-    {
-        int rc = ensureTileBuffers(c); if (rc != RT_OK) return rc;
-        if (n == "TileSend") { *devPtr = c->tileSend.p; *bytes = c->tileSend.count * 16; }
-        else { *devPtr = c->tileRecv.p; *bytes = c->tileRecv.count * 16; }
-    }
-    else return fail(c, RT_E_UNKNOWN_NAME, std::string("rtGetDevicePointer: unknown object ") + name);
-    if (!*devPtr) return fail(c, RT_E_STATE, "rtGetDevicePointer: object not allocated yet (call rtResize)");
+    // the tile staging buffers follow the tile pattern (rtSetTile), not the image alone
+    const std::string n(name);
+    if (n != "TileSend" && n != "TileRecv") return fail(c, RT_E_UNKNOWN_NAME, std::string("rtGetDevicePointer: unknown object ") + name);
+    int rc = ensureTileBuffers(c); if (rc != RT_OK) return rc;
+    const DevBuf<float4>& b = n == "TileSend" ? c->tileSend : c->tileRecv;
+    *devPtr = b.p; *bytes = b.count * 16;
     return RT_OK;
 }
 
@@ -2100,9 +2022,8 @@ static int one_rtGetStats(RtContext* c, RtStats* out)
 static int one_rtResetStats(RtContext* c);
 int rtResetStats(RtContext* c)
 {
-    int rc = one_rtResetStats(c);
+    int rc = forGroup(c, one_rtResetStats);
     if (rc != RT_OK || !c) return rc;
-    for (RtContext* m : c->followers) if ((rc = one_rtResetStats(m)) != RT_OK) return fail(c, rc, m->err);
     if (!c->followers.empty()) CK(cudaSetDevice(c->device));
     return RT_OK;
 }
@@ -2121,7 +2042,7 @@ static int one_rtResetStats(RtContext* c)
 // ---- per-pixel counters ("PixelStats") ----------------------------------------------------------------------------------------
 static int pixelStatsReady(RtContext* c, const char* what)
 {
-    if (c->leader || !c->followers.empty()) return fail(c, RT_E_STATE, std::string(what) + ": not available on a group context (rtCreateMulti)");
+    int rc = refuseGroup(c, what); if (rc != RT_OK) return rc;
     if (!c->pixelStats.p) return fail(c, RT_E_STATE, std::string(what) + ": no counting dispatch yet (rtSetOption(\"countStats\", 1))");
     return RT_OK;
 }
@@ -2143,16 +2064,12 @@ int rtDisplayPixelStats(RtContext* c, int visMode, float debugVisScale, uint8_t*
     if (visMode < 1 || visMode > 4) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: visMode must be 1 (box tests), 2 (triangle tests), 3 (sphere tests) or 4 (rays)");
     if (!std::isfinite(debugVisScale) || !(debugVisScale > 0.0f)) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: debugVisScale must be finite and > 0");
     int rc = pixelStatsReady(c, "rtDisplayPixelStats"); if (rc != RT_OK) return rc;
-    const size_t n = c->pixelStats.count;
-    if (bytes != n * 4) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: bytes must equal W*H*4");
-    CK(cudaSetDevice(c->device));
-    if (c->copyPending) { CK(cudaEventSynchronize(c->copyDone)); c->copyPending = false; }     // rtDisplayAsync may still read the buffer
-    CK(c->display.ensure(n));
-    RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_pixel_stats_display, c->pixelStats.p, c->display.p, n, visMode, debugVisScale);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, c->display.p, bytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    if (bytes != c->pixelStats.count * 4) return fail(c, RT_E_INVALID, "rtDisplayPixelStats: bytes must equal W*H*4");
+    return displayTo(c, [&](size_t n)
+    {
+        RT_LAUNCH((unsigned)((n + 255) / 256), 256, 0, c->stream, k_pixel_stats_display, c->pixelStats.p, c->display.p, n, visMode, debugVisScale);
+        return RT_OK;
+    }, dst, bytes);
 }
 
 } // extern "C"
