@@ -511,12 +511,17 @@ int rtBuildBVH(RtContext* ctx, const float* verts, int vertCount, const int* ind
  *   "kernel"      0 = reference-shaped per-pixel megakernel, 1 = persistent threads (one path per lane),
  *                 2 = persistent-thread wavefront with per-warp path pools, sorting and ray compaction,
  *                 -1 = automatic (default): 2 when the scene has meshes, 1 for sphere-only scenes and for tiles so small that
- *                 a pool slot gets about one pixel (below 1.5 pixels per slot; 2.5 with NumRaysPerPixel = 1: multi-GPU tiles)
+ *                 a pool slot gets about one pixel (below 1.5 pixels per slot; 2.5 with NumRaysPerPixel = 1: multi-GPU tiles),
+ *                 and 1 whenever NumRaysPerPixel > RT_MAX_BATCH_SAMPLES.  Kernel 2 counts a pixel's samples in a 20-bit field, so
+ *                 rtDispatch / rtDispatchAdaptive with "kernel" = 2 and NumRaysPerPixel > RT_MAX_BATCH_SAMPLES are refused
+ *                 (RT_E_STATE, nothing changed); kernels 0 and 1 take any NumRaysPerPixel up to 2^31 - 1, like the reference
  *   "countStats"  1 = also count box / triangle tests (HL:254,271) — slower, off by default
  *   "sampleChunks"  kernel 1: a pixel's NumRaysPerPixel samples as this many consecutive jobs, the RNG state and the running sum
  *                 handed from the lane that finishes a chunk to the lane that takes the next (same samples in the same order:
  *                 same bits).  -1 (default) = automatic: mesh scenes on small tiles only (more than one and fewer than four
- *                 pixels per resident lane: multi-GPU tiles), about eight chunk-rounds per launch; 0 / 1 = whole pixels; 2..64 forced
+ *                 pixels per resident lane: multi-GPU tiles), about eight chunk-rounds per launch; 0 / 1 = whole pixels; 2..64 forced.
+ *                 A forced value is an upper bound: kernel 1 counts at most 2^31 chunk jobs ((8x4-pixel tiles x 32) x chunks), so large
+ *                 images get fewer chunks (whole pixels when fewer than two fit: 8192 x 8192 takes at most 32).  Same bits either way
  *   "exchange"    1 (default) = rtDispatch(RAYTRACE) on a context with a communicator (rtCommInit / rtCreateMulti) ends with the
  *                 all-gather of the frame's tiles; 0 = the caller exchanges (rtExchangeTiles or its own collective)
  *   "smemNodes"   number of top-of-tree node pairs staged in shared memory by TMA bulk copy (0 = off; -1 = automatic, which

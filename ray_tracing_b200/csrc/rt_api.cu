@@ -585,6 +585,7 @@ static int effectiveKernel(const RtContext* c)
     if (c->P.modelCount <= 0) return 1;
     const double slots = (double)c->numSMs * POOL_WARPS * 64.0;
     const long long chain = (long long)c->P.NumRaysPerPixel * c->dispatchFrames;      // samples one slot runs for a pixel
+    if (chain > RT_MAX_BATCH_SAMPLES) return 1;          // the pooled kernel's slot counts a pixel's samples in 20 bits (info_pack); kernel 1 in an int
     const double threshold = chain <= 1 ? RT_SMALL_TILE_PIXELS_PER_SLOT_1SPP : RT_SMALL_TILE_PIXELS_PER_SLOT;
     if (c->dispatchPixels > 0 && (double)c->dispatchPixels < threshold * slots) return 1;
     return 2;
@@ -821,6 +822,8 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     if (c->P.NumRaysPerPixel < 0) return fail(c, RT_E_STATE, "rtDispatch: NumRaysPerPixel is negative");
     if (c->P.MaxBounceCount > 200 || W > 65535u || H > 65535u) return fail(c, RT_E_STATE, "rtDispatch: MaxBounceCount > 200 or a resolution above 65535 is not supported");
     if (c->P.MaxBounceCount < 0) return fail(c, RT_E_STATE, "rtDispatch: MaxBounceCount is negative (the reference clamps it to [0, 32], RCM:15)");
+    if (c->optKernel == 2 && c->P.NumRaysPerPixel > RT_MAX_BATCH_SAMPLES)
+        return fail(c, RT_E_STATE, "rtDispatch: \"kernel\" = 2 counts a pixel's samples in 20 bits: NumRaysPerPixel above RT_MAX_BATCH_SAMPLES needs kernel 0 or 1");
 
     c->dispatchPixels = (unsigned long long)ownedRows(limY, c->bandRows, c->tileWorld, c->tileRank) * limX;
     c->dispatchFrames = frames;
@@ -871,10 +874,18 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     // (kernel 1 only: in the pooled kernel the same hand-off was slower than whole pixels on small tiles and was taken out again)
     P.chunks = kernel == 1 ? wave_chunks(c->optSampleChunks, c->numSMs, c->dispatchPixels, P.NumRaysPerPixel, P.modelCount) : 1;
     if (c->dispatchPixels == 0 || frames > 1 || ad) P.chunks = 1;      // a rank whose tile is empty (an image lower than the band pattern); a batch of frames or a pixel list runs whole pixels
+    const unsigned long long rows = limX ? c->dispatchPixels / limX : 0;
+    const size_t jobs = (size_t)((limX + 7u) / 8u) * (size_t)((rows + 3ull) / 4ull) * 32u;
     if (P.chunks > 1)
     {
-        unsigned long long rows = limX ? c->dispatchPixels / limX : 0;
-        const size_t jobs = (size_t)((limX + 7u) / 8u) * (size_t)((rows + 3ull) / 4ull) * 32u;
+        // kernel 1 counts its chunk jobs (jobs x chunks) in a 32-bit work counter that every resident lane draws from once more after
+        // the last job: at most 2^31 chunk jobs leave 2^31 of headroom for those draws.  Fewer chunks on large images (chunks are
+        // schedule only), whole pixels when fewer than two fit
+        const unsigned long long fit = (1ull << 31) / jobs;
+        if ((unsigned long long)P.chunks > fit) P.chunks = fit < 2ull ? 1 : (int)fit;
+    }
+    if (P.chunks > 1)
+    {
         // four self-validating 64-bit words per pixel job; the tag carries a serial number of the dispatch, so nothing has to be cleared
         // between frames (only a fresh allocation and the wrap of the 24-bit serial zero the buffer: tag 0 is never expected)
         const size_t before = c->handoff.count;

@@ -137,6 +137,37 @@ int rtCameraRays(RtContext* c, RtPathRay* rays, size_t bytes)
 
 int rtCameraRaysDevice(RtContext* c, void*, size_t) { return c ? fail(c, RT_E_STATE, "oracle: no device memory") : RT_E_INVALID; }
 
+/* Test hook beside orRenderPixels: out = n RtPixelFeatures, the FeatureFrame record of each listed pixel (xy = n pairs of global pixel
+ * coordinates) for the context's current uniforms; the feature images are not touched.  Exact, because a pixel's feature ray depends on
+ * its own coordinates and seed only.  Multi-threaded; the counts go to RtStats as rtDispatchFeatures's do. */
+int orFeaturePixels(RtContext* c, const int* xy, int n, RtPixelFeatures* out)
+{
+    if (!c) return RT_E_INVALID;
+    if (!xy || !out || n < 0) return fail(c, RT_E_INVALID, "orFeaturePixels: bad argument");
+    int rc = cameraImage(c, "orFeaturePixels"); if (rc != RT_OK) return rc;
+    if ((rc = traceChecks(c, "orFeaturePixels", c, c, 1, 0)) != RT_OK) return rc;
+    std::atomic<int> next(0);
+    std::vector<Shader> shaders(c->threads, c->sh);
+    std::vector<std::thread> pool;
+    for (int t = 0; t < c->threads; t++)
+    {
+        pool.emplace_back([&, t]() {
+            Shader& s = shaders[t];
+            bind_buffers(c, s);
+            Shader w = s;
+            for (;;)
+            {
+                const int i0 = next.fetch_add(64);
+                if (i0 >= n) break;
+                for (int i = i0; i < n && i < i0 + 64; i++) out[i] = pixelFeatures(c, s, w, xy[2 * i], xy[2 * i + 1]);
+            }
+        });
+    }
+    for (auto& th : pool) th.join();
+    for (auto& s : shaders) { c->stats.rays += s.nRays; c->stats.boxTests += s.nBox; c->stats.triTests += s.nTri; c->stats.sphereTests += s.nSphere; }
+    return RT_OK;
+}
+
 /* ---- the four wrapped entry points: defined under a name of their own, exported under the ABI's ------------------------------------ */
 int orFeatures_rtDestroy(RtContext* c) __asm__("rtDestroy");
 int orFeatures_rtResize(RtContext* c, int w, int h) __asm__("rtResize");
