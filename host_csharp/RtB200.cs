@@ -75,6 +75,14 @@ public static class RtB200
     public struct PathRadiance { public UnityEngine.Vector3 rgb; public uint rngState; }
     [DllImport(Lib)] public static extern int rtTracePaths(IntPtr ctx, PathRay[] rays, int n, int samples, [Out] PathRadiance[] output);
     [DllImport(Lib)] public static extern int rtTracePathsDevice(IntPtr ctx, IntPtr dRays, IntPtr dOut, int n, int samples);
+    // light probes: the radiance arriving at each position from `samples` spherical Fibonacci directions (the same for every probe), path
+    // traced with state H(H(seed + p) + k) and projected onto the real L2 spherical harmonics.  sh[ch * 9 + i]: channel r, g, b, coefficient
+    // i in Unity's SphericalHarmonicsL2 order, before its shader-constant conversion; rejected = samples left out for a non-finite radiance.
+    // positions: 3 floats per probe (UnityEngine.Vector3[] marshals as such)
+    [StructLayout(LayoutKind.Sequential)]
+    public struct ProbeSH { [MarshalAs(UnmanagedType.ByValArray, SizeConst = 27)] public float[] sh; public uint rejected; }
+    [DllImport(Lib)] public static extern int rtBakeProbes(IntPtr ctx, UnityEngine.Vector3[] positions, int n, int samples, uint seed, [Out] ProbeSH[] output);
+    [DllImport(Lib)] public static extern int rtBakeProbesDevice(IntPtr ctx, IntPtr dPositions, IntPtr dOut, int n, int samples, uint seed);
     // one pixel of "FeatureFrame": object = ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1 (dst = +inf, the rest 0)
     [StructLayout(LayoutKind.Sequential)]
     public struct PixelFeatures { public UnityEngine.Vector3 albedo; public float dst; public UnityEngine.Vector3 normal; public int objectId; }

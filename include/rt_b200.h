@@ -188,6 +188,44 @@ int rtTraceOcclusionDevice(RtContext* ctx, const void* dSegs, void* dOccluded, i
 int rtTracePaths(RtContext* ctx, const RtPathRay* rays, int n, int samples, RtPathRadiance* out);
 int rtTracePathsDevice(RtContext* ctx, const void* dRays, void* dOut, int n, int samples);
 
+/* Extension: light-probe baking.  For each of n probe positions, the path tracer's radiance arriving from S = samples directions,
+ * projected onto the real L2 spherical harmonics (Unity's SphericalHarmonicsL2 before its shader-constant conversion; DESIGN.md
+ * section 7d''''''''' gives the constants of that conversion and of the cosine-lobe convolution, which belong to the host).  Every
+ * bit is stated; each operation is one IEEE binary32 operation in the order written (no contraction).
+ *   - Directions: a spherical Fibonacci set, the same for every probe, with no RNG draw.  For sample k = 0 .. S-1:
+ *         t = (float)(uint32_t)(k * 2654435769u) * 2^-32          (RandomValue's conversion, HL:137)
+ *         phi = t * 6.28318548f;  (s, c) = (sin phi, cos phi) as RandomPointInCircle computes them (rt_devmath.cuh sincos_rt)
+ *         z = 1 - (float)(2k + 1) / (float)S;  r = sqrt(max(1 - z * z, 0));  d_k = (r * c, r * s, z), used as given
+ *   - Paths: with H(x) the value NextRandom (HL:127-133) returns from state x and p the probe's index in the call,
+ *         L_pk = Trace(CreateRay(positions[p], d_k, 1, 0), state = H(H(seed + p) + k))        (HL:439-448, HL:479-542)
+ *     so L_pk is rtTracePaths({positions[p], d_k, H(H(seed + p) + k)}, samples = 1).rgb bit for bit.
+ *   - Basis at d = (x, y, z):  Y0 = 0.282094792;  Y1 = 0.488602512 * y;  Y2 = 0.488602512 * z;  Y3 = 0.488602512 * x;
+ *         Y4 = 1.09254843 * (x * y);  Y5 = 1.09254843 * (y * z);  Y6 = 0.315391565 * ((3 * (z * z)) - 1);
+ *         Y7 = 1.09254843 * (x * z);  Y8 = 0.546274215 * ((x * x) - (y * y))
+ *   - Sums: the samples fall into chunks of RT_PROBE_CHUNK consecutive k.  A chunk's 27 sums start at +0 and add L_pk.ch * Y_i(d_k)
+ *     in k order.  A sample with any non-finite component of L_pk adds nothing and counts in `rejected` (a NaN path does not
+ *     poison its probe).  The chunk sums are combined by the full binary tree that pairs adjacent chunks, the chunk count padded with
+ *     +0 chunks to the next power of two (within an aligned group of 32 chunks: a warp's xor 1 / 2 / 4 / 8 / 16 shuffle sum), and
+ *         out[p].sh[ch][i] = tree * (12.566371f / (float)S)
+ *   - Everything else is rtTracePaths': what it reads (the scene, "modelCount", "MaxBounceCount" and the sky / sun uniforms; no camera,
+ *     "Frame", "renderSeed", "NumRaysPerPixel" or "Resolution"; no rtResize needed), what it leaves alone (the images, PixelStats,
+ *     "Frame", RtStats.dispatches and kernelMs), RtStats.rays growing by segments and the countStats counters as there, the per-segment
+ *     gate of model skipping, the TLAS and the sphere accelerator, devices[0] on a group context.  Positions are not validated: a far or
+ *     NaN origin fails the gate and walks every model.
+ *   - Launches: a call runs its probes in launches of floor(RT_PROBE_SCRATCH_CHUNKS / ceil(S / RT_PROBE_CHUNK)) probes (the last one
+ *     partial), each through a device scratch of 112 bytes per chunk (at most RT_PROBE_SCRATCH_CHUNKS chunks: 112 MiB) that the context
+ *     keeps, grown on first use, freed by rtDestroy.  The launches change no bits: p is the index in the call.
+ * Refused: ctx NULL, n < 0, positions / out NULL with n > 0, samples < 1 or > RT_MAX_BATCH_SAMPLES, a device dPositions not 4-byte or
+ * dOut not 16-byte aligned -> RT_E_INVALID; a member context of a group other than the one rtCreateMulti returned, the scene checks of
+ * rtDispatch and "MaxBounceCount" outside 0 .. 200 -> RT_E_STATE.  n = 0 is RT_OK and launches nothing.
+ * rtBakeProbes: host arrays (positions n x 3 floats), through a launch's worth of device buffers the context keeps (12 + 112 bytes per
+ * probe; freed by rtDestroy); synchronises.  rtBakeProbesDevice: n x 3 floats and n RtProbeSH in device memory of the context's
+ * device; allocates only the scratch; asynchronous on the context's stream (rtSetStream). */
+#define RT_PROBE_CHUNK 32
+#define RT_PROBE_SCRATCH_CHUNKS (1 << 20)
+int rtBakeProbes(RtContext* ctx, const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out);
+int rtBakeProbesDevice(RtContext* ctx, const void* dPositions, void* dOut, int n, int samples, uint32_t seed);
+
 /* Extension: first-hit feature images for denoisers (albedo, shading normal, depth, object id: the guides OIDN, a-trous / SVGF filters
  * and mattes take next to the colour), and the camera's own rays.
  *

@@ -115,6 +115,13 @@ typedef struct RtPathRadiance {
     uint32_t rngState;     /* the state after the last sample: a caller continues the chain with it */
 } RtPathRadiance;
 
+/* One probe of rtBakeProbes / rtBakeProbesDevice (include/rt_b200.h): the radiance around a point projected onto the real L2
+ * spherical harmonics, Unity's SphericalHarmonicsL2 layout before its shader-constant conversion.  112 bytes. */
+typedef struct RtProbeSH {
+    float    sh[3][9];     /* [r, g, b][coefficient], coefficients ordered by l, then m = -l .. l (Unity's order) */
+    uint32_t rejected;     /* samples whose radiance was not finite and were left out of the sums */
+} RtProbeSH;
+
 /* One pixel of rtDispatchFeatures' "FeatureFrame" (include/rt_b200.h): what the pixel's feature ray hits first.  32 bytes. */
 typedef struct RtPixelFeatures {
     float   albedo[3];    /* (0, 0, 0) on a miss; (1, 1, 1) for glass; GetMaterialColour (HL:450-466) otherwise */
@@ -134,6 +141,7 @@ static_assert(sizeof(RtRaySegment) == 28, "RtRaySegment record");
 static_assert(sizeof(RtPathRay) == 28, "RtPathRay record");
 static_assert(sizeof(RtPathRadiance) == 16, "RtPathRadiance record");
 static_assert(sizeof(RtPixelFeatures) == 32, "RtPixelFeatures record");
+static_assert(sizeof(RtProbeSH) == 112, "RtProbeSH record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

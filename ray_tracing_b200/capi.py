@@ -119,6 +119,13 @@ def make_path_rays(origins, dirs=None, rng_state=None) -> np.ndarray:
     return rays
 
 
+# rtBakeProbes: one probe's L2 spherical harmonics (RtProbeSH)
+PROBE_SH_DTYPE = np.dtype([("sh", "<f4", (3, 9)), ("rejected", "<u4")])
+assert PROBE_SH_DTYPE.itemsize == 112
+RT_PROBE_CHUNK = 32
+RT_PROBE_SCRATCH_CHUNKS = 1 << 20
+
+
 # rtDispatchFeatures: one pixel of "FeatureFrame" (RtPixelFeatures).  object: ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1
 PIXEL_FEATURES_DTYPE = np.dtype([("albedo", "<f4", 3), ("dst", "<f4"), ("normal", "<f4", 3), ("object", "<i4")])
 assert PIXEL_FEATURES_DTYPE.itemsize == 32
@@ -213,6 +220,8 @@ class RtLib:
             "rtTraceOcclusionDevice": ([vp, vp, vp, ci, ci], ci),
             "rtTracePaths": ([vp, vp, ci, ci, vp], ci),
             "rtTracePathsDevice": ([vp, vp, vp, ci, ci], ci),
+            "rtBakeProbes": ([vp, vp, ci, ci, C.c_uint32, vp], ci),
+            "rtBakeProbesDevice": ([vp, vp, vp, ci, ci, C.c_uint32], ci),
             "rtDispatchFeatures": ([vp, ci, ci, ci], ci),
             "rtCameraRays": ([vp, vp, C.c_size_t], ci),
             "rtCameraRaysDevice": ([vp, vp, C.c_size_t], ci),
@@ -227,7 +236,7 @@ class RtLib:
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
                             "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
-                            "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
+                            "rtBakeProbes", "rtBakeProbesDevice", "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
                             "rtDispatchAdaptive", "rtDisplayMean"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
@@ -404,6 +413,21 @@ class RtContext:
         """rtTracePathsDevice: n RtPathRay at rays_ptr (4-byte aligned) -> n RtPathRadiance at out_ptr (16-byte aligned), both device
         memory of the context's GPU (e.g. torch CUDA tensors' data_ptr()).  Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtTracePathsDevice(self._h, C.c_void_p(rays_ptr), C.c_void_p(out_ptr), int(n), int(samples)))
+
+    def bake_probes(self, positions, samples: int, seed: int = 0):
+        """rtBakeProbes: the L2 spherical harmonics of the radiance arriving at every probe position ((n, 3) floats) from `samples`
+        spherical Fibonacci directions.  Returns (sh, rejected): (n, 3, 9) float32 as [probe][r, g, b][coefficient] in Unity's order,
+        and (n,) uint32, the samples left out for a non-finite radiance."""
+        pos = np.ascontiguousarray(np.asarray(positions, dtype=np.float32).reshape(-1, 3))
+        out = np.empty(pos.shape[0], dtype=PROBE_SH_DTYPE)
+        self._ck(self._L.rtBakeProbes(self._h, pos.ctypes.data if pos.size else None, int(pos.shape[0]), int(samples), int(seed) & 0xFFFFFFFF,
+                                      out.ctypes.data if out.size else None))
+        return out["sh"].copy(), out["rejected"].copy()
+
+    def bake_probes_device(self, positions_ptr: int, out_ptr: int, n: int, samples: int, seed: int = 0):
+        """rtBakeProbesDevice: n x 3 floats at positions_ptr (4-byte aligned) -> n RtProbeSH (PROBE_SH_DTYPE, 112 bytes) at out_ptr
+        (16-byte aligned), both device memory of the context's GPU.  Asynchronous on the context's stream (set_stream)."""
+        self._ck(self._L.rtBakeProbesDevice(self._h, C.c_void_p(positions_ptr), C.c_void_p(out_ptr), int(n), int(samples), int(seed) & 0xFFFFFFFF))
 
     def dispatch_features(self, gx: Optional[int] = None, gy: Optional[int] = None, gz: int = 1):
         """rtDispatchFeatures: the first-hit feature images (albedo, dst, normal, object id) of every pixel's own camera ray of the

@@ -14,6 +14,7 @@
 #include "rt_kernel_denoise.cuh"
 #include "rt_kernel_temporal.cuh"
 #include "rt_kernel_adaptive.cuh"
+#include "rt_kernel_probes.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -122,6 +123,8 @@ struct RtContext
     // rtDispatchAdaptive: "AdaptiveMoments" (W*H, allocated zero-filled by the first traced call), the pixel list (W*H), the selection's
     // scratch (a ballot word per 32 jobs, then the block counts and the list length) and the pinned word the length is read into
     DevBuf<float4> moments; DevBuf<unsigned int> adaptiveList, adaptiveScratch; unsigned int* adaptiveCount = nullptr;
+    // rtBakeProbes: the chunk records of one launch (both forms), and the host form's device copies of one launch's positions and results
+    DevBuf<float> probeScratch, probePositions; DevBuf<RtProbeSH> probeOut;
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -332,6 +335,7 @@ int rtDestroy(RtContext* c)
     c->queryRays.release(); c->queryHits.release(); c->cameraRays.release();
     c->denoiseScratch.release(); c->temporalHist.release();
     c->adaptiveList.release(); c->adaptiveScratch.release();
+    c->probeScratch.release(); c->probePositions.release(); c->probeOut.release();
     if (c->adaptiveCount) cudaFreeHost(c->adaptiveCount);
     c->repack.release();
     closePeers(c);
@@ -1380,6 +1384,75 @@ int rtTracePathsDevice(RtContext* c, const void* dRays, void* dOut, int n, int s
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     return pathsLocal(c, (const RtPathRay*)dRays, (RtPathRadiance*)dOut, n, samples);
+}
+
+// ---- light probes (rtBakeProbes, rt_kernel_probes.cuh) -------------------------------------------------------------------------------
+static int probeArgs(RtContext* c, const char* what, const void* positions, const void* out, int n, int samples)
+{
+    int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
+    if (n < 0 || (n > 0 && (!positions || !out))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or positions / out NULL)");
+    if (samples < 1 || samples > RT_MAX_BATCH_SAMPLES) return fail(c, RT_E_INVALID, std::string(what) + ": samples must be 1 .. RT_MAX_BATCH_SAMPLES");
+    return RT_OK;
+}
+
+// The probes of one launch: as many as RT_PROBE_SCRATCH_CHUNKS chunk records hold
+static int probesPerLaunch(int samples)
+{
+    return RT_PROBE_SCRATCH_CHUNKS / ((samples + (int)RT_PROBE_CHUNK - 1) / (int)RT_PROBE_CHUNK);
+}
+
+// n probes in device memory of this context's GPU, the first of them probe p0 of the call -> n RtProbeSH, in launches of at most
+// probesPerLaunch probes; asynchronous on the context's stream.  The scratch is allocated (or grown) here and nothing else is.
+static int probesLocal(RtContext* c, const float* dPositions, RtProbeSH* dOut, int n, int samples, uint32_t seed, unsigned int p0)
+{
+    if (c->P.MaxBounceCount < 0 || c->P.MaxBounceCount > 200) return fail(c, RT_E_STATE, "rtBakeProbes: MaxBounceCount must be 0 .. 200 (as rtDispatch)");
+    int rc = prepareQueryScene(c, "rtBakeProbes"); if (rc != RT_OK) return rc;
+    const unsigned int chunks = ((unsigned int)samples + RT_PROBE_CHUNK - 1) / RT_PROBE_CHUNK;
+    const int per = probesPerLaunch(samples);
+    const int first = n < per ? n : per;
+    if (c->probeScratch.cap < (size_t)first * chunks * PROBE_WORDS) CK(c->probeScratch.ensure((size_t)first * chunks * PROBE_WORDS));
+    const DevParams P = queryParams(c);
+    ProbeParams Q = {};
+    Q.scratch = c->probeScratch.p; Q.chunks = chunks; Q.samples = samples; Q.seed = seed;
+    sceneBounds(c, Q.modelLo, Q.modelHi, Q.sphLo, Q.sphHi);
+    for (int i0 = 0; i0 < n; i0 += per)
+    {
+        Q.positions = dPositions + 3 * (size_t)i0; Q.out = dOut + i0;
+        Q.n = (unsigned int)(n - i0 < per ? n - i0 : per); Q.p0 = p0 + (unsigned int)i0;
+        cudaError_t e = probes_launch(P, Q, c->numSMs, c->stream);
+        if (e != cudaSuccess) return failCuda(c, e, "rtBakeProbes launch");
+    }
+    return RT_OK;
+}
+
+int rtBakeProbes(RtContext* c, const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = probeArgs(c, "rtBakeProbes", positions, out, n, samples); if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    const int per = probesPerLaunch(samples);
+    const int chunk = n < per ? n : per;
+    if (c->probeOut.cap < (size_t)chunk) { CK(c->probePositions.ensure(3 * (size_t)chunk)); CK(c->probeOut.ensure((size_t)chunk)); }
+    for (int i0 = 0; i0 < n; i0 += chunk)
+    {
+        const int m = n - i0 < chunk ? n - i0 : chunk;
+        if ((rc = stagedH2D(c, c->probePositions.p, positions + 3 * (size_t)i0, (size_t)m * 3 * sizeof(float))) != RT_OK) return rc;
+        if ((rc = probesLocal(c, c->probePositions.p, c->probeOut.p, m, samples, seed, (unsigned int)i0)) != RT_OK) return rc;
+        if ((rc = stagedD2H(c, out + i0, c->probeOut.p, (size_t)m * sizeof(RtProbeSH))) != RT_OK) return rc;
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rtBakeProbesDevice(RtContext* c, const void* dPositions, void* dOut, int n, int samples, uint32_t seed)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = probeArgs(c, "rtBakeProbesDevice", dPositions, dOut, n, samples); if (rc != RT_OK) return rc;
+    if (((uintptr_t)dPositions & 3u) || ((uintptr_t)dOut & 15u)) return fail(c, RT_E_INVALID, "rtBakeProbesDevice: dPositions must be 4-byte and dOut 16-byte aligned");
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    return probesLocal(c, (const float*)dPositions, (RtProbeSH*)dOut, n, samples, seed, 0u);
 }
 
 // ---- first-hit feature images and the camera's own rays (rtDispatchFeatures, rtCameraRays, rt_kernel_features.cuh) ---------------------

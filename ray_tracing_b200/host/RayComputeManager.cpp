@@ -32,6 +32,7 @@ std::string RtApi::Load(const char* path)
     TraceRays = reinterpret_cast<decltype(TraceRays)>(dlsym(dl, "rtTraceRays"));
     TraceOcclusion = reinterpret_cast<decltype(TraceOcclusion)>(dlsym(dl, "rtTraceOcclusion"));
     TracePaths = reinterpret_cast<decltype(TracePaths)>(dlsym(dl, "rtTracePaths"));
+    BakeProbesFn = reinterpret_cast<decltype(BakeProbesFn)>(dlsym(dl, "rtBakeProbes"));
     DispatchFeatures = reinterpret_cast<decltype(DispatchFeatures)>(dlsym(dl, "rtDispatchFeatures"));
     CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
     DenoiseFn = reinterpret_cast<decltype(DenoiseFn)>(dlsym(dl, "rtDenoise"));
@@ -348,6 +349,16 @@ int RayComputeManager::TracePaths(const RtPathRay* rays, int n, int samples, RtP
     int rc;
     if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
     TRY(api.TracePaths(ctx, rays, n, samples, out));
+    return RT_OK;
+}
+
+int RayComputeManager::BakeProbes(const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.BakeProbesFn) { lastError = "the library does not export rtBakeProbes"; return RT_E_STATE; }
+    int rc;
+    if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
+    TRY(api.BakeProbesFn(ctx, positions, n, samples, seed, out));
     return RT_OK;
 }
 

@@ -60,6 +60,7 @@ struct RtApi
     decltype(&rtTraceRays) TraceRays = nullptr;             // optional: closest-hit queries (TraceRays / Pick)
     decltype(&rtTraceOcclusion) TraceOcclusion = nullptr;   // optional: occlusion queries (TraceOcclusion)
     decltype(&rtTracePaths) TracePaths = nullptr;           // optional: radiance along caller rays (TracePaths)
+    decltype(&rtBakeProbes) BakeProbesFn = nullptr;         // optional: light probes (BakeProbes)
     decltype(&rtDispatchFeatures) DispatchFeatures = nullptr;   // optional: first-hit feature images (RenderFeatures)
     decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
     decltype(&rtDenoise) DenoiseFn = nullptr;               // optional: the a-trous denoiser (Denoise)
@@ -149,6 +150,9 @@ public:
     // not in the reference: the path tracer's radiance along caller-supplied rays, the mean of `samples` paths on each ray's RNG chain
     // (rtTracePaths) — custom cameras, probe baking.  The scene is uploaded first as for TraceRays.
     int TracePaths(const RtPathRay* rays, int n, int samples, RtPathRadiance* out);
+    // not in the reference: light probes — the L2 spherical harmonics of the radiance arriving at each of n positions (n x 3 floats)
+    // from `samples` spherical Fibonacci directions (rtBakeProbes).  The scene is uploaded first as for TraceRays.
+    int BakeProbes(const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out);
     // not in the reference: the denoiser guides of the frame the NEXT RenderFrame() renders (rtDispatchFeatures over the whole image):
     // the upload sequence of RenderFrame, Frame = numAccumulatedFrames, and no step of the frame counter.  Call it right before that
     // RenderFrame; ResetAccumulatedRender resets the accumulated guides with the colour.

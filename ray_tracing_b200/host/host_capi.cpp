@@ -246,6 +246,9 @@ int rcmTraceOcclusion(void* hv, const RtRaySegment* segs, int n, uint8_t* occlud
 int rcmTracePaths(void* hv, const RtPathRay* rays, int n, int samples, RtPathRadiance* out)
 { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->TracePaths(rays, n, samples, out); } CATCH_ALL(h) }
 
+int rcmBakeProbes(void* hv, const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->BakeProbes(positions, n, samples, seed, out); } CATCH_ALL(h) }
+
 int rcmRenderFeatures(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFeatures(); } CATCH_ALL(h) }
 int rcmReadFeatureImage(void* hv, const char* name, void* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadFeatureImage(name, dst, bytes); }
 int rcmCameraRays(void* hv, RtPathRay* rays, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->CameraRays(rays, bytes); } CATCH_ALL(h) }

@@ -68,6 +68,7 @@ def host_lib() -> C.CDLL:
         L.rcmTraceRays.argtypes = [vp, vp, ci, vp, ci]
         L.rcmTraceOcclusion.argtypes = [vp, vp, ci, vp, ci]
         L.rcmTracePaths.argtypes = [vp, vp, ci, ci, vp]
+        L.rcmBakeProbes.argtypes = [vp, vp, ci, ci, C.c_uint32, vp]
         L.rcmRenderFeatures.argtypes = [vp]
         L.rcmReadFeatureImage.argtypes = [vp, cp, vp, C.c_size_t]
         L.rcmCameraRays.argtypes = [vp, vp, C.c_size_t]
@@ -341,6 +342,17 @@ class RayComputeManager:
         out = np.empty(r.shape[0], dtype=capi.PATH_RADIANCE_DTYPE)
         self._ck(self._L.rcmTracePaths(self._h, r.ctypes.data if r.size else None, int(r.shape[0]), int(samples), out.ctypes.data if out.size else None))
         return out
+
+    # -- light probes (rtBakeProbes): L2 spherical harmonics of the radiance at each position
+    def bake_probes(self, positions, samples: int, seed: int = 0):
+        """The L2 spherical harmonics of the radiance arriving at each probe position ((n, 3) floats) from `samples` spherical
+        Fibonacci directions: ((n, 3, 9) float32 [probe][r, g, b][coefficient], (n,) uint32 rejected samples).  The scene is uploaded
+        as a frame would upload it; the render textures are not touched."""
+        pos = np.ascontiguousarray(np.asarray(positions, dtype=np.float32).reshape(-1, 3))
+        out = np.empty(pos.shape[0], dtype=capi.PROBE_SH_DTYPE)
+        self._ck(self._L.rcmBakeProbes(self._h, pos.ctypes.data if pos.size else None, int(pos.shape[0]), int(samples), int(seed) & 0xFFFFFFFF,
+                                       out.ctypes.data if out.size else None))
+        return out["sh"].copy(), out["rejected"].copy()
 
     # -- denoiser guides (rtDispatchFeatures) and the camera's own rays (rtCameraRays)
     def RenderFeatures(self):
