@@ -758,14 +758,16 @@ static DevParams queryParams(const RtContext* c)
     return P;
 }
 
-// The boxes the models' and the spheres' padding was computed for (QueryParams, PathParams)
-static void sceneBounds(const RtContext* c, float modelLo[3], float modelHi[3], float sphLo[3], float sphHi[3])
+// The boxes the models' and the spheres' padding was computed for (QueryParams, PathParams, ProbeParams)
+static OriginBox sceneBounds(const RtContext* c)
 {
+    OriginBox b;
     for (int a = 0; a < 3; a++)
     {
-        modelLo[a] = c->repack.modelBoundLo[a]; modelHi[a] = c->repack.modelBoundHi[a];
-        sphLo[a] = c->repack.sphBoundLo[a]; sphHi[a] = c->repack.sphBoundHi[a];
+        b.modelLo[a] = c->repack.modelBoundLo[a]; b.modelHi[a] = c->repack.modelBoundHi[a];
+        b.sphLo[a] = c->repack.sphBoundLo[a]; b.sphHi[a] = c->repack.sphBoundHi[a];
     }
+    return b;
 }
 
 // The pixels groups of 8 x 8 cover: limX x limY, none when gz = 0
@@ -1222,6 +1224,26 @@ int rtDisplayMean(RtContext* c, uint8_t* dst, size_t bytes)
 static int stagedH2D(RtContext* c, void* dst, const void* src, size_t bytes);
 static int stagedD2H(RtContext* c, void* dst, const void* src, size_t bytes);
 
+// The host form of a batch call: n records in batches of `chunk` through the device buffers dIn and dOut — each batch copied in
+// (inBytes per record), run by local(i0, m) on records i0 .. i0 + m - 1 and copied out (outBytes per record) — then one synchronise
+extern "C++" {
+template <class Local>
+static int hostBatches(RtContext* c, int n, int chunk, void* dIn, const void* in, size_t inBytes, const void* dOut, void* out, size_t outBytes,
+                       Local local)
+{
+    int rc;
+    for (int i0 = 0; i0 < n; i0 += chunk)
+    {
+        const int m = n - i0 < chunk ? n - i0 : chunk;
+        if ((rc = stagedH2D(c, dIn, static_cast<const char*>(in) + (size_t)i0 * inBytes, (size_t)m * inBytes)) != RT_OK) return rc;
+        if ((rc = local(i0, m)) != RT_OK) return rc;
+        if ((rc = stagedD2H(c, static_cast<char*>(out) + (size_t)i0 * outBytes, dOut, (size_t)m * outBytes)) != RT_OK) return rc;
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+} // extern "C++"
+
 static int traceArgs(RtContext* c, const char* what, const void* rays, const void* hits, int n, int flags)
 {
     int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
@@ -1238,7 +1260,7 @@ static int queryLocal(RtContext* c, const char* what, QueryParams& Q, int n, int
     int rc = prepareQueryScene(c, what); if (rc != RT_OK) return rc;
     const DevParams P = queryParams(c);
     Q.n = (unsigned int)n; Q.noCull = flags & RT_TRACE_NO_CULL;
-    sceneBounds(c, Q.modelLo, Q.modelHi, Q.sphLo, Q.sphHi);
+    Q.box = sceneBounds(c);
     cudaError_t e = occlusion ? query_launch<true>(P, Q, c->numSMs, c->stream) : query_launch<false>(P, Q, c->numSMs, c->stream);
     if (e != cudaSuccess) return failCuda(c, e, occlusion ? "rtTraceOcclusion launch" : "rtTraceRays launch");
     return RT_OK;
@@ -1274,15 +1296,8 @@ int rtTraceRays(RtContext* c, const RtRay* rays, int n, RtRayHit* hits, int flag
     // batches of at most RT_TRACE_CHUNK_RAYS through device buffers of that size, kept by the context (72 MB at most)
     const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
     if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
-    for (int i0 = 0; i0 < n; i0 += chunk)
-    {
-        const int m = n - i0 < chunk ? n - i0 : chunk;
-        if ((rc = stagedH2D(c, c->queryRays.p, rays + i0, (size_t)m * sizeof(RtRay))) != RT_OK) return rc;
-        if ((rc = traceLocal(c, c->queryRays.p, c->queryHits.p, m, flags)) != RT_OK) return rc;
-        if ((rc = stagedD2H(c, hits + i0, c->queryHits.p, (size_t)m * sizeof(RtRayHit))) != RT_OK) return rc;
-    }
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    return hostBatches(c, n, chunk, c->queryRays.p, rays, sizeof(RtRay), c->queryHits.p, hits, sizeof(RtRayHit),
+                       [&](int, int m) { return traceLocal(c, c->queryRays.p, c->queryHits.p, m, flags); });
 }
 
 int rtTraceRaysDevice(RtContext* c, const void* dRays, void* dHits, int n, int flags)
@@ -1307,15 +1322,8 @@ int rtTraceOcclusion(RtContext* c, const RtRaySegment* segs, int n, uint8_t* occ
     if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
     RtRaySegment* dSegs = reinterpret_cast<RtRaySegment*>(c->queryHits.p);
     unsigned char* dOccluded = reinterpret_cast<unsigned char*>(c->queryRays.p);
-    for (int i0 = 0; i0 < n; i0 += chunk)
-    {
-        const int m = n - i0 < chunk ? n - i0 : chunk;
-        if ((rc = stagedH2D(c, dSegs, segs + i0, (size_t)m * sizeof(RtRaySegment))) != RT_OK) return rc;
-        if ((rc = occlusionLocal(c, dSegs, dOccluded, m, flags)) != RT_OK) return rc;
-        if ((rc = stagedD2H(c, occluded + i0, dOccluded, (size_t)m)) != RT_OK) return rc;
-    }
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    return hostBatches(c, n, chunk, dSegs, segs, sizeof(RtRaySegment), dOccluded, occluded, 1,
+                       [&](int, int m) { return occlusionLocal(c, dSegs, dOccluded, m, flags); });
 }
 
 int rtTraceOcclusionDevice(RtContext* c, const void* dSegs, void* dOccluded, int n, int flags)
@@ -1329,11 +1337,19 @@ int rtTraceOcclusionDevice(RtContext* c, const void* dSegs, void* dOccluded, int
 }
 
 // ---- radiance along caller-supplied rays (rtTracePaths, k_trace_paths in rt_kernel_query.cuh) ------------------------------------------
-static int pathArgs(RtContext* c, const char* what, const void* rays, const void* out, int n, int samples)
+// What both forms of rtTracePaths and rtBakeProbes check; `items` names the input pointer ("rays", "positions")
+static int batchArgs(RtContext* c, const char* what, const char* items, const void* in, const void* out, int n, int samples)
 {
     int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
-    if (n < 0 || (n > 0 && (!rays || !out))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or rays / out NULL)");
+    if (n < 0 || (n > 0 && (!in || !out))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or " + items + " / out NULL)");
     if (samples < 1 || samples > RT_MAX_BATCH_SAMPLES) return fail(c, RT_E_INVALID, std::string(what) + ": samples must be 1 .. RT_MAX_BATCH_SAMPLES");
+    return RT_OK;
+}
+
+// A kernel-1-style loop traces one segment even with a negative bound, where the reference's loop (HL:484) traces none
+static int bounceLimit(RtContext* c, const char* what)
+{
+    if (c->P.MaxBounceCount < 0 || c->P.MaxBounceCount > 200) return fail(c, RT_E_STATE, std::string(what) + ": MaxBounceCount must be 0 .. 200 (as rtDispatch)");
     return RT_OK;
 }
 
@@ -1341,13 +1357,12 @@ static int pathArgs(RtContext* c, const char* what, const void* rays, const void
 // segments traced, through the kernel's counters; no timing events, so dispatches / kernelMs stay the camera kernels'.
 static int pathsLocal(RtContext* c, const RtPathRay* dRays, RtPathRadiance* dOut, int n, int samples)
 {
-    // a kernel-1-style loop traces one segment even with a negative bound, where the reference's loop (HL:484) traces none
-    if (c->P.MaxBounceCount < 0 || c->P.MaxBounceCount > 200) return fail(c, RT_E_STATE, "rtTracePaths: MaxBounceCount must be 0 .. 200 (as rtDispatch)");
-    int rc = prepareQueryScene(c, "rtTracePaths"); if (rc != RT_OK) return rc;
+    int rc = bounceLimit(c, "rtTracePaths"); if (rc != RT_OK) return rc;
+    if ((rc = prepareQueryScene(c, "rtTracePaths")) != RT_OK) return rc;
     const DevParams P = queryParams(c);
     PathParams Q = {};
     Q.rays = dRays; Q.out = dOut; Q.n = (unsigned int)n; Q.samples = samples;
-    sceneBounds(c, Q.modelLo, Q.modelHi, Q.sphLo, Q.sphHi);
+    Q.box = sceneBounds(c);
     cudaError_t e = paths_launch(P, Q, c->numSMs, c->stream);
     if (e != cudaSuccess) return failCuda(c, e, "rtTracePaths launch");
     return RT_OK;
@@ -1358,28 +1373,21 @@ static int pathsLocal(RtContext* c, const RtPathRay* dRays, RtPathRadiance* dOut
 int rtTracePaths(RtContext* c, const RtPathRay* rays, int n, int samples, RtPathRadiance* out)
 {
     if (!c) return RT_E_INVALID;
-    int rc = pathArgs(c, "rtTracePaths", rays, out, n, samples); if (rc != RT_OK) return rc;
+    int rc = batchArgs(c, "rtTracePaths", "rays", rays, out, n, samples); if (rc != RT_OK) return rc;
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
     if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
     RtPathRay* dRays = reinterpret_cast<RtPathRay*>(c->queryHits.p);
     RtPathRadiance* dOut = reinterpret_cast<RtPathRadiance*>(c->queryRays.p);
-    for (int i0 = 0; i0 < n; i0 += chunk)
-    {
-        const int m = n - i0 < chunk ? n - i0 : chunk;
-        if ((rc = stagedH2D(c, dRays, rays + i0, (size_t)m * sizeof(RtPathRay))) != RT_OK) return rc;
-        if ((rc = pathsLocal(c, dRays, dOut, m, samples)) != RT_OK) return rc;
-        if ((rc = stagedD2H(c, out + i0, dOut, (size_t)m * sizeof(RtPathRadiance))) != RT_OK) return rc;
-    }
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    return hostBatches(c, n, chunk, dRays, rays, sizeof(RtPathRay), dOut, out, sizeof(RtPathRadiance),
+                       [&](int, int m) { return pathsLocal(c, dRays, dOut, m, samples); });
 }
 
 int rtTracePathsDevice(RtContext* c, const void* dRays, void* dOut, int n, int samples)
 {
     if (!c) return RT_E_INVALID;
-    int rc = pathArgs(c, "rtTracePathsDevice", dRays, dOut, n, samples); if (rc != RT_OK) return rc;
+    int rc = batchArgs(c, "rtTracePathsDevice", "rays", dRays, dOut, n, samples); if (rc != RT_OK) return rc;
     if (((uintptr_t)dRays & 3u) || ((uintptr_t)dOut & 15u)) return fail(c, RT_E_INVALID, "rtTracePathsDevice: dRays must be 4-byte and dOut 16-byte aligned");
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
@@ -1387,14 +1395,6 @@ int rtTracePathsDevice(RtContext* c, const void* dRays, void* dOut, int n, int s
 }
 
 // ---- light probes (rtBakeProbes, rt_kernel_probes.cuh) -------------------------------------------------------------------------------
-static int probeArgs(RtContext* c, const char* what, const void* positions, const void* out, int n, int samples)
-{
-    int rc = refuseMember(c, what); if (rc != RT_OK) return rc;
-    if (n < 0 || (n > 0 && (!positions || !out))) return fail(c, RT_E_INVALID, std::string(what) + ": bad argument (n < 0, or positions / out NULL)");
-    if (samples < 1 || samples > RT_MAX_BATCH_SAMPLES) return fail(c, RT_E_INVALID, std::string(what) + ": samples must be 1 .. RT_MAX_BATCH_SAMPLES");
-    return RT_OK;
-}
-
 // The probes of one launch: as many as RT_PROBE_SCRATCH_CHUNKS chunk records hold
 static int probesPerLaunch(int samples)
 {
@@ -1405,8 +1405,8 @@ static int probesPerLaunch(int samples)
 // probesPerLaunch probes; asynchronous on the context's stream.  The scratch is allocated (or grown) here and nothing else is.
 static int probesLocal(RtContext* c, const float* dPositions, RtProbeSH* dOut, int n, int samples, uint32_t seed, unsigned int p0)
 {
-    if (c->P.MaxBounceCount < 0 || c->P.MaxBounceCount > 200) return fail(c, RT_E_STATE, "rtBakeProbes: MaxBounceCount must be 0 .. 200 (as rtDispatch)");
-    int rc = prepareQueryScene(c, "rtBakeProbes"); if (rc != RT_OK) return rc;
+    int rc = bounceLimit(c, "rtBakeProbes"); if (rc != RT_OK) return rc;
+    if ((rc = prepareQueryScene(c, "rtBakeProbes")) != RT_OK) return rc;
     const unsigned int chunks = ((unsigned int)samples + RT_PROBE_CHUNK - 1) / RT_PROBE_CHUNK;
     const int per = probesPerLaunch(samples);
     const int first = n < per ? n : per;
@@ -1414,7 +1414,7 @@ static int probesLocal(RtContext* c, const float* dPositions, RtProbeSH* dOut, i
     const DevParams P = queryParams(c);
     ProbeParams Q = {};
     Q.scratch = c->probeScratch.p; Q.chunks = chunks; Q.samples = samples; Q.seed = seed;
-    sceneBounds(c, Q.modelLo, Q.modelHi, Q.sphLo, Q.sphHi);
+    Q.box = sceneBounds(c);
     for (int i0 = 0; i0 < n; i0 += per)
     {
         Q.positions = dPositions + 3 * (size_t)i0; Q.out = dOut + i0;
@@ -1428,27 +1428,20 @@ static int probesLocal(RtContext* c, const float* dPositions, RtProbeSH* dOut, i
 int rtBakeProbes(RtContext* c, const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out)
 {
     if (!c) return RT_E_INVALID;
-    int rc = probeArgs(c, "rtBakeProbes", positions, out, n, samples); if (rc != RT_OK) return rc;
+    int rc = batchArgs(c, "rtBakeProbes", "positions", positions, out, n, samples); if (rc != RT_OK) return rc;
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     const int per = probesPerLaunch(samples);
     const int chunk = n < per ? n : per;
     if (c->probeOut.cap < (size_t)chunk) { CK(c->probePositions.ensure(3 * (size_t)chunk)); CK(c->probeOut.ensure((size_t)chunk)); }
-    for (int i0 = 0; i0 < n; i0 += chunk)
-    {
-        const int m = n - i0 < chunk ? n - i0 : chunk;
-        if ((rc = stagedH2D(c, c->probePositions.p, positions + 3 * (size_t)i0, (size_t)m * 3 * sizeof(float))) != RT_OK) return rc;
-        if ((rc = probesLocal(c, c->probePositions.p, c->probeOut.p, m, samples, seed, (unsigned int)i0)) != RT_OK) return rc;
-        if ((rc = stagedD2H(c, out + i0, c->probeOut.p, (size_t)m * sizeof(RtProbeSH))) != RT_OK) return rc;
-    }
-    CK(cudaStreamSynchronize(c->stream));
-    return RT_OK;
+    return hostBatches(c, n, chunk, c->probePositions.p, positions, 3 * sizeof(float), c->probeOut.p, out, sizeof(RtProbeSH),
+                       [&](int i0, int m) { return probesLocal(c, c->probePositions.p, c->probeOut.p, m, samples, seed, (unsigned int)i0); });
 }
 
 int rtBakeProbesDevice(RtContext* c, const void* dPositions, void* dOut, int n, int samples, uint32_t seed)
 {
     if (!c) return RT_E_INVALID;
-    int rc = probeArgs(c, "rtBakeProbesDevice", dPositions, dOut, n, samples); if (rc != RT_OK) return rc;
+    int rc = batchArgs(c, "rtBakeProbesDevice", "positions", dPositions, dOut, n, samples); if (rc != RT_OK) return rc;
     if (((uintptr_t)dPositions & 3u) || ((uintptr_t)dOut & 15u)) return fail(c, RT_E_INVALID, "rtBakeProbesDevice: dPositions must be 4-byte and dOut 16-byte aligned");
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));

@@ -14,7 +14,7 @@
 // records, the TLAS and the sphere accelerator were padded for (fitOriginPadding, rt_api.cu), so the per-ray test of the queries is
 // not made; Intersect's QUERY form is used only for what it reports, the winner's kind and index.
 #pragma once
-#include "rt_kernel_wave.cuh"
+#include "rt_kernel_query.cuh"
 
 namespace rtd {
 
@@ -42,12 +42,7 @@ template <bool STATS, bool EXT, bool TLAS>
 __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_camera_features(const __grid_constant__ DevParams P, const __grid_constant__ FeatureParams F)
 {
     RT_DYNAMIC_SMEM(smemRaw);
-    DevSphere* smemSpheres = reinterpret_cast<DevSphere*>(smemRaw);
-    {
-        const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
-        for (int i = threadIdx.x; i < nS; i += WAVE_THREADS) smemSpheres[i] = P.spheres[i];
-    }
-    __syncthreads();
+    const DevSphere* smemSpheres = StageSpheres(P, smemRaw);
 
     const unsigned int lane = threadIdx.x & 31u;
     Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
@@ -90,13 +85,7 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_camera_feat
         }
     }
 
-    unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
-    if (lane == 0) atomicAdd(P.counters + 0, (unsigned long long)r);
-    if (STATS)
-    {
-        const unsigned int b = __reduce_add_sync(0xffffffffu, cnt.box), t = __reduce_add_sync(0xffffffffu, cnt.tri), s = __reduce_add_sync(0xffffffffu, cnt.sph), sb = __reduce_add_sync(0xffffffffu, cnt.sbox);
-        if (lane == 0) { atomicAdd(P.counters + 1, (unsigned long long)b); atomicAdd(P.counters + 2, (unsigned long long)t); atomicAdd(P.counters + 3, (unsigned long long)s); atomicAdd(P.counters + 4, (unsigned long long)sb); }
-    }
+    FlushCounters<STATS>(P, cnt);
 }
 
 // The feature ray of every pixel of the image and the RNG state after its four draws: what rtTracePaths takes.  One thread per job.
@@ -115,22 +104,6 @@ __global__ void __launch_bounds__(WAVE_THREADS) k_camera_rays(const __grid_const
     out[6] = __uint_as_float(rngState);
 }
 
-template <bool S, bool X, bool T> inline cudaError_t features_launch_one(const DevParams& P, const FeatureParams& F, int numSMs, cudaStream_t stream)
-{
-    auto kernel = k_camera_features<S, X, T>;
-    const size_t smemBytes = (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
-    int ctasPerSM = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
-    if (e != cudaSuccess) return e;
-    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);                  // persistent: a multiple of the SM count
-    const unsigned int ctasNeeded = (F.totalJobs / 32u + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, F);
-    return cudaGetLastError();
-}
-
 // rows of this rank's bands inside the dispatched region, in 8x4-pixel tiles of 32 jobs (wave_launch's count)
 inline cudaError_t features_jobs(const DevParams& P, FeatureParams& F)
 {
@@ -145,15 +118,13 @@ inline cudaError_t features_jobs(const DevParams& P, FeatureParams& F)
     return cudaSuccess;
 }
 
-// The five instantiations of query_launch, chosen by the same rules
 inline cudaError_t features_launch(const DevParams& P, FeatureParams& F, int numSMs, cudaStream_t stream)
 {
     cudaError_t e = features_jobs(P, F);
     if (e != cudaSuccess || F.totalJobs == 0) return e;
-    const bool ext = P.sphBvh != 0 || P.forceExt != 0;
-    if (P.countStats) return ext ? features_launch_one<true, true, false>(P, F, numSMs, stream) : features_launch_one<true, false, false>(P, F, numSMs, stream);
-    if (P.tlas && P.modelSkip) return features_launch_one<false, true, true>(P, F, numSMs, stream);
-    return ext ? features_launch_one<false, true, false>(P, F, numSMs, stream) : features_launch_one<false, false, false>(P, F, numSMs, stream);
+    return with_query_kernel(P, [&](auto S, auto X, auto T) {
+        return persistent_launch(k_camera_features<S, X, T>, QUERY_SMEM_BYTES, F.totalJobs / 32u, P, F, numSMs, stream);
+    });
 }
 
 inline cudaError_t camera_rays_launch(const DevParams& P, FeatureParams& F, cudaStream_t stream)

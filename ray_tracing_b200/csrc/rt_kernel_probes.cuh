@@ -3,8 +3,8 @@
 // Two launches per batch of probes (include/rt_b200.h states the contract):
 //   k_bake_probes  the path tracer's samples.  A job is one (probe, chunk) pair: RT_PROBE_CHUNK consecutive samples of one probe, so
 //                  the grid fills from n * ceil(S / 32) jobs however few the probes are.  Each lane runs its job sample by sample and
-//                  segment by segment with kernel 1's refill (paths_body: ballot, one atomicAdd per warp, jobs by popcount rank),
-//                  Intersect<..., QUERY = true> with the per-segment gate and ShadeSegment, and adds L * Y_i into the chunk's 27
+//                  segment by segment in rtTracePaths' path lanes (path_lanes, rt_kernel_query.cuh: kernel 1's refill,
+//                  Intersect<..., QUERY = true> with the per-segment gate and ShadeSegment), and adds L * Y_i into the chunk's 27
 //                  sums.  The sums live in shared memory, one column per lane (sums[v * WAVE_THREADS + threadIdx.x]: no bank
 //                  conflicts), not in registers: k_trace_paths already spills at the 80-register cap, and 27 more live floats
 //                  across Intersect would all go to local memory (DESIGN.md §7d''''''''' has the -Xptxas -v figures).  A finished
@@ -29,8 +29,7 @@ struct ProbeParams
     unsigned int chunks;                         // ceil(samples / RT_PROBE_CHUNK)
     int samples;                                 // 1 .. RT_MAX_BATCH_SAMPLES
     uint32_t seed;
-    float modelLo[3], modelHi[3];                // as QueryParams
-    float sphLo[3], sphHi[3];
+    OriginBox box;
 };
 
 // Sample k of S: a spherical Fibonacci set, one binary32 operation at a time (the contract in include/rt_b200.h)
@@ -63,124 +62,67 @@ RT_DI void ProbeBasis(f3 d, float Y[9])
     Y[8] = 0.546274215f * ((d.x * d.x) - (d.y * d.y));
 }
 
-template <bool STATS, bool EXT, bool TLAS>
-RT_DI void probes_body(const DevParams& P, const ProbeParams& Q)
+// A job is one (probe, chunk) pair: samples k .. kEnd - 1 of probe job / Q.chunks, each from CreateRay(position, d_k, 1, 0)
+// (HL:439-448) with state H(H(seed + p) + k), projected onto the basis at d_k into the lane's column of the shared sums.
+struct ProbeJob
 {
-    RT_DYNAMIC_SMEM(smemRaw);
-    DevSphere* smemSpheres = reinterpret_cast<DevSphere*>(smemRaw);
-    float* sums = reinterpret_cast<float*>(smemSpheres + WAVE_MAX_SMEM_SPHERES) + threadIdx.x;     // this lane's column of 27
-    {
-        const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
-        for (int i = threadIdx.x; i < nS; i += WAVE_THREADS) smemSpheres[i] = P.spheres[i];
-    }
-    __syncthreads();
-
-    const unsigned int lane = threadIdx.x & 31u;
-    const unsigned int laneMaskLt = (1u << lane) - 1u;
-    const unsigned int jobs = Q.n * Q.chunks;
-    Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
-    bool exhausted = false, haveJob = false;
+    const ProbeParams& Q;
+    float* sums;                                 // this lane's column of 27 (sums[v * WAVE_THREADS])
     unsigned int job = 0, k = 0, kEnd = 0, rejected = 0;    // the lane's (probe, chunk) job, its current sample, the chunk's end
-    uint32_t probeKey = 0, rngState = 0;                    // H(seed + p); the path's RNG state
-    int bounce = 0;
-    PathState ray; ray.pos = ray.dir = ray.transmittance = ray.totalLight = splat3(0.0f);
+    uint32_t probeKey = 0;                                  // H(seed + p)
 
-    for (;;)
+    RT_DI void take(unsigned int j, uint32_t&)
     {
-        // [refill] lanes without a job take the next ones (ballot + one atomic per warp)
-        const bool need = !haveJob && !exhausted;
-        const unsigned int needMask = __ballot_sync(0xffffffffu, need);
-        if (needMask)
+        job = j;
+        const unsigned int p = job / Q.chunks, chunk = job - p * Q.chunks;
+        k = chunk * PROBE_CHUNK;
+        kEnd = k + PROBE_CHUNK < (unsigned int)Q.samples ? k + PROBE_CHUNK : (unsigned int)Q.samples;
+        probeKey = ProbeHash(Q.seed + Q.p0 + p);
+        for (int v = 0; v < 27; v++) sums[v * WAVE_THREADS] = 0.0f;
+        rejected = 0;
+    }
+    RT_DI void begin(PathState& ray, uint32_t& rngState) const
+    {
+        const float* o = Q.positions + 3u * (job / Q.chunks);
+        ray.pos = make_f3(__ldg(o), __ldg(o + 1), __ldg(o + 2));
+        ray.dir = ProbeDirection(k, Q.samples);
+        ray.transmittance = splat3(1.0f);
+        ray.totalLight = splat3(0.0f);
+        rngState = ProbeHash(probeKey + k);
+    }
+    RT_DI bool end(const PathState& ray, uint32_t)
+    {
+        // [project] the sample's Trace result onto the basis at its direction (recomputed: fewer live registers)
+        const f3 L = ray.totalLight;
+        if (Finite3(L))
         {
-            unsigned int base = 0;
-            const int leader = __ffs(needMask) - 1;
-            if ((int)lane == leader) base = atomicAdd(P.workCounter, (unsigned int)__popc(needMask));
-            base = __shfl_sync(0xffffffffu, base, leader);
-            if (need)
+            float Y[9]; ProbeBasis(ProbeDirection(k, Q.samples), Y);
+#pragma unroll
+            for (int i = 0; i < 9; i++)
             {
-                job = base + (unsigned int)__popc(needMask & laneMaskLt);
-                if (job >= jobs) exhausted = true;
-                else
-                {
-                    const unsigned int p = job / Q.chunks, chunk = job - p * Q.chunks;
-                    k = chunk * PROBE_CHUNK;
-                    kEnd = k + PROBE_CHUNK < (unsigned int)Q.samples ? k + PROBE_CHUNK : (unsigned int)Q.samples;
-                    probeKey = ProbeHash(Q.seed + Q.p0 + p);
-                    for (int v = 0; v < 27; v++) sums[v * WAVE_THREADS] = 0.0f;
-                    rejected = 0;
-                    bounce = -1;                 // a path starts below
-                    haveJob = true;
-                }
+                sums[i * WAVE_THREADS] = sums[i * WAVE_THREADS] + L.x * Y[i];
+                sums[(9 + i) * WAVE_THREADS] = sums[(9 + i) * WAVE_THREADS] + L.y * Y[i];
+                sums[(18 + i) * WAVE_THREADS] = sums[(18 + i) * WAVE_THREADS] + L.z * Y[i];
             }
         }
-        if (__ballot_sync(0xffffffffu, haveJob) == 0u) break;
-
-        if (haveJob)
-        {
-            if (bounce < 0)
-            {
-                // CreateRay(position, d_k, 1, 0) (HL:439-448) with state H(H(seed + p) + k)
-                const float* o = Q.positions + 3u * (job / Q.chunks);
-                ray.pos = make_f3(__ldg(o), __ldg(o + 1), __ldg(o + 2));
-                ray.dir = ProbeDirection(k, Q.samples);
-                ray.transmittance = splat3(1.0f);
-                ray.totalLight = splat3(0.0f);
-                rngState = ProbeHash(probeKey + k);
-                bounce = 0;
-            }
-            // [intersect] the segment, with rtTraceRays' gate on its own origin and direction
-            QueryRay q;
-            const bool dirOk = DirectionInRange(ray.dir);
-            q.modelsExact = dirOk && OriginInside(ray.pos, Q.modelLo, Q.modelHi);
-            q.spheresExact = dirOk && OriginInside(ray.pos, Q.sphLo, Q.sphHi);
-            q.noCull = false;                    // HL:487
-            const Hit hit = Intersect<STATS, EXT, TLAS, true>(P, nullptr, smemSpheres, ray.pos, ray.dir, cnt, &q);
-            // [shade]
-            const bool cont = ShadeSegment(P, hit, ray, rngState);
-            bounce++;
-            if (!cont || bounce > P.MaxBounceCount)
-            {
-                // [project] the sample's Trace result onto the basis at its direction (recomputed: fewer live registers)
-                const f3 L = ray.totalLight;
-                if (Finite3(L))
-                {
-                    float Y[9]; ProbeBasis(ProbeDirection(k, Q.samples), Y);
+        else rejected++;
+        if (++k < kEnd) return false;
+        float4* rec = reinterpret_cast<float4*>(Q.scratch + (size_t)job * PROBE_WORDS);
 #pragma unroll
-                    for (int i = 0; i < 9; i++)
-                    {
-                        sums[i * WAVE_THREADS] = sums[i * WAVE_THREADS] + L.x * Y[i];
-                        sums[(9 + i) * WAVE_THREADS] = sums[(9 + i) * WAVE_THREADS] + L.y * Y[i];
-                        sums[(18 + i) * WAVE_THREADS] = sums[(18 + i) * WAVE_THREADS] + L.z * Y[i];
-                    }
-                }
-                else rejected++;
-                bounce = -1;
-                if (++k >= kEnd)
-                {
-                    float4* rec = reinterpret_cast<float4*>(Q.scratch + (size_t)job * PROBE_WORDS);
-#pragma unroll
-                    for (int w = 0; w < 6; w++)
-                        rec[w] = make_float4(sums[(4 * w) * WAVE_THREADS], sums[(4 * w + 1) * WAVE_THREADS], sums[(4 * w + 2) * WAVE_THREADS], sums[(4 * w + 3) * WAVE_THREADS]);
-                    rec[6] = make_float4(sums[24 * WAVE_THREADS], sums[25 * WAVE_THREADS], sums[26 * WAVE_THREADS], __uint_as_float(rejected));
-                    haveJob = false;
-                }
-            }
-        }
+        for (int w = 0; w < 6; w++)
+            rec[w] = make_float4(sums[(4 * w) * WAVE_THREADS], sums[(4 * w + 1) * WAVE_THREADS], sums[(4 * w + 2) * WAVE_THREADS], sums[(4 * w + 3) * WAVE_THREADS]);
+        rec[6] = make_float4(sums[24 * WAVE_THREADS], sums[25 * WAVE_THREADS], sums[26 * WAVE_THREADS], __uint_as_float(rejected));
+        return true;
     }
+};
 
-    unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
-    if (lane == 0) atomicAdd(P.counters + 0, (unsigned long long)r);
-    if (STATS)
-    {
-        const unsigned int b = __reduce_add_sync(0xffffffffu, cnt.box), t = __reduce_add_sync(0xffffffffu, cnt.tri), s = __reduce_add_sync(0xffffffffu, cnt.sph), sb = __reduce_add_sync(0xffffffffu, cnt.sbox);
-        if (lane == 0) { atomicAdd(P.counters + 1, (unsigned long long)b); atomicAdd(P.counters + 2, (unsigned long long)t); atomicAdd(P.counters + 3, (unsigned long long)s); atomicAdd(P.counters + 4, (unsigned long long)sb); }
-    }
-}
-
+// The sums follow the staged spheres in the dynamic shared memory
 template <bool STATS, bool EXT, bool TLAS>
 __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_bake_probes(const __grid_constant__ DevParams P, const __grid_constant__ ProbeParams Q)
 {
-    probes_body<STATS, EXT, TLAS>(P, Q);
+    RT_DYNAMIC_SMEM(smemRaw);
+    ProbeJob J{Q, reinterpret_cast<float*>(smemRaw + QUERY_SMEM_BYTES) + threadIdx.x};
+    path_lanes<STATS, EXT, TLAS>(P, J, Q.n * Q.chunks, Q.box);
 }
 
 // Word v of probe p: the chunks' sums combined by the full binary tree over the chunk count padded to a power of two with +0 chunks,
@@ -215,32 +157,16 @@ __global__ void __launch_bounds__(PROBE_SUM_THREADS) k_probe_sums(const __grid_c
     *o = r * (12.566371f / __int2float_rn(Q.samples));
 }
 
-template <bool S, bool X, bool T> inline cudaError_t probes_launch_one(const DevParams& P, const ProbeParams& Q, int numSMs, cudaStream_t stream)
-{
-    auto kernel = k_bake_probes<S, X, T>;
-    const size_t smemBytes = (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere) + (size_t)27 * WAVE_THREADS * sizeof(float);
-    int ctasPerSM = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
-    if (e != cudaSuccess) return e;
-    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);                  // persistent: a multiple of the SM count
-    const unsigned int warpsNeeded = (Q.n * Q.chunks + 31u) / 32u;
-    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, Q);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    RT_LAUNCH((Q.n * PROBE_WORDS + PROBE_SUM_THREADS - 1) / PROBE_SUM_THREADS, PROBE_SUM_THREADS, 0, stream, k_probe_sums, Q);
-    return cudaGetLastError();
-}
-
-// The five instantiations of query_launch, chosen by the same rules
+// k_bake_probes over the launch's n * chunks jobs, then k_probe_sums over its records
 inline cudaError_t probes_launch(const DevParams& P, const ProbeParams& Q, int numSMs, cudaStream_t stream)
 {
-    const bool ext = P.sphBvh != 0 || P.forceExt != 0;
-    if (P.countStats) return ext ? probes_launch_one<true, true, false>(P, Q, numSMs, stream) : probes_launch_one<true, false, false>(P, Q, numSMs, stream);
-    if (P.tlas && P.modelSkip) return probes_launch_one<false, true, true>(P, Q, numSMs, stream);
-    return ext ? probes_launch_one<false, true, false>(P, Q, numSMs, stream) : probes_launch_one<false, false, false>(P, Q, numSMs, stream);
+    cudaError_t e = with_query_kernel(P, [&](auto S, auto X, auto T) {
+        return persistent_launch(k_bake_probes<S, X, T>, QUERY_SMEM_BYTES + (size_t)27 * WAVE_THREADS * sizeof(float), (Q.n * Q.chunks + 31u) / 32u,
+                                 P, Q, numSMs, stream);
+    });
+    if (e != cudaSuccess) return e;
+    RT_LAUNCH((Q.n * PROBE_WORDS + PROBE_SUM_THREADS - 1) / PROBE_SUM_THREADS, PROBE_SUM_THREADS, 0, stream, k_probe_sums, Q);
+    return cudaGetLastError();
 }
 
 } // namespace rtd

@@ -20,9 +20,13 @@
 // directions with QUERY_DIR2_MIN <= dot(dir, dir) <= QUERY_DIR2_MAX (NaN fails): |dir| within a factor 2^10 of a camera ray's, which
 // keeps every squared term within 2^+-20 of what unit-length rays produce.  Any other direction takes the linear loop as well.
 #pragma once
+#include <type_traits>
 #include "rt_kernel_wave.cuh"
 
 namespace rtd {
+
+// The boxes of origins the model records (world boxes, TLAS) and the sphere accelerator were padded for
+struct OriginBox { float modelLo[3], modelHi[3], sphLo[3], sphHi[3]; };
 
 struct QueryParams
 {
@@ -30,14 +34,14 @@ struct QueryParams
     RtRayHit* hits;
     unsigned int n;
     int noCull;                                  // RT_TRACE_NO_CULL: forceDontCullBack (HL:356)
-    float modelLo[3], modelHi[3];                // origins the model records (world boxes, TLAS) were padded for
-    float sphLo[3], sphHi[3];                    // origins the sphere accelerator was padded for
+    OriginBox box;
     const RtRaySegment* segs;                    // rtTraceOcclusion: the segments and their answers (rays / hits unused)
     unsigned char* occluded;
 };
 
 constexpr float QUERY_DIR2_MIN = 9.5367431640625e-07f;      // 2^-20: |dir| >= 2^-10
 constexpr float QUERY_DIR2_MAX = 1048576.0f;                 // 2^20:  |dir| <= 2^10
+constexpr size_t QUERY_SMEM_BYTES = (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
 
 RT_DI bool OriginInside(f3 o, const float lo[3], const float hi[3])
 {
@@ -50,17 +54,22 @@ RT_DI bool DirectionInRange(f3 d)
     return dd >= QUERY_DIR2_MIN && dd <= QUERY_DIR2_MAX;
 }
 
+// The first WAVE_MAX_SMEM_SPHERES spheres into the CTA's dynamic shared memory, as wave_body stages them (no tree tops)
+RT_DI DevSphere* StageSpheres(const DevParams& P, unsigned char* smem)
+{
+    DevSphere* smemSpheres = reinterpret_cast<DevSphere*>(smem);
+    const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
+    for (int i = threadIdx.x; i < nS; i += WAVE_THREADS) smemSpheres[i] = P.spheres[i];
+    __syncthreads();
+    return smemSpheres;
+}
+
 // One persistent grid over Q.n rays (ANY = false: RtRay -> RtRayHit) or segments (ANY = true: RtRaySegment -> one byte, 1 = occluded)
 template <bool STATS, bool EXT, bool TLAS, bool ANY>
 RT_DI void query_body(const DevParams& P, const QueryParams& Q)
 {
     RT_DYNAMIC_SMEM(smemRaw);
-    DevSphere* smemSpheres = reinterpret_cast<DevSphere*>(smemRaw);
-    {
-        const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
-        for (int i = threadIdx.x; i < nS; i += WAVE_THREADS) smemSpheres[i] = P.spheres[i];
-    }
-    __syncthreads();
+    const DevSphere* smemSpheres = StageSpheres(P, smemRaw);
 
     const unsigned int lane = threadIdx.x & 31u;
     Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
@@ -76,10 +85,12 @@ RT_DI void query_body(const DevParams& P, const QueryParams& Q)
             const float* r = ANY ? reinterpret_cast<const float*>(Q.segs + i) : reinterpret_cast<const float*>(Q.rays + i);
             const f3 o = make_f3(__ldg(r), __ldg(r + 1), __ldg(r + 2));
             const f3 d = make_f3(__ldg(r + 3), __ldg(r + 4), __ldg(r + 5));
+            // the per-ray gate (the header's conditions), as path_lanes has it per segment.  Written out in both: behind a function
+            // the two flags are carried as bytes rather than predicates, and the query and path kernels spill more.
             QueryRay q;
             const bool dirOk = DirectionInRange(d);
-            q.modelsExact = dirOk && OriginInside(o, Q.modelLo, Q.modelHi);
-            q.spheresExact = dirOk && OriginInside(o, Q.sphLo, Q.sphHi);
+            q.modelsExact = dirOk && OriginInside(o, Q.box.modelLo, Q.box.modelHi);
+            q.spheresExact = dirOk && OriginInside(o, Q.box.sphLo, Q.box.sphHi);
             q.noCull = Q.noCull != 0;
             if constexpr (ANY)
             {
@@ -97,14 +108,7 @@ RT_DI void query_body(const DevParams& P, const QueryParams& Q)
             }
         }
     }
-
-    unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
-    if (lane == 0) atomicAdd(P.counters + 0, (unsigned long long)r);
-    if (STATS)
-    {
-        const unsigned int b = __reduce_add_sync(0xffffffffu, cnt.box), t = __reduce_add_sync(0xffffffffu, cnt.tri), s = __reduce_add_sync(0xffffffffu, cnt.sph), sb = __reduce_add_sync(0xffffffffu, cnt.sbox);
-        if (lane == 0) { atomicAdd(P.counters + 1, (unsigned long long)b); atomicAdd(P.counters + 2, (unsigned long long)t); atomicAdd(P.counters + 3, (unsigned long long)s); atomicAdd(P.counters + 4, (unsigned long long)sb); }
-    }
+    FlushCounters<STATS>(P, cnt);
 }
 
 template <bool STATS, bool EXT, bool TLAS>
@@ -119,16 +123,17 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_occlu
     query_body<STATS, EXT, TLAS, true>(P, Q);
 }
 
-template <bool S, bool X, bool T, bool ANY> inline cudaError_t query_launch_one(const DevParams& P, const QueryParams& Q, int numSMs, cudaStream_t stream)
+// A persistent launch of the query family: as many CTAs as fit on every SM (a multiple of the SM count), but no more than the jobs
+// of warpsNeeded warps fill (at least one); the work counter the warps draw from starts at 0.
+template <class Kernel, class Params>
+inline cudaError_t persistent_launch(Kernel kernel, size_t smemBytes, unsigned int warpsNeeded, const DevParams& P, const Params& Q, int numSMs,
+                                     cudaStream_t stream)
 {
-    auto kernel = ANY ? k_trace_occlusion<S, X, T> : k_trace_rays<S, X, T>;
-    const size_t smemBytes = (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
     int ctasPerSM = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
     if (e != cudaSuccess) return e;
     if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);                  // persistent: a multiple of the SM count
-    const unsigned int warpsNeeded = (Q.n + 31u) / 32u;
+    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);
     const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
     if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
     if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
@@ -136,59 +141,57 @@ template <bool S, bool X, bool T, bool ANY> inline cudaError_t query_launch_one(
     return cudaGetLastError();
 }
 
-// The instantiation follows the scene the way wave_launch chooses a camera kernel: the counting build walks every model; the TLAS
-// kernel when the scene has a TLAS and skipping is on; the extension family with the sphere accelerator (or "extInstantiation").
-// ANY: the occlusion kernels, chosen by the same rules.
+// The instantiation <STATS, EXT, TLAS> of a query-family kernel, chosen the way wave_launch chooses a camera kernel: the counting
+// build walks every model; the TLAS kernel when the scene has a TLAS and skipping is on; the extension family with the sphere
+// accelerator (or "extInstantiation").  `launch` is called with three std::integral_constant<bool, ...>.
+template <class Launch>
+inline cudaError_t with_query_kernel(const DevParams& P, Launch launch)
+{
+    std::true_type Y;
+    std::false_type N;
+    const bool ext = P.sphBvh != 0 || P.forceExt != 0;
+    if (P.countStats) return ext ? launch(Y, Y, N) : launch(Y, N, N);
+    if (P.tlas && P.modelSkip) return launch(N, Y, Y);
+    return ext ? launch(N, Y, N) : launch(N, N, N);
+}
+
+// ANY: the occlusion kernels
 template <bool ANY = false>
 inline cudaError_t query_launch(const DevParams& P, const QueryParams& Q, int numSMs, cudaStream_t stream)
 {
-    const bool ext = P.sphBvh != 0 || P.forceExt != 0;
-    if (P.countStats) return ext ? query_launch_one<true, true, false, ANY>(P, Q, numSMs, stream) : query_launch_one<true, false, false, ANY>(P, Q, numSMs, stream);
-    if (P.tlas && P.modelSkip) return query_launch_one<false, true, true, ANY>(P, Q, numSMs, stream);
-    return ext ? query_launch_one<false, true, false, ANY>(P, Q, numSMs, stream) : query_launch_one<false, false, false, ANY>(P, Q, numSMs, stream);
+    return with_query_kernel(P, [&](auto S, auto X, auto T) {
+        auto kernel = ANY ? k_trace_occlusion<S, X, T> : k_trace_rays<S, X, T>;
+        return persistent_launch(kernel, QUERY_SMEM_BYTES, (Q.n + 31u) / 32u, P, Q, numSMs, stream);
+    });
 }
 
-// ---- rtTracePaths: the radiance along caller-supplied rays ------------------------------------------------------------------------
-// A lane keeps its ray for all Q.samples paths (one RNG chain) and runs them segment by segment: Intersect<..., QUERY = true> with the
-// per-segment gate, then ShadeSegment — HL:479-542 as the camera kernels run it.  Paths of a ray take 1 .. MaxBounceCount + 1 segments
-// each, so a warp that took 32 rays at once would wait for its longest chain; instead, as in kernel 1 (wave_body), every iteration
-// first refills the lanes whose ray has ended (ballot, one atomicAdd per warp, rays handed out by popcount rank), then traces one
-// segment on every lane that has a ray.
-struct PathParams
-{
-    const RtPathRay* rays;
-    RtPathRadiance* out;
-    unsigned int n;
-    int samples;                                 // 1 .. RT_MAX_BATCH_SAMPLES
-    float modelLo[3], modelHi[3];                // as QueryParams
-    float sphLo[3], sphHi[3];
-};
-
-template <bool STATS, bool EXT, bool TLAS>
-RT_DI void paths_body(const DevParams& P, const PathParams& Q)
+// ---- path lanes: the refill loop of rtTracePaths and rtBakeProbes --------------------------------------------------------------------
+// Each lane runs its job sample by sample and segment by segment: Intersect<..., QUERY = true> with the per-segment gate, then
+// ShadeSegment — HL:479-542 as the camera kernels run it.  A path takes 1 .. MaxBounceCount + 1 segments, so a warp that took 32 jobs
+// at once would wait for its longest chain; instead, as in kernel 1 (wave_body), every iteration first refills the lanes whose job
+// has ended (ballot, one atomicAdd per warp, jobs handed out by popcount rank), then traces one segment on every lane that has a job.
+// What a job is comes from the policy J, per lane:
+//   J.take(job, rng)      job < jobs becomes the lane's: load it or reset its sums
+//   J.begin(ray, rng)     start the ray of the job's next sample
+//   J.end(ray, rng)       the sample has ended: add it up; when it was the job's last, store the result and return true
+template <bool STATS, bool EXT, bool TLAS, class Job>
+RT_DI void path_lanes(const DevParams& P, Job& J, unsigned int jobs, const OriginBox& box)
 {
     RT_DYNAMIC_SMEM(smemRaw);
-    DevSphere* smemSpheres = reinterpret_cast<DevSphere*>(smemRaw);
-    {
-        const int nS = P.sphereCount < WAVE_MAX_SMEM_SPHERES ? P.sphereCount : WAVE_MAX_SMEM_SPHERES;
-        for (int i = threadIdx.x; i < nS; i += WAVE_THREADS) smemSpheres[i] = P.spheres[i];
-    }
-    __syncthreads();
+    const DevSphere* smemSpheres = StageSpheres(P, smemRaw);
 
     const unsigned int lane = threadIdx.x & 31u;
     const unsigned int laneMaskLt = (1u << lane) - 1u;
     Counters cnt; cnt.rays = cnt.box = cnt.tri = cnt.sph = cnt.sbox = 0;
-    bool exhausted = false, haveRay = false;
-    unsigned int i = 0;                          // the lane's ray
+    bool exhausted = false, haveJob = false;
     uint32_t rngState = 0;
-    f3 total = splat3(0.0f);
-    int sample = 0, bounce = 0;
+    int bounce = 0;
     PathState ray; ray.pos = ray.dir = ray.transmittance = ray.totalLight = splat3(0.0f);
 
     for (;;)
     {
-        // [refill] lanes without a ray take the next ones (ballot + one atomic per warp)
-        const bool need = !haveRay && !exhausted;
+        // [refill] lanes without a job take the next ones (ballot + one atomic per warp)
+        const bool need = !haveJob && !exhausted;
         const unsigned int needMask = __ballot_sync(0xffffffffu, need);
         if (needMask)
         {
@@ -198,38 +201,31 @@ RT_DI void paths_body(const DevParams& P, const PathParams& Q)
             base = __shfl_sync(0xffffffffu, base, leader);
             if (need)
             {
-                i = base + (unsigned int)__popc(needMask & laneMaskLt);
-                if (i >= Q.n) exhausted = true;
+                const unsigned int job = base + (unsigned int)__popc(needMask & laneMaskLt);
+                if (job >= jobs) exhausted = true;
                 else
                 {
-                    rngState = __ldg(&Q.rays[i].rngState);
-                    total = splat3(0.0f);
-                    sample = 0;
+                    J.take(job, rngState);
                     bounce = -1;                 // a path starts below
-                    haveRay = true;
+                    haveJob = true;
                 }
             }
         }
-        // every lane now holds a ray or has run out of them
-        if (__ballot_sync(0xffffffffu, haveRay) == 0u) break;
+        // every lane now holds a job or has run out of them
+        if (__ballot_sync(0xffffffffu, haveJob) == 0u) break;
 
-        if (haveRay)
+        if (haveJob)
         {
             if (bounce < 0)
             {
-                // CreateRay(origin, dir, 1, 0) (HL:439-448), for every sample from the caller's record
-                const float* r = reinterpret_cast<const float*>(Q.rays + i);
-                ray.pos = make_f3(__ldg(r), __ldg(r + 1), __ldg(r + 2));
-                ray.dir = make_f3(__ldg(r + 3), __ldg(r + 4), __ldg(r + 5));
-                ray.transmittance = splat3(1.0f);
-                ray.totalLight = splat3(0.0f);
+                J.begin(ray, rngState);
                 bounce = 0;
             }
-            // [intersect] the segment, with rtTraceRays' gate on its own origin and direction
+            // [intersect] the segment, with rtTraceRays' gate on its own origin and direction (written out as in query_body)
             QueryRay q;
             const bool dirOk = DirectionInRange(ray.dir);
-            q.modelsExact = dirOk && OriginInside(ray.pos, Q.modelLo, Q.modelHi);
-            q.spheresExact = dirOk && OriginInside(ray.pos, Q.sphLo, Q.sphHi);
+            q.modelsExact = dirOk && OriginInside(ray.pos, box.modelLo, box.modelHi);
+            q.spheresExact = dirOk && OriginInside(ray.pos, box.sphLo, box.sphHi);
             q.noCull = false;                    // HL:487
             const Hit hit = Intersect<STATS, EXT, TLAS, true>(P, nullptr, smemSpheres, ray.pos, ray.dir, cnt, &q);
             // [shade]
@@ -237,57 +233,70 @@ RT_DI void paths_body(const DevParams& P, const PathParams& Q)
             bounce++;
             if (!cont || bounce > P.MaxBounceCount)
             {
-                total = total + ray.totalLight;                      // HL:578
                 bounce = -1;
-                if (++sample >= Q.samples)
-                {
-                    const f3 c = total / __int2float_rn(Q.samples);  // HL:581
-                    reinterpret_cast<float4*>(Q.out)[i] = make_float4(c.x, c.y, c.z, __uint_as_float(rngState));
-                    haveRay = false;
-                }
+                if (J.end(ray, rngState)) haveJob = false;
             }
         }
     }
-
-    unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
-    if (lane == 0) atomicAdd(P.counters + 0, (unsigned long long)r);
-    if (STATS)
-    {
-        const unsigned int b = __reduce_add_sync(0xffffffffu, cnt.box), t = __reduce_add_sync(0xffffffffu, cnt.tri), s = __reduce_add_sync(0xffffffffu, cnt.sph), sb = __reduce_add_sync(0xffffffffu, cnt.sbox);
-        if (lane == 0) { atomicAdd(P.counters + 1, (unsigned long long)b); atomicAdd(P.counters + 2, (unsigned long long)t); atomicAdd(P.counters + 3, (unsigned long long)s); atomicAdd(P.counters + 4, (unsigned long long)sb); }
-    }
+    FlushCounters<STATS>(P, cnt);
 }
+
+// ---- rtTracePaths: the radiance along caller-supplied rays ------------------------------------------------------------------------
+// A job is one caller ray: all Q.samples paths of it, on one RNG chain.
+struct PathParams
+{
+    const RtPathRay* rays;
+    RtPathRadiance* out;
+    unsigned int n;
+    int samples;                                 // 1 .. RT_MAX_BATCH_SAMPLES
+    OriginBox box;
+};
+
+struct PathJob
+{
+    const PathParams& Q;
+    unsigned int i = 0;                          // the lane's ray
+    int sample = 0;
+    f3 total = splat3(0.0f);
+
+    RT_DI void take(unsigned int job, uint32_t& rngState)
+    {
+        i = job;
+        rngState = __ldg(&Q.rays[i].rngState);
+        total = splat3(0.0f);
+        sample = 0;
+    }
+    // CreateRay(origin, dir, 1, 0) (HL:439-448), for every sample from the caller's record
+    RT_DI void begin(PathState& ray, uint32_t&) const
+    {
+        const float* r = reinterpret_cast<const float*>(Q.rays + i);
+        ray.pos = make_f3(__ldg(r), __ldg(r + 1), __ldg(r + 2));
+        ray.dir = make_f3(__ldg(r + 3), __ldg(r + 4), __ldg(r + 5));
+        ray.transmittance = splat3(1.0f);
+        ray.totalLight = splat3(0.0f);
+    }
+    RT_DI bool end(const PathState& ray, uint32_t rngState)
+    {
+        total = total + ray.totalLight;                          // HL:578
+        if (++sample < Q.samples) return false;
+        const f3 c = total / __int2float_rn(Q.samples);          // HL:581
+        reinterpret_cast<float4*>(Q.out)[i] = make_float4(c.x, c.y, c.z, __uint_as_float(rngState));
+        return true;
+    }
+};
 
 template <bool STATS, bool EXT, bool TLAS>
 __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_paths(const __grid_constant__ DevParams P, const __grid_constant__ PathParams Q)
 {
-    paths_body<STATS, EXT, TLAS>(P, Q);
+    PathJob J{Q};
+    path_lanes<STATS, EXT, TLAS>(P, J, Q.n, Q.box);
 }
 
-template <bool S, bool X, bool T> inline cudaError_t paths_launch_one(const DevParams& P, const PathParams& Q, int numSMs, cudaStream_t stream)
-{
-    auto kernel = k_trace_paths<S, X, T>;
-    const size_t smemBytes = (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
-    int ctasPerSM = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
-    if (e != cudaSuccess) return e;
-    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);                  // persistent: a multiple of the SM count
-    const unsigned int warpsNeeded = (Q.n + 31u) / 32u;
-    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, Q);
-    return cudaGetLastError();
-}
-
-// The five instantiations of query_launch, chosen by the same rules
 inline cudaError_t paths_launch(const DevParams& P, const PathParams& Q, int numSMs, cudaStream_t stream)
 {
-    const bool ext = P.sphBvh != 0 || P.forceExt != 0;
-    if (P.countStats) return ext ? paths_launch_one<true, true, false>(P, Q, numSMs, stream) : paths_launch_one<true, false, false>(P, Q, numSMs, stream);
-    if (P.tlas && P.modelSkip) return paths_launch_one<false, true, true>(P, Q, numSMs, stream);
-    return ext ? paths_launch_one<false, true, false>(P, Q, numSMs, stream) : paths_launch_one<false, false, false>(P, Q, numSMs, stream);
+    return with_query_kernel(P, [&](auto S, auto X, auto T) {
+        return persistent_launch(k_trace_paths<S, X, T>, QUERY_SMEM_BYTES, (Q.n + 31u) / 32u, P, Q, numSMs, stream);
+    });
 }
 
 } // namespace rtd

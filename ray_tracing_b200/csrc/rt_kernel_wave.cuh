@@ -282,6 +282,21 @@ RT_DI Hit Intersect(const DevParams& P, const float4* __restrict__ smemPairs, co
 #ifndef RT_WAVE_MINBLOCKS
 #define RT_WAVE_MINBLOCKS 6      // <= 85 registers: 24 warps per SM (faster than 16 warps on config 2)
 #endif
+
+// The end of a persistent kernel: the warp's counters summed, then added by lane 0 into P.counters (rays; with STATS the others too)
+template <bool STATS>
+RT_DI void FlushCounters(const DevParams& P, const Counters& cnt)
+{
+    const unsigned int lane = threadIdx.x & 31u;
+    unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
+    if (lane == 0) atomicAdd(P.counters + 0, (unsigned long long)r);
+    if (STATS)
+    {
+        const unsigned int b = __reduce_add_sync(0xffffffffu, cnt.box), t = __reduce_add_sync(0xffffffffu, cnt.tri), s = __reduce_add_sync(0xffffffffu, cnt.sph), sb = __reduce_add_sync(0xffffffffu, cnt.sbox);
+        if (lane == 0) { atomicAdd(P.counters + 1, (unsigned long long)b); atomicAdd(P.counters + 2, (unsigned long long)t); atomicAdd(P.counters + 3, (unsigned long long)s); atomicAdd(P.counters + 4, (unsigned long long)sb); }
+    }
+}
+
 // The kernel body.  TLAS = the many-model instantiation (its own kernel, k_raytrace_wave_tlas, so that the kernels measured in
 // round 1 keep their code: the TLAS walk and its mask exist only there).  FRAMES = the batch instantiations of rtDispatchFrames (never
 // CHUNKED): a lane keeps its pixel for frames Frame .. Frame + P.frames - 1, writing and accumulating each frame when its samples end.
@@ -492,14 +507,7 @@ RT_DI void wave_body(const DevParams& P, const unsigned int totalJobs, const uns
         }
     }
 
-    // ---- counters ---------------------------------------------------------------------------------------------------------------
-    unsigned int r = __reduce_add_sync(0xffffffffu, cnt.rays);
-    if (lane == 0) atomicAdd(P.counters + 0, (unsigned long long)r);
-    if (STATS)
-    {
-        const unsigned int b = __reduce_add_sync(0xffffffffu, cnt.box), t = __reduce_add_sync(0xffffffffu, cnt.tri), s = __reduce_add_sync(0xffffffffu, cnt.sph), sb = __reduce_add_sync(0xffffffffu, cnt.sbox);
-        if (lane == 0) { atomicAdd(P.counters + 1, (unsigned long long)b); atomicAdd(P.counters + 2, (unsigned long long)t); atomicAdd(P.counters + 3, (unsigned long long)s); atomicAdd(P.counters + 4, (unsigned long long)sb); }
-    }
+    FlushCounters<STATS>(P, cnt);
 }
 
 template <bool STATS, bool EXT, bool CHUNKED = false>
