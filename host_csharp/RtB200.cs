@@ -83,6 +83,13 @@ public static class RtB200
     public struct ProbeSH { [MarshalAs(UnmanagedType.ByValArray, SizeConst = 27)] public float[] sh; public uint rejected; }
     [DllImport(Lib)] public static extern int rtBakeProbes(IntPtr ctx, UnityEngine.Vector3[] positions, int n, int samples, uint seed, [Out] ProbeSH[] output);
     [DllImport(Lib)] public static extern int rtBakeProbesDevice(IntPtr ctx, IntPtr dPositions, IntPtr dOut, int n, int samples, uint seed);
+    // reflection probes: an HDR cube map per position, output[((p * 6 + f) * N + y) * N + x] with faces in CubemapFace order (+X, -X, +Y,
+    // -Y, +Z, -Z) and row 0 the top of the face; each texel the mean of `samples` paths over its area (R2 sub-texel offsets), rejected =
+    // samples left out for a non-finite radiance (they count as black).  Cubemap.SetPixels takes one face's rows bottom-up: flip y.
+    [StructLayout(LayoutKind.Sequential)]
+    public struct CubeTexel { public UnityEngine.Vector3 rgb; public uint rejected; }
+    [DllImport(Lib)] public static extern int rtBakeCubemaps(IntPtr ctx, UnityEngine.Vector3[] positions, int n, int faceSize, int samples, uint seed, [Out] CubeTexel[] output);
+    [DllImport(Lib)] public static extern int rtBakeCubemapsDevice(IntPtr ctx, IntPtr dPositions, IntPtr dOut, int n, int faceSize, int samples, uint seed);
     // one pixel of "FeatureFrame": object = ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1 (dst = +inf, the rest 0)
     [StructLayout(LayoutKind.Sequential)]
     public struct PixelFeatures { public UnityEngine.Vector3 albedo; public float dst; public UnityEngine.Vector3 normal; public int objectId; }

@@ -226,6 +226,44 @@ int rtTracePathsDevice(RtContext* ctx, const void* dRays, void* dOut, int n, int
 int rtBakeProbes(RtContext* ctx, const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out);
 int rtBakeProbesDevice(RtContext* ctx, const void* dPositions, void* dOut, int n, int samples, uint32_t seed);
 
+/* Extension: reflection-probe baking.  For each of n positions, an HDR cube map of the path tracer's radiance: 6 faces of N x N texels
+ * (N = faceSize), out[((p * 6 + f) * N + y) * N + x], faces in Unity's CubemapFace order +X, -X, +Y, -Y, +Z, -Z, row y = 0 first in
+ * memory and the top of the face.  Each texel is the mean of S = samples paths spread over its area.  Every bit is stated; each
+ * operation is one IEEE binary32 operation in the order written (no contraction); H(x) is the value NextRandom (HL:127-133) returns
+ * from state x.
+ *   - Sub-texel offset of sample k: an R2 low-discrepancy point, the same for every texel, with no RNG draw, k = 0 at the centre:
+ *         u = (float)(uint32_t)(k * 3242174889u + 2147483648u) * 2^-32;  v = (float)(uint32_t)(k * 2447445414u + 2147483648u) * 2^-32
+ *     (RandomValue's conversion, HL:137; the constants are 2^32 / g and 2^32 / g^2 rounded, g = 1.3247... the plastic number)
+ *   - Face coordinates:  a = (((float)x + u) / (float)N) * 2 - 1;  b = (((float)y + v) / (float)N) * 2 - 1
+ *   - Face vectors (the Direct3D / OpenGL cube-map table of DDS and KTX):  +X (1, -b, -a);  -X (-1, -b, a);  +Y (a, 1, b);
+ *     -Y (a, -1, -b);  +Z (a, -b, 1);  -Z (-a, -b, -1).  d = normalize(vector) = vector * (1 / sqrt(dot(vector, vector))), the dot
+ *     summed left to right.  Seen from inside the cube in Unity's left-handed, y-up world every face is upright and unmirrored:
+ *     texel (0, 0) of +X points towards (1, 1, 1).
+ *   - Paths: with tau = ((p * 6 + f) * N + y) * N + x the texel's index in the call (uint32),
+ *         L = Trace(CreateRay(positions[p], d, 1, 0), state = H(H(seed + tau) + k))        (HL:439-448, HL:479-542)
+ *     so a sample is rtTracePaths({positions[p], d, H(H(seed + tau) + k)}, samples = 1).rgb bit for bit.
+ *   - Sums: as rtBakeProbes' with 3 words: chunks of RT_PROBE_CHUNK consecutive k, each summing L from +0 in k order; a sample with any
+ *     non-finite component adds nothing and counts in `rejected`; the chunks combined by the full binary tree over the chunk count
+ *     padded with +0 chunks to a power of two, and
+ *         out.rgb = tree / (float)S
+ *     one IEEE division, as rtTracePaths divides its total: a rejected sample counts as black, and a texel is never 0 / 0.
+ *   - Everything else is rtBakeProbes': what it reads and leaves alone, RtStats.rays growing by segments and the countStats counters, the
+ *     per-segment gate of model skipping, the TLAS and the sphere accelerator, devices[0] on a group context, positions not validated.
+ *   - Launches: a call runs its texels in launches of floor(RT_CUBE_SCRATCH_CHUNKS / ceil(S / RT_PROBE_CHUNK)) texels (the last one
+ *     partial; a launch may end inside a probe or a face), each through rtBakeProbes' device scratch at 16 bytes per chunk (at most
+ *     RT_CUBE_SCRATCH_CHUNKS chunks: 112 MiB).  The launches change no bits: tau is the index in the call.
+ * Refused: rtBakeProbes' RT_E_INVALID cases, faceSize < 1 or > RT_CUBE_MAX_FACE, n * 6 * faceSize^2 > 2^31 - 1 texels, a device
+ * dPositions not 4-byte or dOut not 16-byte aligned -> RT_E_INVALID; rtBakeProbes' RT_E_STATE cases -> RT_E_STATE.  n = 0 is RT_OK and
+ * launches nothing.
+ * rtBakeCubemaps: host arrays (positions n x 3 floats, out n * 6 * N^2 RtCubeTexel); the positions are copied to the device once and
+ * the texels come back a launch at a time, through device buffers the context keeps (12 bytes per probe, 16 per texel of a launch;
+ * freed by rtDestroy); synchronises.  rtBakeCubemapsDevice: the same arrays in device memory of the context's device; allocates only
+ * the scratch; asynchronous on the context's stream (rtSetStream). */
+#define RT_CUBE_MAX_FACE 4096
+#define RT_CUBE_SCRATCH_CHUNKS (7 << 20)
+int rtBakeCubemaps(RtContext* ctx, const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out);
+int rtBakeCubemapsDevice(RtContext* ctx, const void* dPositions, void* dOut, int n, int faceSize, int samples, uint32_t seed);
+
 /* Extension: first-hit feature images for denoisers (albedo, shading normal, depth, object id: the guides OIDN, a-trous / SVGF filters
  * and mattes take next to the colour), and the camera's own rays.
  *

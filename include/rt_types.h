@@ -122,6 +122,12 @@ typedef struct RtProbeSH {
     uint32_t rejected;     /* samples whose radiance was not finite and were left out of the sums */
 } RtProbeSH;
 
+/* One texel of rtBakeCubemaps / rtBakeCubemapsDevice (include/rt_b200.h): the mean radiance over the texel's area.  16 bytes. */
+typedef struct RtCubeTexel {
+    float    rgb[3];
+    uint32_t rejected;     /* samples whose radiance was not finite and were left out of the sum (they count as black) */
+} RtCubeTexel;
+
 /* One pixel of rtDispatchFeatures' "FeatureFrame" (include/rt_b200.h): what the pixel's feature ray hits first.  32 bytes. */
 typedef struct RtPixelFeatures {
     float   albedo[3];    /* (0, 0, 0) on a miss; (1, 1, 1) for glass; GetMaterialColour (HL:450-466) otherwise */
@@ -142,6 +148,7 @@ static_assert(sizeof(RtPathRay) == 28, "RtPathRay record");
 static_assert(sizeof(RtPathRadiance) == 16, "RtPathRadiance record");
 static_assert(sizeof(RtPixelFeatures) == 32, "RtPixelFeatures record");
 static_assert(sizeof(RtProbeSH) == 112, "RtProbeSH record");
+static_assert(sizeof(RtCubeTexel) == 16, "RtCubeTexel record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

@@ -98,10 +98,11 @@ def build_oracle(force: bool = False) -> str:
     # images around that (tests/oracle_ext/rt_oracle_denoise.cpp); rtDenoiseTemporal is the reprojected, variance-guided filter with its
     # history around that (tests/oracle_ext/rt_oracle_temporal.cpp); rtDispatchAdaptive is the selection on its moments and Kernel_RayTrace
     # per active pixel around that (tests/oracle_ext/rt_oracle_adaptive.cpp); rtBakeProbes is Shader::Trace per probe sample, its SH
-    # chunk sums and their padded tree around that (tests/oracle_ext/rt_oracle_probes.cpp, the translation unit built here)
+    # chunk sums and their padded tree around that (tests/oracle_ext/rt_oracle_probes.cpp); rtBakeCubemaps is Shader::Trace per texel
+    # sample, its chunk sums and their padded tree around that (tests/oracle_ext/rt_oracle_cubemaps.cpp, the translation unit built here)
     srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(ORACLE_EXT, (".cpp",)) + _glob(INCLUDE, (".h",))
     if force or _newer(LIB_ORACLE, srcs):
-        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_probes.cpp")])
+        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_cubemaps.cpp")])
     return LIB_ORACLE
 
 

@@ -125,6 +125,12 @@ assert PROBE_SH_DTYPE.itemsize == 112
 RT_PROBE_CHUNK = 32
 RT_PROBE_SCRATCH_CHUNKS = 1 << 20
 
+# rtBakeCubemaps: one cube-map texel (RtCubeTexel)
+CUBE_TEXEL_DTYPE = np.dtype([("rgb", "<f4", 3), ("rejected", "<u4")])
+assert CUBE_TEXEL_DTYPE.itemsize == 16
+RT_CUBE_MAX_FACE = 4096
+RT_CUBE_SCRATCH_CHUNKS = 7 << 20
+
 
 # rtDispatchFeatures: one pixel of "FeatureFrame" (RtPixelFeatures).  object: ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1
 PIXEL_FEATURES_DTYPE = np.dtype([("albedo", "<f4", 3), ("dst", "<f4"), ("normal", "<f4", 3), ("object", "<i4")])
@@ -222,6 +228,8 @@ class RtLib:
             "rtTracePathsDevice": ([vp, vp, vp, ci, ci], ci),
             "rtBakeProbes": ([vp, vp, ci, ci, C.c_uint32, vp], ci),
             "rtBakeProbesDevice": ([vp, vp, vp, ci, ci, C.c_uint32], ci),
+            "rtBakeCubemaps": ([vp, vp, ci, ci, ci, C.c_uint32, vp], ci),
+            "rtBakeCubemapsDevice": ([vp, vp, vp, ci, ci, ci, C.c_uint32], ci),
             "rtDispatchFeatures": ([vp, ci, ci, ci], ci),
             "rtCameraRays": ([vp, vp, C.c_size_t], ci),
             "rtCameraRaysDevice": ([vp, vp, C.c_size_t], ci),
@@ -236,7 +244,7 @@ class RtLib:
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
                             "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
-                            "rtBakeProbes", "rtBakeProbesDevice", "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
+                            "rtBakeProbes", "rtBakeProbesDevice", "rtBakeCubemaps", "rtBakeCubemapsDevice", "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
                             "rtDispatchAdaptive", "rtDisplayMean"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
@@ -428,6 +436,23 @@ class RtContext:
         """rtBakeProbesDevice: n x 3 floats at positions_ptr (4-byte aligned) -> n RtProbeSH (PROBE_SH_DTYPE, 112 bytes) at out_ptr
         (16-byte aligned), both device memory of the context's GPU.  Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtBakeProbesDevice(self._h, C.c_void_p(positions_ptr), C.c_void_p(out_ptr), int(n), int(samples), int(seed) & 0xFFFFFFFF))
+
+    def bake_cubemaps(self, positions, face_size: int, samples: int, seed: int = 0) -> np.ndarray:
+        """rtBakeCubemaps: an HDR cube map of the radiance at every probe position ((n, 3) floats), each texel the mean of `samples`
+        paths spread over its area.  Returns an (n, 6, N, N) CUBE_TEXEL_DTYPE array [probe][face +X, -X, +Y, -Y, +Z, -Z][row][column]
+        (row 0 the top of the face): "rgb" the mean, "rejected" the samples left out for a non-finite radiance."""
+        pos = np.ascontiguousarray(np.asarray(positions, dtype=np.float32).reshape(-1, 3))
+        N = int(face_size)
+        out = np.empty((pos.shape[0], 6, max(N, 0), max(N, 0)), dtype=CUBE_TEXEL_DTYPE)
+        self._ck(self._L.rtBakeCubemaps(self._h, pos.ctypes.data if pos.size else None, int(pos.shape[0]), N, int(samples),
+                                        int(seed) & 0xFFFFFFFF, out.ctypes.data if out.size else None))
+        return out
+
+    def bake_cubemaps_device(self, positions_ptr: int, out_ptr: int, n: int, face_size: int, samples: int, seed: int = 0):
+        """rtBakeCubemapsDevice: n x 3 floats at positions_ptr (4-byte aligned) -> n * 6 * N^2 RtCubeTexel (CUBE_TEXEL_DTYPE, 16 bytes)
+        at out_ptr (16-byte aligned), both device memory of the context's GPU.  Asynchronous on the context's stream (set_stream)."""
+        self._ck(self._L.rtBakeCubemapsDevice(self._h, C.c_void_p(positions_ptr), C.c_void_p(out_ptr), int(n), int(face_size), int(samples),
+                                              int(seed) & 0xFFFFFFFF))
 
     def dispatch_features(self, gx: Optional[int] = None, gy: Optional[int] = None, gz: int = 1):
         """rtDispatchFeatures: the first-hit feature images (albedo, dst, normal, object id) of every pixel's own camera ray of the

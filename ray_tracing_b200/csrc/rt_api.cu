@@ -15,6 +15,7 @@
 #include "rt_kernel_temporal.cuh"
 #include "rt_kernel_adaptive.cuh"
 #include "rt_kernel_probes.cuh"
+#include "rt_kernel_cubemaps.cuh"
 #include "rt_repack.cuh"
 #include "rt_bvh_build.cuh"
 #include "rt_comm.cuh"
@@ -125,6 +126,9 @@ struct RtContext
     DevBuf<float4> moments; DevBuf<unsigned int> adaptiveList, adaptiveScratch; unsigned int* adaptiveCount = nullptr;
     // rtBakeProbes: the chunk records of one launch (both forms), and the host form's device copies of one launch's positions and results
     DevBuf<float> probeScratch, probePositions; DevBuf<RtProbeSH> probeOut;
+    // rtBakeCubemaps: the host form's results of one launch (the positions of the whole call go to probePositions, the records to
+    // probeScratch)
+    DevBuf<RtCubeTexel> cubeOut;
     std::vector<EventPair> pending, pendingX, freeEvents;
     RtStats stats;
 };
@@ -335,7 +339,7 @@ int rtDestroy(RtContext* c)
     c->queryRays.release(); c->queryHits.release(); c->cameraRays.release();
     c->denoiseScratch.release(); c->temporalHist.release();
     c->adaptiveList.release(); c->adaptiveScratch.release();
-    c->probeScratch.release(); c->probePositions.release(); c->probeOut.release();
+    c->probeScratch.release(); c->probePositions.release(); c->probeOut.release(); c->cubeOut.release();
     if (c->adaptiveCount) cudaFreeHost(c->adaptiveCount);
     c->repack.release();
     closePeers(c);
@@ -1225,7 +1229,8 @@ static int stagedH2D(RtContext* c, void* dst, const void* src, size_t bytes);
 static int stagedD2H(RtContext* c, void* dst, const void* src, size_t bytes);
 
 // The host form of a batch call: n records in batches of `chunk` through the device buffers dIn and dOut — each batch copied in
-// (inBytes per record), run by local(i0, m) on records i0 .. i0 + m - 1 and copied out (outBytes per record) — then one synchronise
+// (inBytes per record; none with inBytes = 0, for a call whose input went to the device whole), run by local(i0, m) on records
+// i0 .. i0 + m - 1 and copied out (outBytes per record) — then one synchronise
 extern "C++" {
 template <class Local>
 static int hostBatches(RtContext* c, int n, int chunk, void* dIn, const void* in, size_t inBytes, const void* dOut, void* out, size_t outBytes,
@@ -1446,6 +1451,77 @@ int rtBakeProbesDevice(RtContext* c, const void* dPositions, void* dOut, int n, 
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     return probesLocal(c, (const float*)dPositions, (RtProbeSH*)dOut, n, samples, seed, 0u);
+}
+
+// ---- reflection probes (rtBakeCubemaps, rt_kernel_cubemaps.cuh) -------------------------------------------------------------------
+// The texels of one launch: as many as RT_CUBE_SCRATCH_CHUNKS chunk records hold
+static int texelsPerLaunch(int samples)
+{
+    return RT_CUBE_SCRATCH_CHUNKS / ((samples + (int)RT_PROBE_CHUNK - 1) / (int)RT_PROBE_CHUNK);
+}
+
+// What both forms check beyond batchArgs; *texels gets n * 6 * faceSize^2
+static int cubemapArgs(RtContext* c, const char* what, const void* positions, const void* out, int n, int faceSize, int samples, int* texels)
+{
+    int rc = batchArgs(c, what, "positions", positions, out, n, samples); if (rc != RT_OK) return rc;
+    if (faceSize < 1 || faceSize > RT_CUBE_MAX_FACE) return fail(c, RT_E_INVALID, std::string(what) + ": faceSize must be 1 .. RT_CUBE_MAX_FACE");
+    const long long t = (long long)n * 6 * faceSize * faceSize;
+    if (t > 0x7fffffffLL) return fail(c, RT_E_INVALID, std::string(what) + ": n * 6 * faceSize^2 must be at most 2^31 - 1 texels");
+    *texels = (int)t;
+    return RT_OK;
+}
+
+// Texels t0 .. t0 + n - 1 of the call (dPositions: the call's probes; dOut: texel t0's record), in device memory of this context's
+// GPU, in launches of at most texelsPerLaunch texels; asynchronous on the context's stream.  The scratch is allocated (or grown) here
+// and nothing else is.
+static int cubemapsLocal(RtContext* c, const float* dPositions, RtCubeTexel* dOut, int n, unsigned int t0, int faceSize, int samples, uint32_t seed)
+{
+    int rc = bounceLimit(c, "rtBakeCubemaps"); if (rc != RT_OK) return rc;
+    if ((rc = prepareQueryScene(c, "rtBakeCubemaps")) != RT_OK) return rc;
+    const unsigned int chunks = ((unsigned int)samples + RT_PROBE_CHUNK - 1) / RT_PROBE_CHUNK;
+    const int per = texelsPerLaunch(samples);
+    const int first = n < per ? n : per;
+    if (c->probeScratch.cap < (size_t)first * chunks * CUBE_WORDS) CK(c->probeScratch.ensure((size_t)first * chunks * CUBE_WORDS));
+    const DevParams P = queryParams(c);
+    CubeParams Q = {};
+    Q.positions = dPositions; Q.scratch = c->probeScratch.p; Q.chunks = chunks; Q.faceSize = (unsigned int)faceSize;
+    Q.samples = samples; Q.seed = seed;
+    Q.box = sceneBounds(c);
+    for (int i0 = 0; i0 < n; i0 += per)
+    {
+        Q.out = dOut + i0; Q.n = (unsigned int)(n - i0 < per ? n - i0 : per); Q.t0 = t0 + (unsigned int)i0;
+        cudaError_t e = cubemaps_launch(P, Q, c->numSMs, c->stream);
+        if (e != cudaSuccess) return failCuda(c, e, "rtBakeCubemaps launch");
+    }
+    return RT_OK;
+}
+
+// The positions go to the device once; the texels come back a launch at a time
+int rtBakeCubemaps(RtContext* c, const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out)
+{
+    if (!c) return RT_E_INVALID;
+    int texels = 0;
+    int rc = cubemapArgs(c, "rtBakeCubemaps", positions, out, n, faceSize, samples, &texels); if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    const int per = texelsPerLaunch(samples);
+    const int chunk = texels < per ? texels : per;
+    if (c->probePositions.cap < 3 * (size_t)n) CK(c->probePositions.ensure(3 * (size_t)n));
+    if (c->cubeOut.cap < (size_t)chunk) CK(c->cubeOut.ensure((size_t)chunk));
+    if ((rc = stagedH2D(c, c->probePositions.p, positions, 3 * sizeof(float) * (size_t)n)) != RT_OK) return rc;
+    return hostBatches(c, texels, chunk, nullptr, nullptr, 0, c->cubeOut.p, out, sizeof(RtCubeTexel),
+                       [&](int i0, int m) { return cubemapsLocal(c, c->probePositions.p, c->cubeOut.p, m, (unsigned int)i0, faceSize, samples, seed); });
+}
+
+int rtBakeCubemapsDevice(RtContext* c, const void* dPositions, void* dOut, int n, int faceSize, int samples, uint32_t seed)
+{
+    if (!c) return RT_E_INVALID;
+    int texels = 0;
+    int rc = cubemapArgs(c, "rtBakeCubemapsDevice", dPositions, dOut, n, faceSize, samples, &texels); if (rc != RT_OK) return rc;
+    if (((uintptr_t)dPositions & 3u) || ((uintptr_t)dOut & 15u)) return fail(c, RT_E_INVALID, "rtBakeCubemapsDevice: dPositions must be 4-byte and dOut 16-byte aligned");
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    return cubemapsLocal(c, (const float*)dPositions, (RtCubeTexel*)dOut, texels, 0u, faceSize, samples, seed);
 }
 
 // ---- first-hit feature images and the camera's own rays (rtDispatchFeatures, rtCameraRays, rt_kernel_features.cuh) ---------------------

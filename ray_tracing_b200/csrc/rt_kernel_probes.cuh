@@ -9,7 +9,8 @@
 //                  conflicts), not in registers: k_trace_paths already spills at the 80-register cap, and 27 more live floats
 //                  across Intersect would all go to local memory (DESIGN.md §7d''''''''' has the -Xptxas -v figures).  A finished
 //                  chunk writes its 27 sums and its rejected count as one 112-byte record of the scratch.
-//   k_probe_sums   one thread per (probe, word): the tree over the probe's chunk records, the scale, the store into RtProbeSH.
+//   k_probe_sums   one thread per (probe, word): the tree over the probe's chunk records, the scale, the store into RtProbeSH
+//                  (ChunkTree, which rtBakeCubemaps' k_cube_sums shares).
 #pragma once
 #include "rt_kernel_query.cuh"
 
@@ -125,36 +126,45 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_bake_probes
     path_lanes<STATS, EXT, TLAS>(P, J, Q.n * Q.chunks, Q.box);
 }
 
-// Word v of probe p: the chunks' sums combined by the full binary tree over the chunk count padded to a power of two with +0 chunks,
-// adjacent chunks paired, then scaled by 4 pi / S.  The tree is built left to right on a stack: after chunk c the stack holds the
+// Word v of item p (a probe, a cube-map texel): the item's chunk records (WORDS words each, item-major; the last word the rejected
+// count) combined by the full binary tree over the chunk count padded to a power of two with +0 chunks, adjacent chunks paired, then
+// finished by fin (the scale or the division by S).  The tree is built left to right on a stack: after chunk c the stack holds the
 // complete subtrees of the first c + 1 chunks (one per set bit of c + 1, largest first), and the padded root is their right fold:
 // a subtree made only of padding is +0, and x + +0 = x for every value a sum from +0 can take (never -0).  The rejected counts add
-// as integers.
-__global__ void __launch_bounds__(PROBE_SUM_THREADS) k_probe_sums(const __grid_constant__ ProbeParams Q)
+// as integers.  out holds n items (Item: WORDS words laid out as the records are).
+template <int WORDS, class Item, class Finish>
+RT_DI void ChunkTree(const float* scratch, Item* out, unsigned int n, unsigned int chunks, Finish fin)
 {
     const unsigned int t = blockIdx.x * PROBE_SUM_THREADS + threadIdx.x;
-    if (t >= Q.n * PROBE_WORDS) return;
-    const unsigned int p = t / PROBE_WORDS, v = t - p * PROBE_WORDS;
-    const float* rec = Q.scratch + (size_t)p * Q.chunks * PROBE_WORDS + v;
-    float* o = reinterpret_cast<float*>(Q.out + p) + v;
-    if (v == PROBE_WORDS - 1)
+    if (t >= n * WORDS) return;
+    const unsigned int p = t / WORDS, v = t - p * WORDS;
+    const float* rec = scratch + (size_t)p * chunks * WORDS + v;
+    float* o = reinterpret_cast<float*>(out + p) + v;
+    if (v == WORDS - 1)
     {
         unsigned int r = 0;
-        for (unsigned int c = 0; c < Q.chunks; c++) r += __float_as_uint(rec[(size_t)c * PROBE_WORDS]);
+        for (unsigned int c = 0; c < chunks; c++) r += __float_as_uint(rec[(size_t)c * WORDS]);
         *o = __uint_as_float(r);
         return;
     }
     float stack[16];                             // chunks <= 2^15: at most 16 complete subtrees
     int top = 0;
-    for (unsigned int c = 0; c < Q.chunks; c++)
+    for (unsigned int c = 0; c < chunks; c++)
     {
-        float s = rec[(size_t)c * PROBE_WORDS];
+        float s = rec[(size_t)c * WORDS];
         for (unsigned int m = c + 1u; (m & 1u) == 0u; m >>= 1) s = stack[--top] + s;
         stack[top++] = s;
     }
     float r = stack[--top];
     while (top > 0) r = stack[--top] + r;
-    *o = r * (12.566371f / __int2float_rn(Q.samples));
+    *o = fin(r);
+}
+
+// The probe's SH coefficients: the tree scaled by 4 pi / S
+__global__ void __launch_bounds__(PROBE_SUM_THREADS) k_probe_sums(const __grid_constant__ ProbeParams Q)
+{
+    ChunkTree<PROBE_WORDS>(Q.scratch, Q.out, Q.n, Q.chunks,
+                           [&](float r) { return r * (12.566371f / __int2float_rn(Q.samples)); });
 }
 
 // k_bake_probes over the launch's n * chunks jobs, then k_probe_sums over its records

@@ -89,6 +89,19 @@ def write_exr(path: str, rgba: np.ndarray) -> None:
             f.write(struct.pack("<ii", y, row_bytes) + row[:, 3].tobytes() + row[:, 2].tobytes() + row[:, 1].tobytes() + row[:, 0].tobytes())
 
 
+def write_cubemap_exr(path: str, faces: np.ndarray) -> None:
+    """One probe of rtBakeCubemaps as an OpenEXR horizontal strip, 6N wide and N high: the faces left to right in their order (+X, -X,
+    +Y, -Y, +Z, -Z), each with row 0 at the top, rgb and alpha 1.  `faces` is one probe's (6, N, N) CUBE_TEXEL_DTYPE records or a
+    (6, N, N, 3) float array."""
+    rgb = np.asarray(faces["rgb"] if getattr(faces, "dtype", None) is not None and faces.dtype.names else faces, dtype=np.float32)
+    if rgb.ndim != 4 or rgb.shape[0] != 6 or rgb.shape[1] != rgb.shape[2] or rgb.shape[3] != 3:
+        raise ValueError("write_cubemap_exr expects one probe's (6, N, N) texels or a (6, N, N, 3) float array")
+    n = rgb.shape[1]
+    strip = np.ones((n, 6 * n, 4), dtype=np.float32)
+    strip[:, :, :3] = rgb.transpose(1, 0, 2, 3).reshape(n, 6 * n, 3)
+    write_exr(path, strip)
+
+
 def read_exr(path: str) -> np.ndarray:
     """Reads back what write_exr wrote (uncompressed scan lines, FLOAT channels A, B, G, R) -> (H, W, 4) float32 RGBA."""
     data = open(path, "rb").read()

@@ -33,6 +33,7 @@ std::string RtApi::Load(const char* path)
     TraceOcclusion = reinterpret_cast<decltype(TraceOcclusion)>(dlsym(dl, "rtTraceOcclusion"));
     TracePaths = reinterpret_cast<decltype(TracePaths)>(dlsym(dl, "rtTracePaths"));
     BakeProbesFn = reinterpret_cast<decltype(BakeProbesFn)>(dlsym(dl, "rtBakeProbes"));
+    BakeCubemapsFn = reinterpret_cast<decltype(BakeCubemapsFn)>(dlsym(dl, "rtBakeCubemaps"));
     DispatchFeatures = reinterpret_cast<decltype(DispatchFeatures)>(dlsym(dl, "rtDispatchFeatures"));
     CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
     DenoiseFn = reinterpret_cast<decltype(DenoiseFn)>(dlsym(dl, "rtDenoise"));
@@ -359,6 +360,16 @@ int RayComputeManager::BakeProbes(const float* positions, int n, int samples, ui
     int rc;
     if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
     TRY(api.BakeProbesFn(ctx, positions, n, samples, seed, out));
+    return RT_OK;
+}
+
+int RayComputeManager::BakeCubemaps(const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.BakeCubemapsFn) { lastError = "the library does not export rtBakeCubemaps"; return RT_E_STATE; }
+    int rc;
+    if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
+    TRY(api.BakeCubemapsFn(ctx, positions, n, faceSize, samples, seed, out));
     return RT_OK;
 }
 

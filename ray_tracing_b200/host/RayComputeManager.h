@@ -61,6 +61,7 @@ struct RtApi
     decltype(&rtTraceOcclusion) TraceOcclusion = nullptr;   // optional: occlusion queries (TraceOcclusion)
     decltype(&rtTracePaths) TracePaths = nullptr;           // optional: radiance along caller rays (TracePaths)
     decltype(&rtBakeProbes) BakeProbesFn = nullptr;         // optional: light probes (BakeProbes)
+    decltype(&rtBakeCubemaps) BakeCubemapsFn = nullptr;     // optional: reflection probes (BakeCubemaps)
     decltype(&rtDispatchFeatures) DispatchFeatures = nullptr;   // optional: first-hit feature images (RenderFeatures)
     decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
     decltype(&rtDenoise) DenoiseFn = nullptr;               // optional: the a-trous denoiser (Denoise)
@@ -153,6 +154,9 @@ public:
     // not in the reference: light probes — the L2 spherical harmonics of the radiance arriving at each of n positions (n x 3 floats)
     // from `samples` spherical Fibonacci directions (rtBakeProbes).  The scene is uploaded first as for TraceRays.
     int BakeProbes(const float* positions, int n, int samples, uint32_t seed, RtProbeSH* out);
+    // not in the reference: reflection probes — an HDR cube map of the radiance at each of n positions, 6 faces of faceSize^2 texels,
+    // each texel the mean of `samples` paths over its area (rtBakeCubemaps).  The scene is uploaded first as for TraceRays.
+    int BakeCubemaps(const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out);
     // not in the reference: the denoiser guides of the frame the NEXT RenderFrame() renders (rtDispatchFeatures over the whole image):
     // the upload sequence of RenderFrame, Frame = numAccumulatedFrames, and no step of the frame counter.  Call it right before that
     // RenderFrame; ResetAccumulatedRender resets the accumulated guides with the colour.

@@ -69,6 +69,7 @@ def host_lib() -> C.CDLL:
         L.rcmTraceOcclusion.argtypes = [vp, vp, ci, vp, ci]
         L.rcmTracePaths.argtypes = [vp, vp, ci, ci, vp]
         L.rcmBakeProbes.argtypes = [vp, vp, ci, ci, C.c_uint32, vp]
+        L.rcmBakeCubemaps.argtypes = [vp, vp, ci, ci, ci, C.c_uint32, vp]
         L.rcmRenderFeatures.argtypes = [vp]
         L.rcmReadFeatureImage.argtypes = [vp, cp, vp, C.c_size_t]
         L.rcmCameraRays.argtypes = [vp, vp, C.c_size_t]
@@ -353,6 +354,18 @@ class RayComputeManager:
         self._ck(self._L.rcmBakeProbes(self._h, pos.ctypes.data if pos.size else None, int(pos.shape[0]), int(samples), int(seed) & 0xFFFFFFFF,
                                        out.ctypes.data if out.size else None))
         return out["sh"].copy(), out["rejected"].copy()
+
+    # -- reflection probes (rtBakeCubemaps): an HDR cube map of the radiance at each position
+    def bake_cubemaps(self, positions, face_size: int, samples: int, seed: int = 0) -> np.ndarray:
+        """An HDR cube map of the radiance at each probe position ((n, 3) floats), each texel the mean of `samples` paths over its
+        area: (n, 6, N, N) capi.CUBE_TEXEL_DTYPE [probe][face +X, -X, +Y, -Y, +Z, -Z][row][column].  The scene is uploaded as a frame
+        would upload it; the render textures are not touched."""
+        pos = np.ascontiguousarray(np.asarray(positions, dtype=np.float32).reshape(-1, 3))
+        N = int(face_size)
+        out = np.empty((pos.shape[0], 6, max(N, 0), max(N, 0)), dtype=capi.CUBE_TEXEL_DTYPE)
+        self._ck(self._L.rcmBakeCubemaps(self._h, pos.ctypes.data if pos.size else None, int(pos.shape[0]), N, int(samples),
+                                         int(seed) & 0xFFFFFFFF, out.ctypes.data if out.size else None))
+        return out
 
     # -- denoiser guides (rtDispatchFeatures) and the camera's own rays (rtCameraRays)
     def RenderFeatures(self):
