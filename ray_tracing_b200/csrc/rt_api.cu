@@ -782,15 +782,6 @@ static void groupLimits(int gx, int gy, int gz, unsigned W, unsigned H, unsigned
     if (gz == 0) limX = limY = 0;
 }
 
-// The rows among the first limY that the bands of bandRows rows, dealt round-robin to tileWorld ranks, give to `rank`
-static unsigned ownedRows(unsigned limY, int bandRows, int tileWorld, int rank)
-{
-    unsigned rows = 0;
-    for (unsigned y0 = 0, b = 0; y0 < limY; y0 += (unsigned)bandRows, b++)
-        if ((int)(b % (unsigned)tileWorld) == rank) rows += limY - y0 < (unsigned)bandRows ? limY - y0 : (unsigned)bandRows;
-    return rows;
-}
-
 // A pair of timing events: one the context timed before and has read, or a new one
 static int takeEventPair(RtContext* c, EventPair& ev)
 {
@@ -835,7 +826,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     if (c->optKernel == 2 && c->P.NumRaysPerPixel > RT_MAX_BATCH_SAMPLES)
         return fail(c, RT_E_STATE, "rtDispatch: \"kernel\" = 2 counts a pixel's samples in 20 bits: NumRaysPerPixel above RT_MAX_BATCH_SAMPLES needs kernel 0 or 1");
 
-    c->dispatchPixels = (unsigned long long)ownedRows(limY, c->bandRows, c->tileWorld, c->tileRank) * limX;
+    c->dispatchPixels = (unsigned long long)owned_rows(limY, c->bandRows, c->tileWorld, c->tileRank) * limX;
     c->dispatchFrames = frames;
     int rc = RT_OK;
     if (ad)
@@ -884,8 +875,7 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
     // (kernel 1 only: in the pooled kernel the same hand-off was slower than whole pixels on small tiles and was taken out again)
     P.chunks = kernel == 1 ? wave_chunks(c->optSampleChunks, c->numSMs, c->dispatchPixels, P.NumRaysPerPixel, P.modelCount) : 1;
     if (c->dispatchPixels == 0 || frames > 1 || ad) P.chunks = 1;      // a rank whose tile is empty (an image lower than the band pattern); a batch of frames or a pixel list runs whole pixels
-    const unsigned long long rows = limX ? c->dispatchPixels / limX : 0;
-    const size_t jobs = (size_t)((limX + 7u) / 8u) * (size_t)((rows + 3ull) / 4ull) * 32u;
+    const size_t jobs = tile_jobs(limX, (unsigned)(c->dispatchPixels / limX));
     if (P.chunks > 1)
     {
         // kernel 1 counts its chunk jobs (jobs x chunks) in a 32-bit work counter that every resident lane draws from once more after
@@ -914,26 +904,13 @@ static int dispatchLocal(RtContext* c, int kernelIndex, int gx, int gy, int gz, 
         P.poolCold = c->poolCold.p;
     }
     // ad: the same kernels over the selected pixels only (adaptiveList, count long), with their moments
+    const CameraForm form = ad ? FORM_LIST : frames > 1 ? FORM_FRAMES : FORM_PLAIN;
     const unsigned count = ad ? (unsigned)ad->active : 0u;
-    cudaError_t e = cudaSuccess;
-    if (kernel == 0)
-    {
-        CK(cudaEventRecord(ev.a, c->stream));
-        dim3 grid((limX + 7) / 8, (limY + 7) / 8, 1), block(8, 8, 1);
-        if (ad) RT_LAUNCH((count + 63u) / 64u, 64, 0, c->stream, k_raytrace_mega_list<64>, P, count, c->adaptiveList.p, c->moments.p);
-        else if (frames > 1) RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega_frames, P);
-        else RT_LAUNCH(grid, block, 0, c->stream, k_raytrace_mega, P);
-        CK(cudaEventRecord(ev.b, c->stream));
-    }
-    else if (kernel == 1 && ad)
-    {
-        P.pixelList = c->adaptiveList.p; P.adaptiveMoments = c->moments.p;       // (the hand-off's and the cold pool's slots: unused here)
-        e = wave_launch_list(P, c->numSMs, count, c->stream, ev.a, ev.b);
-    }
-    else if (kernel == 1) e = wave_launch(P, c->numSMs, c->stream, ev.a, ev.b);
-    else if (ad) e = pool_launch_list(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b, count, c->adaptiveList.p, c->moments.p);
-    else e = pool_launch(P, c->optPoolSlots, c->numSMs, c->stream, ev.a, ev.b);
-    if (e != cudaSuccess) return failCuda(c, e, ad ? "adaptive launch" : kernel == 1 ? "wavefront launch" : "pool wavefront launch");
+    cudaError_t e;
+    if (kernel == 0) e = mega_launch(form, P, count, c->adaptiveList.p, c->moments.p, c->stream, ev.a, ev.b);
+    else if (kernel == 1) e = wave_launch(form, P, c->numSMs, count, c->adaptiveList.p, c->moments.p, c->stream, ev.a, ev.b);
+    else e = pool_launch(form, P, c->optPoolSlots, c->numSMs, count, c->adaptiveList.p, c->moments.p, c->stream, ev.a, ev.b);
+    if (e != cudaSuccess) return failCuda(c, e, ad ? "adaptive launch" : kernel == 0 ? "megakernel launch" : kernel == 1 ? "wavefront launch" : "pool wavefront launch");
     CK(cudaGetLastError());
     c->pending.push_back(ev);
     c->stats.dispatches += (unsigned long long)frames;
@@ -1038,7 +1015,7 @@ int rtSynchronize(RtContext* c)
 
 // ---- multi-GPU tile staging -----------------------------------------------------------------------------------------------
 
-static size_t tileRows(const RtContext* c, int rank) { return ownedRows((unsigned)c->height, c->bandRows, c->tileWorld, rank); }
+static size_t tileRows(const RtContext* c, int rank) { return owned_rows((unsigned)c->height, c->bandRows, c->tileWorld, rank); }
 
 static int ensureTileBuffers(RtContext* c)
 {
@@ -1168,9 +1145,9 @@ int rtDispatchFrames(RtContext* c, int gx, int gy, int gz, int frameCount)
 // back into ad.active (the call's one synchronisation).  Before the first traced call the moments are all zero (none allocated yet).
 static int adaptiveSelect(RtContext* c, unsigned limX, unsigned limY, AdaptiveCall& ad)
 {
-    const unsigned int rows = ownedRows(limY, c->bandRows, c->tileWorld, c->tileRank);
+    const unsigned int rows = owned_rows(limY, c->bandRows, c->tileWorld, c->tileRank);
     const unsigned int tilesX = (limX + 7u) / 8u;
-    const unsigned long long jobs = (unsigned long long)tilesX * ((rows + 3u) / 4u) * 32ull;       // < 2^32: W, H <= 65535
+    const unsigned long long jobs = tile_jobs(limX, rows);       // < 2^32: W, H <= 65535
     const unsigned int nBlocks = (unsigned int)((jobs + ADAPTIVE_BLOCK - 1) / ADAPTIVE_BLOCK);
     const size_t n = (size_t)c->width * c->height;
     CK(c->adaptiveList.ensure(n));

@@ -218,6 +218,10 @@ struct DevParams
 
 struct Counters { unsigned int rays, box, tri, sph, sbox; };
 
+// What a camera-kernel launch renders: one frame of the region (rtDispatch), P.frames frames of it (rtDispatchFrames) or the pixels of a
+// list (rtDispatchAdaptive).  Every kernel family has kernels of its own for each form.
+enum CameraForm { FORM_PLAIN, FORM_FRAMES, FORM_LIST };
+
 // Instrumented launches: add one pixel's share of the counters (`now` - `before`, all of it by the lane that traced it) into its
 // PixelStats record.  Relaxed atomics: several lanes may add to one pixel in the same launch (sample chunks, the pooled kernel's
 // rays of one pixel traced by different lanes); the sums are order-independent and wrap modulo 2^32.

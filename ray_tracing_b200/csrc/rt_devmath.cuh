@@ -56,8 +56,7 @@ struct f3 { float x, y, z; };
 #else
 #define RT_DNI __device__ __noinline__
 #endif
-// kernel launch: kernel<<<grid, block, smem, stream>>>(args).  RT_K() protects the commas of a template-id.
-#define RT_K(...) __VA_ARGS__
+// kernel launch: kernel<<<grid, block, smem, stream>>>(args)
 #ifndef RT_SIMT_EMU
 #define RT_LAUNCH(grid, block, smem, stream, kern, ...) kern<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #define RT_DYNAMIC_SMEM(name) extern __shared__ __align__(128) unsigned char name[]      // the CTA's dynamic shared memory

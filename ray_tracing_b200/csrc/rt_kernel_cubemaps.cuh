@@ -107,7 +107,7 @@ __global__ void __launch_bounds__(PROBE_SUM_THREADS) k_cube_sums(const __grid_co
 // k_bake_cubemaps over the launch's n * chunks jobs, then k_cube_sums over its records
 inline cudaError_t cubemaps_launch(const DevParams& P, const CubeParams& Q, int numSMs, cudaStream_t stream)
 {
-    cudaError_t e = with_query_kernel(P, [&](auto S, auto X, auto T) {
+    cudaError_t e = with_persistent_kernel(P, [&](auto S, auto X, auto T) {
         return persistent_launch(k_bake_cubemaps<S, X, T>, QUERY_SMEM_BYTES, (Q.n * Q.chunks + 31u) / 32u, P, Q, numSMs, stream);
     });
     if (e != cudaSuccess) return e;

@@ -24,7 +24,7 @@ struct FeatureParams
     float4* accumAlbedo;                         // "AccumulatedAlbedo" += (albedo, 1) on a hit
     float4* accumNormal;                         // "AccumulatedNormal" += (normal, dst) on a hit
     RtPathRay* rays;                             // k_camera_rays: W*H records, [y][x] (4-byte aligned)
-    unsigned int totalJobs, tilesX, ownedRows;   // 32 jobs per 8x4-pixel tile, as wave_launch counts them
+    unsigned int totalJobs, tilesX, ownedRows;   // 32 jobs per 8x4-pixel tile, as camera_jobs counts them
 };
 
 // job -> pixel, as wave_body maps it: tile job >> 5, lane job & 31; rows counted through this rank's bands.  false = outside the image
@@ -104,17 +104,12 @@ __global__ void __launch_bounds__(WAVE_THREADS) k_camera_rays(const __grid_const
     out[6] = __uint_as_float(rngState);
 }
 
-// rows of this rank's bands inside the dispatched region, in 8x4-pixel tiles of 32 jobs (wave_launch's count)
+// this rank's jobs over the dispatched region, counted as the camera kernels count them
 inline cudaError_t features_jobs(const DevParams& P, FeatureParams& F)
 {
-    unsigned int ownedRows = 0;
-    for (unsigned int y0 = 0, b = 0; y0 < P.limY; y0 += (unsigned int)P.bandRows, b++)
-        if ((int)(b % (unsigned int)P.tileWorld) == P.tileRank) ownedRows += (P.limY - y0) < (unsigned int)P.bandRows ? (P.limY - y0) : (unsigned int)P.bandRows;
-    F.tilesX = (P.limX + 7u) / 8u;
-    F.ownedRows = ownedRows;
-    const unsigned long long jobs64 = (unsigned long long)F.tilesX * ((ownedRows + 3u) / 4u) * 32ull;
-    if (jobs64 >= 0xffff0000ull) return cudaErrorInvalidValue;
-    F.totalJobs = (unsigned int)jobs64;
+    CameraJobs J;
+    if (!camera_jobs(FORM_PLAIN, P, 0u, J)) return cudaErrorInvalidValue;
+    F.totalJobs = J.total; F.tilesX = J.tilesX; F.ownedRows = J.ownedRows;
     return cudaSuccess;
 }
 
@@ -122,7 +117,7 @@ inline cudaError_t features_launch(const DevParams& P, FeatureParams& F, int num
 {
     cudaError_t e = features_jobs(P, F);
     if (e != cudaSuccess || F.totalJobs == 0) return e;
-    return with_query_kernel(P, [&](auto S, auto X, auto T) {
+    return with_persistent_kernel(P, [&](auto S, auto X, auto T) {
         return persistent_launch(k_camera_features<S, X, T>, QUERY_SMEM_BYTES, F.totalJobs / 32u, P, F, numSMs, stream);
     });
 }

@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(64) k_raytrace_mega_frames(const __grid_consta
 
 // rtDispatchAdaptive: k_raytrace_mega over the `count` pixels of the selection's list ((y << 16) | x each), a 1-D grid of BLOCK-thread
 // blocks; the write also updates the pixel's moments.  (A kernel of its own, so that k_raytrace_mega keeps its code; and a template,
-// instantiated where rt_api.cu launches it: defined here as a plain kernel, it moved ahead of the wavefront kernels in the module and
+// instantiated where mega_launch launches it: defined here as a plain kernel, it moved ahead of the wavefront kernels in the module and
 // the compiler then numbered the registers of the k_raytrace_wave_frames kernels differently.)
 template <unsigned int BLOCK>
 __global__ void __launch_bounds__(BLOCK) k_raytrace_mega_list(const __grid_constant__ DevParams P, const unsigned int count,
@@ -236,6 +236,20 @@ __global__ void __launch_bounds__(BLOCK) k_raytrace_mega_list(const __grid_const
     WritePixel<true, true>(P, o, pixelCol.x, pixelCol.y, pixelCol.z, moments);
     if (P.countStats) { Counters zero; zero.rays = zero.box = zero.tri = zero.sph = zero.sbox = 0; AddPixelStats(P, o, cnt, zero); }
     FlushCounters(P, cnt);
+}
+
+// Kernel 0 over one dispatch: 8 x 8-pixel groups over P's region, or (FORM_LIST) 64-thread blocks over the `count` pixels of `list`,
+// between the timing events.  A launch error is left to the caller's cudaGetLastError.
+inline cudaError_t mega_launch(CameraForm form, const DevParams& P, unsigned int count, const unsigned int* list, float4* moments,
+                               cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
+{
+    const cudaError_t e = cudaEventRecord(evA, stream);
+    if (e != cudaSuccess) return e;
+    const dim3 grid((P.limX + 7) / 8, (P.limY + 7) / 8, 1), block(8, 8, 1);
+    if (form == FORM_LIST) RT_LAUNCH((count + 63u) / 64u, 64, 0, stream, k_raytrace_mega_list<64>, P, count, list, moments);
+    else if (form == FORM_FRAMES) RT_LAUNCH(grid, block, 0, stream, k_raytrace_mega_frames, P);
+    else RT_LAUNCH(grid, block, 0, stream, k_raytrace_mega, P);
+    return cudaEventRecord(evB, stream);
 }
 
 } // namespace rtd

@@ -898,31 +898,41 @@ template <int M> inline size_t pool_smem_bytes(const DevParams& P)
          + (size_t)POOL_WARPS * POOL_CLOCK_BYTES;
 }
 
-template <int M> inline cudaError_t pool_configure_one()
+// Kernel 2's table: the __global__ of form F, <STATS, EXT, TLAS> and pool size M
+template <CameraForm F, bool S, bool X, bool T, int M>
+inline auto pool_kernel()
 {
-    cudaError_t e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool<false, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool<true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<false, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_frames<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas_frames<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<false, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<false, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_list<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_pool_tlas_list<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k_raytrace_pool<true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if constexpr (F == FORM_LIST && T) return k_raytrace_pool_tlas_list<M>;
+    else if constexpr (F == FORM_LIST) return k_raytrace_pool_list<S, X, M>;
+    else if constexpr (F == FORM_FRAMES && T) return k_raytrace_pool_tlas_frames<M>;
+    else if constexpr (F == FORM_FRAMES) return k_raytrace_pool_frames<S, X, M>;
+    else if constexpr (T) return k_raytrace_pool_tlas<M>;
+    else return k_raytrace_pool<S, X, M>;
 }
+
+// `f` with the pool size M (slots per warp) as a std::integral_constant; M = 0 is automatic: 64.  (96 slots so that every pixel of a
+// small tile is resident at once lost on small tiles: the 96-slot pools have no room for the stack ring.)
+template <class F>
+inline cudaError_t with_pool_slots(int M, F f)
+{
+    if (M == 0 || M == 64) return f(std::integral_constant<int, 64>());
+    if (M == 32) return f(std::integral_constant<int, 32>());
+    if (M == 96) return f(std::integral_constant<int, 96>());
+    return cudaErrorInvalidValue;
+}
+
 inline cudaError_t pool_configure()
 {
-    cudaError_t e;
-    if ((e = pool_configure_one<32>()) != cudaSuccess) return e;
-    if ((e = pool_configure_one<64>()) != cudaSuccess) return e;
-    return pool_configure_one<96>();
+    for (const int M : {32, 64, 96})
+    {
+        const cudaError_t e = with_pool_slots(M, [](auto m) {
+            return for_each_camera_kernel([](auto F, auto S, auto X, auto T) {
+                return cudaFuncSetAttribute(pool_kernel<F, S, X, T, decltype(m)::value>(), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+            });
+        });
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 // shared-memory bytes the pools leave for the tree-top cache (in NodePair records)
@@ -935,86 +945,30 @@ inline int pool_max_smem_pairs(int M, int sphereCount)
     return left <= 0 ? 0 : (int)(left / (long long)sizeof(NodePair));
 }
 
-template <int M> inline cudaError_t pool_launch_m(const DevParams& P, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB,
-                                                  unsigned totalJobs, unsigned tilesX, unsigned ownedRows)
+// Kernel 2 over one dispatch in `form` with pools of M slots; FORM_LIST: over the `count` pixels of `list`, whose moments its writes update
+inline cudaError_t pool_launch(CameraForm form, const DevParams& P, int M, int numSMs, unsigned int count, const unsigned int* list,
+                               float4* moments, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
 {
-    const size_t smemBytes = pool_smem_bytes<M>(P);
-    if (smemBytes > 227 * 1024) return cudaErrorInvalidConfiguration;
-    unsigned grid = (unsigned)numSMs;                                   // one persistent CTA per SM
-    const unsigned slots = POOL_WARPS * M;
-    const unsigned ctasNeeded = (totalJobs + POOL_WARPS - 1) / POOL_WARPS;   // at least one pixel per warp: small images spread over the SMs (fair share, pool_body)
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    grid = fit_persistent_grid(P.gridFit, grid, slots, totalJobs);
-    cudaError_t e;
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
-    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;   // extensions (peer stores, sphere accelerator, staged tree tops) compiled into their own instantiation
-    if (P.frames > 1)      // a batch of frames (rtDispatchFrames): the FRAMES kernels, chosen like the single-frame ones
-    {
-        if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<true, true, M>), P, totalJobs, tilesX, ownedRows);
-                            else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<true, false, M>), P, totalJobs, tilesX, ownedRows); }
-        else if (P.tlas && P.modelSkip) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_tlas_frames<M>), P, totalJobs, tilesX, ownedRows);
-        else { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<false, true, M>), P, totalJobs, tilesX, ownedRows);
-               else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_frames<false, false, M>), P, totalJobs, tilesX, ownedRows); }
-    }
-    else if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<true, true, M>), P, totalJobs, tilesX, ownedRows);
-                        else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<true, false, M>), P, totalJobs, tilesX, ownedRows); }
-    else if (P.tlas && P.modelSkip) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_tlas<M>), P, totalJobs, tilesX, ownedRows);
-    else { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<false, true, M>), P, totalJobs, tilesX, ownedRows);
-           else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool<false, false, M>), P, totalJobs, tilesX, ownedRows); }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return cudaEventRecord(evB, stream);
-}
-
-inline cudaError_t pool_launch(const DevParams& P, int M, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
-{
-    unsigned int ownedRows = 0;
-    for (unsigned int y0 = 0, b = 0; y0 < P.limY; y0 += (unsigned int)P.bandRows, b++)
-        if ((int)(b % (unsigned int)P.tileWorld) == P.tileRank) ownedRows += (P.limY - y0) < (unsigned int)P.bandRows ? (P.limY - y0) : (unsigned int)P.bandRows;
-    const unsigned int tilesX = (P.limX + 7u) / 8u;
-    const unsigned int tileRows = (ownedRows + 3u) / 4u;
-    const unsigned long long jobs64 = (unsigned long long)tilesX * tileRows * 32ull;
-    if (jobs64 >= 0xffff0000ull) return cudaErrorInvalidValue;
-    const unsigned int totalJobs = (unsigned int)jobs64;
-    if (M == 0) M = 64;      // automatic.  (96 slots so that every pixel of a small tile is resident at once lost on small tiles: the 96-slot
-                             // pools have no room for the stack ring.)
-    if (M == 32) return pool_launch_m<32>(P, numSMs, stream, evA, evB, totalJobs, tilesX, ownedRows);
-    if (M == 64) return pool_launch_m<64>(P, numSMs, stream, evA, evB, totalJobs, tilesX, ownedRows);
-    if (M == 96) return pool_launch_m<96>(P, numSMs, stream, evA, evB, totalJobs, tilesX, ownedRows);
-    return cudaErrorInvalidValue;
-}
-
-// rtDispatchAdaptive: kernel 2 over the `count` pixels of `list`, sized from the count and chosen like pool_launch_m's kernels
-template <int M> inline cudaError_t pool_launch_list_m(const DevParams& P, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB,
-                                                       unsigned count, const unsigned* list, float4* moments)
-{
-    const size_t smemBytes = pool_smem_bytes<M>(P);
-    if (smemBytes > 227 * 1024) return cudaErrorInvalidConfiguration;
-    unsigned grid = (unsigned)numSMs;
-    const unsigned ctasNeeded = (count + POOL_WARPS - 1) / POOL_WARPS;
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    grid = fit_persistent_grid(P.gridFit, grid, POOL_WARPS * M, count);
-    cudaError_t e;
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
-    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;
-    if (P.countStats) { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<true, true, M>), P, count, list, moments);
-                        else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<true, false, M>), P, count, list, moments); }
-    else if (P.tlas && P.modelSkip) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_tlas_list<M>), P, count, list, moments);
-    else { if (ext) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<false, true, M>), P, count, list, moments);
-           else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, RT_K(k_raytrace_pool_list<false, false, M>), P, count, list, moments); }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return cudaEventRecord(evB, stream);
-}
-
-inline cudaError_t pool_launch_list(const DevParams& P, int M, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB,
-                                    unsigned count, const unsigned* list, float4* moments)
-{
-    if (M == 0) M = 64;
-    if (M == 32) return pool_launch_list_m<32>(P, numSMs, stream, evA, evB, count, list, moments);
-    if (M == 64) return pool_launch_list_m<64>(P, numSMs, stream, evA, evB, count, list, moments);
-    if (M == 96) return pool_launch_list_m<96>(P, numSMs, stream, evA, evB, count, list, moments);
-    return cudaErrorInvalidValue;
+    CameraJobs J;
+    if (!camera_jobs(form, P, count, J)) return cudaErrorInvalidValue;
+    return with_pool_slots(M, [&](auto m) -> cudaError_t {
+        const size_t smemBytes = pool_smem_bytes<m>(P);
+        if (smemBytes > 227 * 1024) return cudaErrorInvalidConfiguration;
+        unsigned int grid = (unsigned int)numSMs;                                   // one persistent CTA per SM
+        const unsigned int ctasNeeded = (J.total + POOL_WARPS - 1) / POOL_WARPS;   // at least one pixel per warp: small images spread over the SMs (fair share, pool_body)
+        if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
+        grid = fit_persistent_grid(P.gridFit, grid, POOL_WARPS * m, J.total);
+        return with_camera_kernel(form, P, [&](auto F, auto S, auto X, auto T) -> cudaError_t {
+            const auto kernel = pool_kernel<F, S, X, T, decltype(m)::value>();
+            cudaError_t e;
+            if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
+            if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
+            if constexpr (F == FORM_LIST) RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, kernel, P, J.total, list, moments);
+            else RT_LAUNCH(grid, POOL_THREADS, smemBytes, stream, kernel, P, J.total, J.tilesX, J.ownedRows);
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            return cudaEventRecord(evB, stream);
+        });
+    });
 }
 
 } // namespace rtd

@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(PROBE_SUM_THREADS) k_probe_sums(const __grid_c
 // k_bake_probes over the launch's n * chunks jobs, then k_probe_sums over its records
 inline cudaError_t probes_launch(const DevParams& P, const ProbeParams& Q, int numSMs, cudaStream_t stream)
 {
-    cudaError_t e = with_query_kernel(P, [&](auto S, auto X, auto T) {
+    cudaError_t e = with_persistent_kernel(P, [&](auto S, auto X, auto T) {
         return persistent_launch(k_bake_probes<S, X, T>, QUERY_SMEM_BYTES + (size_t)27 * WAVE_THREADS * sizeof(float), (Q.n * Q.chunks + 31u) / 32u,
                                  P, Q, numSMs, stream);
     });

@@ -20,7 +20,6 @@
 // directions with QUERY_DIR2_MIN <= dot(dir, dir) <= QUERY_DIR2_MAX (NaN fails): |dir| within a factor 2^10 of a camera ray's, which
 // keeps every squared term within 2^+-20 of what unit-length rays produce.  Any other direction takes the linear loop as well.
 #pragma once
-#include <type_traits>
 #include "rt_kernel_wave.cuh"
 
 namespace rtd {
@@ -123,43 +122,25 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_occlu
     query_body<STATS, EXT, TLAS, true>(P, Q);
 }
 
-// A persistent launch of the query family: as many CTAs as fit on every SM (a multiple of the SM count), but no more than the jobs
-// of warpsNeeded warps fill (at least one); the work counter the warps draw from starts at 0.
+// A persistent launch of the query family: persistent_grid's grid over the jobs of warpsNeeded warps; the work counter the warps draw
+// from starts at 0
 template <class Kernel, class Params>
 inline cudaError_t persistent_launch(Kernel kernel, size_t smemBytes, unsigned int warpsNeeded, const DevParams& P, const Params& Q, int numSMs,
                                      cudaStream_t stream)
 {
-    int ctasPerSM = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
+    unsigned int grid = 0;
+    cudaError_t e = persistent_grid(kernel, smemBytes, warpsNeeded, numSMs, grid);
     if (e != cudaSuccess) return e;
-    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);
-    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
     if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
     RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, Q);
     return cudaGetLastError();
-}
-
-// The instantiation <STATS, EXT, TLAS> of a query-family kernel, chosen the way wave_launch chooses a camera kernel: the counting
-// build walks every model; the TLAS kernel when the scene has a TLAS and skipping is on; the extension family with the sphere
-// accelerator (or "extInstantiation").  `launch` is called with three std::integral_constant<bool, ...>.
-template <class Launch>
-inline cudaError_t with_query_kernel(const DevParams& P, Launch launch)
-{
-    std::true_type Y;
-    std::false_type N;
-    const bool ext = P.sphBvh != 0 || P.forceExt != 0;
-    if (P.countStats) return ext ? launch(Y, Y, N) : launch(Y, N, N);
-    if (P.tlas && P.modelSkip) return launch(N, Y, Y);
-    return ext ? launch(N, Y, N) : launch(N, N, N);
 }
 
 // ANY: the occlusion kernels
 template <bool ANY = false>
 inline cudaError_t query_launch(const DevParams& P, const QueryParams& Q, int numSMs, cudaStream_t stream)
 {
-    return with_query_kernel(P, [&](auto S, auto X, auto T) {
+    return with_persistent_kernel(P, [&](auto S, auto X, auto T) {
         auto kernel = ANY ? k_trace_occlusion<S, X, T> : k_trace_rays<S, X, T>;
         return persistent_launch(kernel, QUERY_SMEM_BYTES, (Q.n + 31u) / 32u, P, Q, numSMs, stream);
     });
@@ -294,7 +275,7 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_trace_paths
 
 inline cudaError_t paths_launch(const DevParams& P, const PathParams& Q, int numSMs, cudaStream_t stream)
 {
-    return with_query_kernel(P, [&](auto S, auto X, auto T) {
+    return with_persistent_kernel(P, [&](auto S, auto X, auto T) {
         return persistent_launch(k_trace_paths<S, X, T>, QUERY_SMEM_BYTES, (Q.n + 31u) / 32u, P, Q, numSMs, stream);
     });
 }

@@ -22,6 +22,7 @@
 //     counts equal the oracle's.  What is removed is the re-read of a popped node (the stack carries the
 //     node's (start,count)) and the push/pop round trip of the near child.
 #pragma once
+#include <type_traits>
 #include "rt_device.cuh"
 
 namespace rtd {
@@ -540,7 +541,7 @@ __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wa
 
 // rtDispatchAdaptive: the selection's pixel list (P.pixelList, totalJobs = its length), one frame per pixel (kernels of their own, so
 // that the kernels above keep their code; TLAS = the many-model form, <false, true, true>).  Templates, instantiated where
-// wave_launch_list launches them: a plain kernel defined here changed the register numbering of the k_raytrace_wave_frames kernels.
+// wave_kernel names them: a plain kernel defined here changed the register numbering of the k_raytrace_wave_frames kernels.
 template <bool STATS, bool EXT, bool TLAS>
 __global__ void __launch_bounds__(WAVE_THREADS, RT_WAVE_MINBLOCKS) k_raytrace_wave_list(const __grid_constant__ DevParams P, const unsigned int totalJobs)
 {
@@ -580,121 +581,137 @@ inline int wave_chunks(int forced, int numSMs, unsigned long long pixels, int sa
     return c < 1 ? 1 : c;
 }
 
-template <bool S, bool X> inline cudaError_t wave_configure_one()
+// ---- choosing and launching a persistent kernel (kernels 1 and 2 here and in rt_kernel_pool.cuh, the query family in rt_kernel_query.cuh)
+
+// The instantiation <STATS, EXT, TLAS> of a persistent kernel, chosen here and nowhere else: the counting build walks every model like the
+// reference; the TLAS kernel when the scene has a TLAS and skipping is on; otherwise the extension family when an extension is active —
+// peer stores, the sphere accelerator, "extInstantiation" or staged tree tops (the plain instantiation carries none of them).  The query
+// family's launches come here with nPeers = smemPairs = 0 (queryParams), so for them ext is sphBvh || forceExt.  `launch` is called with
+// three std::integral_constant<bool, ...>.
+template <class Launch>
+inline cudaError_t with_persistent_kernel(const DevParams& P, Launch launch)
 {
-    return cudaFuncSetAttribute(k_raytrace_wave<S, X>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024);
+    std::true_type Y;
+    std::false_type N;
+    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;
+    if (P.countStats) return ext ? launch(Y, Y, N) : launch(Y, N, N);
+    if (P.tlas && P.modelSkip) return launch(N, Y, Y);
+    return ext ? launch(N, Y, N) : launch(N, N, N);
 }
+
+// A camera kernel's variant: `launch` is called with the form and with_persistent_kernel's <STATS, EXT, TLAS>, all std::integral_constants
+template <class Launch>
+inline cudaError_t with_camera_kernel(CameraForm form, const DevParams& P, Launch launch)
+{
+    return with_persistent_kernel(P, [&](auto S, auto X, auto T) {
+        if (form == FORM_LIST) return launch(std::integral_constant<CameraForm, FORM_LIST>(), S, X, T);
+        if (form == FORM_FRAMES) return launch(std::integral_constant<CameraForm, FORM_FRAMES>(), S, X, T);
+        return launch(std::integral_constant<CameraForm, FORM_PLAIN>(), S, X, T);
+    });
+}
+
+// Every variant with_camera_kernel can choose (most of them more than once), for the *_configure functions: the rule is run on every
+// combination of its inputs, so that no kernel a launch can pick is left without its shared-memory limit
+template <class Launch>
+inline cudaError_t for_each_camera_kernel(Launch launch)
+{
+    DevParams P = {};
+    for (int in = 0; in < 24; in++)
+    {
+        P.countStats = in & 1; P.tlas = P.modelSkip = (in >> 1) & 1; P.forceExt = (in >> 2) & 1;
+        const cudaError_t e = with_camera_kernel((CameraForm)(in >> 3), P, launch);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+// The rows among the first limY that the bands of bandRows rows, dealt round-robin to tileWorld ranks, give to `rank`
+inline unsigned int owned_rows(unsigned int limY, int bandRows, int tileWorld, int rank)
+{
+    unsigned int rows = 0;
+    for (unsigned int y0 = 0, b = 0; y0 < limY; y0 += (unsigned int)bandRows, b++)
+        if ((int)(b % (unsigned int)tileWorld) == rank) rows += limY - y0 < (unsigned int)bandRows ? limY - y0 : (unsigned int)bandRows;
+    return rows;
+}
+
+// The camera kernels' jobs over limX x rows pixels: 32 per 8 x 4-pixel tile, tiles cut off at the region's edges included
+inline unsigned long long tile_jobs(unsigned int limX, unsigned int rows)
+{
+    return (unsigned long long)((limX + 7u) / 8u) * ((rows + 3u) / 4u) * 32ull;
+}
+
+// The jobs of a launch of kernel 1 or 2: the `listCount` pixels of a list (FORM_LIST), or the tiles of P's region in this rank's bands.
+// False when the tiles' jobs would not fit the 32-bit work counter, which every resident lane draws from once more after the last job.
+struct CameraJobs { unsigned int total = 0, tilesX = 0, ownedRows = 0; };
+inline bool camera_jobs(CameraForm form, const DevParams& P, unsigned int listCount, CameraJobs& J)
+{
+    if (form == FORM_LIST) { J.total = listCount; return true; }
+    J.ownedRows = owned_rows(P.limY, P.bandRows, P.tileWorld, P.tileRank);
+    J.tilesX = (P.limX + 7u) / 8u;
+    const unsigned long long jobs = tile_jobs(P.limX, J.ownedRows);
+    if (jobs >= 0xffff0000ull) return false;
+    J.total = (unsigned int)jobs;
+    return true;
+}
+
+// The grid of a persistent launch of kernel 1 or of the query family: as many CTAs as fit on every SM (a multiple of the SM count), but
+// no more than warpsNeeded warps fill (at least one)
+template <class Kernel>
+inline cudaError_t persistent_grid(Kernel kernel, size_t smemBytes, unsigned int warpsNeeded, int numSMs, unsigned int& grid)
+{
+    int ctasPerSM = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, kernel, WAVE_THREADS, smemBytes);
+    if (e != cudaSuccess) return e;
+    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
+    grid = (unsigned int)(numSMs * ctasPerSM);
+    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
+    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
+    return cudaSuccess;
+}
+
+// Kernel 1's table: the __global__ of form F and <STATS, EXT, TLAS>.  CHUNKED: sample chunks (P.chunks > 1, the plain form only), which
+// live in instantiations of their own, <STATS, true, false, CHUNKED>; the TLAS kernel carries the hand-off itself.
+template <CameraForm F, bool S, bool X, bool T, bool CHUNKED>
+inline auto wave_kernel()
+{
+    if constexpr (F == FORM_LIST) return k_raytrace_wave_list<S, X, T>;
+    else if constexpr (F == FORM_FRAMES && T) return k_raytrace_wave_tlas_frames;
+    else if constexpr (F == FORM_FRAMES) return k_raytrace_wave_frames<S, X>;
+    else if constexpr (T) return k_raytrace_wave_tlas;
+    else if constexpr (CHUNKED) return k_raytrace_wave<S, true, true>;
+    else return k_raytrace_wave<S, X>;
+}
+
 inline cudaError_t wave_configure()
 {
-    cudaError_t e;
-    if ((e = wave_configure_one<false, false>()) != cudaSuccess) return e;
-    if ((e = wave_configure_one<true, false>()) != cudaSuccess) return e;
-    if ((e = wave_configure_one<false, true>()) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_tlas, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_frames<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_tlas_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_raytrace_wave_list<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024)) != cudaSuccess) return e;
-    return wave_configure_one<true, true>();
+    return for_each_camera_kernel([](auto F, auto S, auto X, auto T) {
+        const cudaError_t e = cudaFuncSetAttribute(wave_kernel<F, S, X, T, false>(), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024);
+        return e != cudaSuccess ? e : cudaFuncSetAttribute(wave_kernel<F, S, X, T, true>(), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024);
+    });
 }
 
-// F = the batch kernels of rtDispatchFrames (k_raytrace_wave_frames, k_raytrace_wave_tlas_frames)
-template <bool S, bool X, bool T = false, bool C = false, bool F = false> inline cudaError_t wave_launch_one(const DevParams& P, int numSMs, size_t smemBytes, unsigned totalJobs, unsigned tilesX, unsigned ownedRows,
-                                                             cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
+// Kernel 1 over one dispatch in `form`; FORM_LIST: over the `count` pixels of `list`, whose moments its writes update (both reach the
+// kernel in P's parameter slots)
+inline cudaError_t wave_launch(CameraForm form, DevParams P, int numSMs, unsigned int count, const unsigned int* list, float4* moments,
+                               cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
 {
-    int ctasPerSM = 0;
-    cudaError_t e = F ? (T ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_tlas_frames, WAVE_THREADS, smemBytes)
-                           : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_frames<S, X>, WAVE_THREADS, smemBytes))
-                      : T ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_tlas, WAVE_THREADS, smemBytes)
-                      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave<S, X, C>, WAVE_THREADS, smemBytes);
-    if (e != cudaSuccess) return e;
-    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);                  // persistent: a multiple of the SM count
-    const unsigned int warpsNeeded = (totalJobs + 31u) / 32u;      // (whole pixels: a chunk of a pixel cannot run beside the chunk before it)
-    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    grid = fit_persistent_grid(P.gridFit, grid, WAVE_THREADS, totalJobs);
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
-    if (F && T) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, k_raytrace_wave_tlas_frames, P, totalJobs, tilesX, ownedRows);
-    else if (F) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_raytrace_wave_frames<S, X>), P, totalJobs, tilesX, ownedRows);
-    else if (T) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, k_raytrace_wave_tlas, P, totalJobs, tilesX, ownedRows);
-    else RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_raytrace_wave<S, X, C>), P, totalJobs, tilesX, ownedRows);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return cudaEventRecord(evB, stream);
-}
-
-inline cudaError_t wave_launch(const DevParams& P, int numSMs, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
-{
-    // rows of this rank's bands inside the dispatched region
-    unsigned int ownedRows = 0;
-    for (unsigned int y0 = 0, b = 0; y0 < P.limY; y0 += (unsigned int)P.bandRows, b++)
-        if ((int)(b % (unsigned int)P.tileWorld) == P.tileRank) ownedRows += (P.limY - y0) < (unsigned int)P.bandRows ? (P.limY - y0) : (unsigned int)P.bandRows;
-    const unsigned int tilesX = (P.limX + 7u) / 8u;
-    const unsigned int tileRows = (ownedRows + 3u) / 4u;
-    const unsigned long long jobs64 = (unsigned long long)tilesX * tileRows * 32ull;
-    if (jobs64 >= 0xffff0000ull) return cudaErrorInvalidValue;
-    const unsigned int totalJobs = (unsigned int)jobs64;
-
+    CameraJobs J;
+    if (!camera_jobs(form, P, count, J)) return cudaErrorInvalidValue;
+    if (form == FORM_LIST) { P.pixelList = list; P.adaptiveMoments = moments; }       // (the hand-off's and the cold pool's slots: unused here)
     const size_t smemBytes = sizeof(WaveSmemHeader) + (size_t)P.smemPairs * sizeof(NodePair) + (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
-    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;   // extensions (peer stores, sphere accelerator, staged tree tops) compiled into their own instantiation
-    // a batch of frames (rtDispatchFrames, P.frames > 1, whole pixels): the FRAMES kernels, chosen like the single-frame ones
-    if (P.frames > 1)
-    {
-        if (P.countStats) return ext ? wave_launch_one<true, true, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
-                                     : wave_launch_one<true, false, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-        if (P.tlas && P.modelSkip) return wave_launch_one<false, true, true, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-        return ext ? wave_launch_one<false, true, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
-                   : wave_launch_one<false, false, false, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-    }
-    // sample chunks (P.chunks > 1, small tiles): the hand-off lives in instantiations of its own (the extension family and the TLAS kernel)
-    if (P.chunks > 1 && !(P.tlas && P.modelSkip && !P.countStats))
-        return P.countStats ? wave_launch_one<true, true, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
-                            : wave_launch_one<false, true, false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-    if (P.countStats) return ext ? wave_launch_one<true, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
-                                 : wave_launch_one<true, false>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-    if (P.tlas && P.modelSkip) return wave_launch_one<false, true, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-    return ext ? wave_launch_one<false, true>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB)
-               : wave_launch_one<false, false>(P, numSMs, smemBytes, totalJobs, tilesX, ownedRows, stream, evA, evB);
-}
-
-// rtDispatchAdaptive: kernel 1 over the `count` pixels of P.pixelList, sized and chosen like wave_launch's whole-pixel kernels
-template <bool S, bool X, bool T> inline cudaError_t wave_launch_list_one(const DevParams& P, int numSMs, size_t smemBytes, unsigned count,
-                                                                          cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
-{
-    int ctasPerSM = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctasPerSM, k_raytrace_wave_list<S, X, T>, WAVE_THREADS, smemBytes);
-    if (e != cudaSuccess) return e;
-    if (ctasPerSM < 1) return cudaErrorInvalidConfiguration;
-    unsigned int grid = (unsigned int)(numSMs * ctasPerSM);
-    const unsigned int warpsNeeded = (count + 31u) / 32u;
-    const unsigned int ctasNeeded = (warpsNeeded + (WAVE_THREADS / 32) - 1) / (WAVE_THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded ? ctasNeeded : 1;
-    grid = fit_persistent_grid(P.gridFit, grid, WAVE_THREADS, count);
-    if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
-    if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
-    RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, RT_K(k_raytrace_wave_list<S, X, T>), P, count);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return cudaEventRecord(evB, stream);
-}
-
-inline cudaError_t wave_launch_list(const DevParams& P, int numSMs, unsigned count, cudaStream_t stream, cudaEvent_t evA, cudaEvent_t evB)
-{
-    const size_t smemBytes = sizeof(WaveSmemHeader) + (size_t)P.smemPairs * sizeof(NodePair) + (size_t)WAVE_MAX_SMEM_SPHERES * sizeof(DevSphere);
-    const bool ext = P.nPeers > 0 || P.sphBvh != 0 || P.forceExt != 0 || P.smemPairs > 0;
-    if (P.countStats) return ext ? wave_launch_list_one<true, true, false>(P, numSMs, smemBytes, count, stream, evA, evB)
-                                 : wave_launch_list_one<true, false, false>(P, numSMs, smemBytes, count, stream, evA, evB);
-    if (P.tlas && P.modelSkip) return wave_launch_list_one<false, true, true>(P, numSMs, smemBytes, count, stream, evA, evB);
-    return ext ? wave_launch_list_one<false, true, false>(P, numSMs, smemBytes, count, stream, evA, evB)
-               : wave_launch_list_one<false, false, false>(P, numSMs, smemBytes, count, stream, evA, evB);
+    return with_camera_kernel(form, P, [&](auto F, auto S, auto X, auto T) -> cudaError_t {
+        const auto kernel = P.chunks > 1 ? wave_kernel<F, S, X, T, true>() : wave_kernel<F, S, X, T, false>();
+        unsigned int grid = 0;
+        cudaError_t e = persistent_grid(kernel, smemBytes, (J.total + 31u) / 32u, numSMs, grid);      // (whole pixels: a chunk of a pixel cannot run beside the chunk before it)
+        if (e != cudaSuccess) return e;
+        grid = fit_persistent_grid(P.gridFit, grid, WAVE_THREADS, J.total);
+        if ((e = cudaMemsetAsync(P.workCounter, 0, sizeof(unsigned int), stream)) != cudaSuccess) return e;
+        if ((e = cudaEventRecord(evA, stream)) != cudaSuccess) return e;
+        if constexpr (F == FORM_LIST) RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, J.total);
+        else RT_LAUNCH(grid, WAVE_THREADS, smemBytes, stream, kernel, P, J.total, J.tilesX, J.ownedRows);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        return cudaEventRecord(evB, stream);
+    });
 }
 
 } // namespace rtd
