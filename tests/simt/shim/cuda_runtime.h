@@ -14,6 +14,9 @@
 // until every non-exited lane named in its mask has arrived; __syncthreads likewise for the CTA.  Divergent lanes really
 // do run at different times, so a missing __syncwarp or a collective under divergent control flow shows up as a wrong
 // result or a reported deadlock instead of passing by luck.
+//
+// Launches follow the H100's shared-memory rule: one above 48 KB of dynamic shared memory runs only if cudaFuncSetAttribute gave the
+// kernel that much, and every launch that runs is logged as (kernel, bytes) for tests/test_simt_kernel_matrix.py.
 #pragma once
 #ifndef RT_SIMT_EMU
 #error "tests/simt/shim/cuda_runtime.h is only for the RT_SIMT_EMU test build"
@@ -29,6 +32,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
@@ -62,6 +66,7 @@ static inline int2 make_int2(int x, int y) { int2 r; r.x = x; r.y = y; return r;
 static inline uchar4 make_uchar4(unsigned char x, unsigned char y, unsigned char z, unsigned char w) { uchar4 r; r.x = x; r.y = y; r.z = z; r.w = w; return r; }
 
 #include "simt_core.h"
+#include <cxxabi.h>
 
 // ---- built-in variables (per fiber; refreshed by the scheduler at every switch) -------------------------------------------------
 #define threadIdx (simt::tl_threadIdx)
@@ -150,7 +155,9 @@ static inline const char* cudaGetErrorString(cudaError_t e)
     switch (e) { case 0: return "no error"; case 1: return "invalid value"; case 2: return "out of memory"; case 9: return "invalid configuration";
                  case 801: return "not supported by the SIMT test build"; default: return "error"; }
 }
-static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
+// The error a refused launch leaves pending for the launching host thread (per thread, as the runtime keeps it)
+namespace simt { inline thread_local cudaError_t tl_lastError = cudaSuccess; }
+static inline cudaError_t cudaGetLastError() { const cudaError_t e = simt::tl_lastError; simt::tl_lastError = cudaSuccess; return e; }
 static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 8; return cudaSuccess; }          // eight "devices" sharing the host's memory: lets rtCreateMulti groups run here
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int)
@@ -191,7 +198,20 @@ static inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEve
 {
     *ms = std::chrono::duration<float, std::milli>(b->t - a->t).count(); return cudaSuccess;
 }
-template <class F> static inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }
+// cudaFuncAttributeMaxDynamicSharedMemorySize is recorded per function: simt::launch_kernel refuses a launch above 48 KB of dynamic
+// shared memory that the function was not given, as the H100 does (the other attributes the product does not set)
+namespace simt {
+inline std::mutex attrMutex;
+inline std::map<const void*, size_t> maxDynamicSmem;
+}
+template <class F> static inline cudaError_t cudaFuncSetAttribute(F f, int attr, int value)
+{
+    if (attr != cudaFuncAttributeMaxDynamicSharedMemorySize) return cudaErrorInvalidValue;
+    if (value < 0 || value > 232448) return cudaErrorInvalidValue;
+    std::lock_guard<std::mutex> lock(simt::attrMutex);
+    simt::maxDynamicSmem[reinterpret_cast<const void*>(f)] = (size_t)value;
+    return cudaSuccess;
+}
 template <class F> static inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* n, F, int, size_t) { *n = simt::env_int("RT_SIMT_CTAS_PER_SM", 2); return cudaSuccess; }
 static inline cudaError_t cudaIpcGetMemHandle(cudaIpcMemHandle_t*, void*) { return cudaErrorNotSupported; }
 static inline cudaError_t cudaIpcOpenMemHandle(void**, cudaIpcMemHandle_t, unsigned int) { return cudaErrorNotSupported; }
@@ -200,7 +220,66 @@ static inline cudaError_t cudaGetDriverEntryPoint(const char*, void** fn, unsign
 
 // ---- kernel launch ------------------------------------------------------------------------------------------------------------
 #define RT_DYNAMIC_SMEM(name) unsigned char* const name = rtd::simtSmem
-#define RT_LAUNCH(grid, block, smem, stream, kern, ...) simt::launch(dim3(grid), dim3(block), (size_t)(smem), [&]() { kern(__VA_ARGS__); })
+// A launch runs only when its dynamic shared memory is at most 48 KB or at most what cudaFuncSetAttribute gave the kernel; otherwise
+// it leaves cudaErrorInvalidValue for cudaGetLastError, as the H100 does.  Every launch that runs is logged as (kernel's demangled
+// symbol, dynamic shared-memory bytes) for the tests that check which instantiation a call chose (simtLaunchLog* below).
+namespace simt {
+constexpr size_t DEFAULT_DYNAMIC_SMEM = 48 * 1024;
+struct LaunchRecord { std::string symbol; size_t smem; };
+inline std::mutex logMutex;
+inline std::vector<LaunchRecord> launchLog;
+
+inline std::string kernel_symbol(const void* kern)
+{
+    Dl_info info; memset(&info, 0, sizeof(info));
+    if (!dladdr(kern, &info) || !info.dli_sname || info.dli_saddr != kern) return "?";
+    int status = 0;
+    char* d = abi::__cxa_demangle(info.dli_sname, nullptr, nullptr, &status);
+    std::string out = status == 0 && d ? d : info.dli_sname;
+    free(d);
+    return out;
+}
+
+inline void launch_kernel(const void* kern, dim3 grid, dim3 block, size_t smemBytes, const std::function<void()>& body)
+{
+    if (smemBytes > DEFAULT_DYNAMIC_SMEM)
+    {
+        std::lock_guard<std::mutex> lock(attrMutex);
+        const auto it = maxDynamicSmem.find(kern);
+        if (it == maxDynamicSmem.end() || smemBytes > it->second) { tl_lastError = cudaErrorInvalidValue; return; }
+    }
+    {
+        LaunchRecord r{kernel_symbol(kern), smemBytes};
+        std::lock_guard<std::mutex> lock(logMutex);
+        launchLog.push_back(std::move(r));
+    }
+    launch(grid, block, smemBytes, body);
+}
+} // namespace simt
+
+// The launch log, for the tests only (the product's ABI has no such calls): the number of records, record i's symbol and shared
+// memory, and a reset
+extern "C" __attribute__((visibility("default"))) size_t simtLaunchLogCount()
+{
+    std::lock_guard<std::mutex> lock(simt::logMutex);
+    return simt::launchLog.size();
+}
+extern "C" __attribute__((visibility("default"))) size_t simtLaunchLogEntry(size_t i, char* symbol, size_t cap)
+{
+    std::lock_guard<std::mutex> lock(simt::logMutex);
+    if (i >= simt::launchLog.size()) return 0;
+    const simt::LaunchRecord& r = simt::launchLog[i];
+    if (cap) { const size_t n = std::min(cap - 1, r.symbol.size()); memcpy(symbol, r.symbol.data(), n); symbol[n] = 0; }
+    return r.smem;
+}
+extern "C" __attribute__((visibility("default"))) void simtLaunchLogReset()
+{
+    std::lock_guard<std::mutex> lock(simt::logMutex);
+    simt::launchLog.clear();
+}
+
+#define RT_LAUNCH(grid, block, smem, stream, kern, ...) \
+    simt::launch_kernel(reinterpret_cast<const void*>(kern), dim3(grid), dim3(block), (size_t)(smem), [&]() { kern(__VA_ARGS__); })
 
 // ---- dynamic shared memory + the PTX helpers of rt_kernel_wave.cuh (mbarrier / TMA bulk copy), by their semantics ----------------
 namespace rtd {
