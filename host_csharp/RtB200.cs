@@ -90,6 +90,13 @@ public static class RtB200
     public struct CubeTexel { public UnityEngine.Vector3 rgb; public uint rejected; }
     [DllImport(Lib)] public static extern int rtBakeCubemaps(IntPtr ctx, UnityEngine.Vector3[] positions, int n, int faceSize, int samples, uint seed, [Out] CubeTexel[] output);
     [DllImport(Lib)] public static extern int rtBakeCubemapsDevice(IntPtr ctx, IntPtr dPositions, IntPtr dOut, int n, int faceSize, int samples, uint seed);
+    // lightmaps: per surface texel (world position and normal; the normal need not be unit length) the mean of `samples` paths over the
+    // normal's cosine-weighted hemisphere, output[p].rgb an estimate of E / pi (multiply by the surface's diffuse colour); rejected as
+    // for cube maps.  INTEGRATION.md shows how Mesh.uv2 atlas texels become SurfacePoints.
+    [StructLayout(LayoutKind.Sequential)]
+    public struct SurfacePoint { public UnityEngine.Vector3 position; public UnityEngine.Vector3 normal; }
+    [DllImport(Lib)] public static extern int rtBakeLightmap(IntPtr ctx, SurfacePoint[] points, int n, int samples, uint seed, [Out] CubeTexel[] output);
+    [DllImport(Lib)] public static extern int rtBakeLightmapDevice(IntPtr ctx, IntPtr dPoints, IntPtr dOut, int n, int samples, uint seed);
     // one pixel of "FeatureFrame": object = ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1 (dst = +inf, the rest 0)
     [StructLayout(LayoutKind.Sequential)]
     public struct PixelFeatures { public UnityEngine.Vector3 albedo; public float dst; public UnityEngine.Vector3 normal; public int objectId; }

@@ -264,6 +264,42 @@ int rtBakeProbesDevice(RtContext* ctx, const void* dPositions, void* dOut, int n
 int rtBakeCubemaps(RtContext* ctx, const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out);
 int rtBakeCubemapsDevice(RtContext* ctx, const void* dPositions, void* dOut, int n, int faceSize, int samples, uint32_t seed);
 
+/* Extension: lightmap baking.  For each of n surface texels, the diffuse lighting arriving at points[p].position over the hemisphere of
+ * points[p].normal: out[p].rgb is the mean of S = samples paths along a cosine-weighted set of directions, an estimate of E / pi, the
+ * radiance a white Lambertian surface at the texel reflects (multiply by a diffuse colour for that surface's baked lighting; the
+ * irradiance is pi * rgb).  It is the expected value of what the reference's own diffuse bounce (HL:524-525, normalize(normal +
+ * RandomDirection), cosine-distributed) gathers there.  Every bit is stated; each operation is one IEEE binary32 operation in the order
+ * written (no contraction); H(x) is the value NextRandom (HL:127-133) returns from state x; p is the texel's index in the call.
+ *   - Normal: m = points[p].normal;  n = m * (1 / sqrt(dot(m, m))), the dot summed left to right.  Normals are not validated: a zero,
+ *     denormal-underflowing or non-finite normal gives the NaN directions Trace makes of it.
+ *   - Tangent frame (Duff et al. 2017, "Building an Orthonormal Basis, Revisited"):
+ *         sg = copysign(1, n.z);  a = -1 / (sg + n.z);  b = (n.x * n.y) * a
+ *         T = (1 + ((sg * n.x) * n.x) * a,  sg * b,  -(sg * n.x));  B = (b,  sg + (n.y * n.y) * a,  -n.y)
+ *   - Direction of sample k: (u, v) the R2 point of rtBakeCubemaps (the same constants; k = 0 at (0.5, 0.5)), with no RNG draw;
+ *         r = sqrt(u);  (s, c) = (sin, cos)(v * 6.28318548f) as RandomPointInCircle computes them (rt_devmath.cuh sincos_rt);
+ *         x = r * c;  y = r * s;  z = sqrt(max(1 - u, 0));  d = normalize(w), w.i = (T.i * x + B.i * y) + n.i * z
+ *     with normalize as rtBakeCubemaps': a cosine-weighted hemisphere around n.
+ *   - Origin: o = points[p].position + (n * 0.001f), the offset of the reference's diffuse bounce (HL:524, epsilon of HL:468).
+ *   - Paths:  L = Trace(CreateRay(o, d, 1, 0), state = H(H(seed + p) + k))        (HL:439-448, HL:479-542)
+ *     so a sample is rtTracePaths({o, d, H(H(seed + p) + k)}, samples = 1).rgb bit for bit.
+ *   - Sums: rtBakeCubemaps': chunks of RT_PROBE_CHUNK consecutive k, each summing L from +0 in k order; a sample with any non-finite
+ *     component adds nothing and counts in `rejected`; the chunks combined by the full binary tree over the chunk count padded with +0
+ *     chunks to a power of two, and out.rgb = tree / (float)S.
+ *   - Everything else is rtBakeCubemaps': what it reads and leaves alone (no camera, "Frame", "renderSeed", "NumRaysPerPixel" or
+ *     "Resolution"; no rtResize needed), RtStats.rays growing by segments and the countStats counters, the per-segment gate of model
+ *     skipping, the TLAS and the sphere accelerator, devices[0] on a group context, the "MaxBounceCount" and scene-check refusals.
+ *     Positions are not validated: a far or NaN origin fails the gate and walks every model.
+ *   - Launches: a call runs its texels in launches of floor(RT_CUBE_SCRATCH_CHUNKS / ceil(S / RT_PROBE_CHUNK)) texels, rtBakeCubemaps'
+ *     rule, through rtBakeProbes' device scratch at 16 bytes per chunk.  The launches change no bits: p is the index in the call.
+ * Refused: ctx NULL, n < 0, points / out NULL with n > 0, samples < 1 or > RT_MAX_BATCH_SAMPLES, a device dPoints not 4-byte or dOut
+ * not 16-byte aligned -> RT_E_INVALID; rtBakeCubemaps' RT_E_STATE cases -> RT_E_STATE.  n = 0 is RT_OK and launches nothing.
+ * rtBakeLightmap: host arrays, in batches of at most RT_TRACE_CHUNK_RAYS texels through the two device buffers rtTraceRays keeps (points
+ * in the ray buffer, 24 of its 24 bytes; texels in the hit buffer, 16 of its 48), so a 4096^2 atlas needs no more device memory than
+ * one batch; synchronises.  rtBakeLightmapDevice: n RtSurfacePoint and n RtCubeTexel in device memory of the context's device;
+ * allocates only the scratch; asynchronous on the context's stream (rtSetStream). */
+int rtBakeLightmap(RtContext* ctx, const RtSurfacePoint* points, int n, int samples, uint32_t seed, RtCubeTexel* out);
+int rtBakeLightmapDevice(RtContext* ctx, const void* dPoints, void* dOut, int n, int samples, uint32_t seed);
+
 /* Extension: first-hit feature images for denoisers (albedo, shading normal, depth, object id: the guides OIDN, a-trous / SVGF filters
  * and mattes take next to the colour), and the camera's own rays.
  *

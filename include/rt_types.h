@@ -128,6 +128,13 @@ typedef struct RtCubeTexel {
     uint32_t rejected;     /* samples whose radiance was not finite and were left out of the sum (they count as black) */
 } RtCubeTexel;
 
+/* One texel of rtBakeLightmap / rtBakeLightmapDevice (include/rt_b200.h): a point on a surface and the normal that sets its
+ * hemisphere (world space; the normal need not be unit length).  The baked value is an RtCubeTexel.  24 bytes. */
+typedef struct RtSurfacePoint {
+    float position[3];
+    float normal[3];
+} RtSurfacePoint;
+
 /* One pixel of rtDispatchFeatures' "FeatureFrame" (include/rt_b200.h): what the pixel's feature ray hits first.  32 bytes. */
 typedef struct RtPixelFeatures {
     float   albedo[3];    /* (0, 0, 0) on a miss; (1, 1, 1) for glass; GetMaterialColour (HL:450-466) otherwise */
@@ -149,6 +156,7 @@ static_assert(sizeof(RtPathRadiance) == 16, "RtPathRadiance record");
 static_assert(sizeof(RtPixelFeatures) == 32, "RtPixelFeatures record");
 static_assert(sizeof(RtProbeSH) == 112, "RtProbeSH record");
 static_assert(sizeof(RtCubeTexel) == 16, "RtCubeTexel record");
+static_assert(sizeof(RtSurfacePoint) == 24, "RtSurfacePoint record");
 static_assert(sizeof(RtNode) == 32, "BVHNode stride");
 static_assert(sizeof(RtTriangle) == 72, "Triangle stride");
 static_assert(sizeof(RtMaterial) == 88, "RayTracingMaterial stride");

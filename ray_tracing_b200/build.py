@@ -99,10 +99,11 @@ def build_oracle(force: bool = False) -> str:
     # history around that (tests/oracle_ext/rt_oracle_temporal.cpp); rtDispatchAdaptive is the selection on its moments and Kernel_RayTrace
     # per active pixel around that (tests/oracle_ext/rt_oracle_adaptive.cpp); rtBakeProbes is Shader::Trace per probe sample, its SH
     # chunk sums and their padded tree around that (tests/oracle_ext/rt_oracle_probes.cpp); rtBakeCubemaps is Shader::Trace per texel
-    # sample, its chunk sums and their padded tree around that (tests/oracle_ext/rt_oracle_cubemaps.cpp, the translation unit built here)
+    # sample, its chunk sums and their padded tree around that (tests/oracle_ext/rt_oracle_cubemaps.cpp); rtBakeLightmap is Shader::Trace
+    # per surface-texel sample and the same sums around that (tests/oracle_ext/rt_oracle_lightmaps.cpp, the translation unit built here)
     srcs = _glob(ORACLE, (".cpp", ".h")) + _glob(ORACLE_EXT, (".cpp",)) + _glob(INCLUDE, (".h",))
     if force or _newer(LIB_ORACLE, srcs):
-        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_cubemaps.cpp")])
+        _run([os.environ.get("CXX", "g++")] + GXX_FLAGS + ["-I", INCLUDE, "-o", LIB_ORACLE, os.path.join(ORACLE_EXT, "rt_oracle_lightmaps.cpp")])
     return LIB_ORACLE
 
 

@@ -131,6 +131,17 @@ assert CUBE_TEXEL_DTYPE.itemsize == 16
 RT_CUBE_MAX_FACE = 4096
 RT_CUBE_SCRATCH_CHUNKS = 7 << 20
 
+# rtBakeLightmap: one surface texel (RtSurfacePoint); its result is a CUBE_TEXEL_DTYPE record
+SURFACE_POINT_DTYPE = np.dtype([("position", "<f4", 3), ("normal", "<f4", 3)])
+assert SURFACE_POINT_DTYPE.itemsize == 24
+
+
+def as_surface_points(points) -> np.ndarray:
+    """An (n,) SURFACE_POINT_DTYPE array as given, or (n, 6) floats (position, normal) as one; contiguous."""
+    if isinstance(points, np.ndarray) and points.dtype == SURFACE_POINT_DTYPE:
+        return np.ascontiguousarray(points.reshape(-1))
+    return np.ascontiguousarray(np.asarray(points, dtype=np.float32).reshape(-1, 6)).view(SURFACE_POINT_DTYPE).reshape(-1)
+
 
 # rtDispatchFeatures: one pixel of "FeatureFrame" (RtPixelFeatures).  object: ModelInfo index m -> m, Spheres index s -> -2 - s, miss -> -1
 PIXEL_FEATURES_DTYPE = np.dtype([("albedo", "<f4", 3), ("dst", "<f4"), ("normal", "<f4", 3), ("object", "<i4")])
@@ -230,6 +241,8 @@ class RtLib:
             "rtBakeProbesDevice": ([vp, vp, vp, ci, ci, C.c_uint32], ci),
             "rtBakeCubemaps": ([vp, vp, ci, ci, ci, C.c_uint32, vp], ci),
             "rtBakeCubemapsDevice": ([vp, vp, vp, ci, ci, ci, C.c_uint32], ci),
+            "rtBakeLightmap": ([vp, vp, ci, ci, C.c_uint32, vp], ci),
+            "rtBakeLightmapDevice": ([vp, vp, vp, ci, ci, C.c_uint32], ci),
             "rtDispatchFeatures": ([vp, ci, ci, ci], ci),
             "rtCameraRays": ([vp, vp, C.c_size_t], ci),
             "rtCameraRaysDevice": ([vp, vp, C.c_size_t], ci),
@@ -244,7 +257,7 @@ class RtLib:
                 if name in ("rtGetIpcHandles", "rtSetPeers", "rtBuildBVH", "rtCreateMulti", "rtGetUniqueId", "rtCommInit", "rtCommDestroy", "rtExchangeTiles", "rtReadbackAsync", "rtDisplayAsync", "rtReadbackWait",
                             "rtReadbackPixelStats", "rtDisplayPixelStats", "rtDispatchFrames", "rtTraceRays", "rtTraceRaysDevice",
                             "rtTraceOcclusion", "rtTraceOcclusionDevice", "rtTracePaths", "rtTracePathsDevice",
-                            "rtBakeProbes", "rtBakeProbesDevice", "rtBakeCubemaps", "rtBakeCubemapsDevice", "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
+                            "rtBakeProbes", "rtBakeProbesDevice", "rtBakeCubemaps", "rtBakeCubemapsDevice", "rtBakeLightmap", "rtBakeLightmapDevice", "rtDispatchFeatures", "rtCameraRays", "rtCameraRaysDevice", "rtDenoise", "rtDisplayDenoised", "rtDenoiseTemporal",
                             "rtDispatchAdaptive", "rtDisplayMean"):      # absent from older experimental builds used in A/B runs
                     continue
                 raise AttributeError(f"{self.path} does not export {name}")
@@ -453,6 +466,23 @@ class RtContext:
         at out_ptr (16-byte aligned), both device memory of the context's GPU.  Asynchronous on the context's stream (set_stream)."""
         self._ck(self._L.rtBakeCubemapsDevice(self._h, C.c_void_p(positions_ptr), C.c_void_p(out_ptr), int(n), int(face_size), int(samples),
                                               int(seed) & 0xFFFFFFFF))
+
+
+    def bake_lightmap(self, points, samples: int, seed: int = 0) -> np.ndarray:
+        """rtBakeLightmap: the cosine-weighted lighting arriving at every surface texel (an (n,) SURFACE_POINT_DTYPE array, or (n, 6) floats
+        position then normal), each the mean of `samples` paths over the normal's hemisphere.  Returns an (n,) CUBE_TEXEL_DTYPE array:
+        "rgb" estimates E / pi (a white Lambertian surface's radiance), "rejected" the samples left out for a non-finite radiance."""
+        pts = as_surface_points(points)
+        out = np.empty(pts.shape[0], dtype=CUBE_TEXEL_DTYPE)
+        self._ck(self._L.rtBakeLightmap(self._h, pts.ctypes.data if pts.size else None, int(pts.shape[0]), int(samples),
+                                        int(seed) & 0xFFFFFFFF, out.ctypes.data if out.size else None))
+        return out
+
+    def bake_lightmap_device(self, points_ptr: int, out_ptr: int, n: int, samples: int, seed: int = 0):
+        """rtBakeLightmapDevice: n RtSurfacePoint (SURFACE_POINT_DTYPE, 24 bytes) at points_ptr (4-byte aligned) -> n RtCubeTexel
+        (CUBE_TEXEL_DTYPE, 16 bytes) at out_ptr (16-byte aligned), both device memory of the context's GPU.  Asynchronous on the
+        context's stream (set_stream)."""
+        self._ck(self._L.rtBakeLightmapDevice(self._h, C.c_void_p(points_ptr), C.c_void_p(out_ptr), int(n), int(samples), int(seed) & 0xFFFFFFFF))
 
     def dispatch_features(self, gx: Optional[int] = None, gy: Optional[int] = None, gz: int = 1):
         """rtDispatchFeatures: the first-hit feature images (albedo, dst, normal, object id) of every pixel's own camera ray of the

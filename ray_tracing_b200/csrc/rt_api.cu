@@ -1448,29 +1448,37 @@ static int cubemapArgs(RtContext* c, const char* what, const void* positions, co
     return RT_OK;
 }
 
-// Texels t0 .. t0 + n - 1 of the call (dPositions: the call's probes; dOut: texel t0's record), in device memory of this context's
-// GPU, in launches of at most texelsPerLaunch texels; asynchronous on the context's stream.  The scratch is allocated (or grown) here
-// and nothing else is.
-static int cubemapsLocal(RtContext* c, const float* dPositions, RtCubeTexel* dOut, int n, unsigned int t0, int faceSize, int samples, uint32_t seed)
+// Texels t0 .. t0 + n - 1 of a cube-map or lightmap call (Q: the call's parameters, with Q.points, if set, at texel t0's point) -> dOut,
+// in device memory of this context's GPU, in launches of at most texelsPerLaunch texels; asynchronous on the context's stream.  The
+// scratch is allocated (or grown) here and nothing else is.
+static int texelLaunches(RtContext* c, const char* what, CubeParams Q, RtCubeTexel* dOut, int n, unsigned int t0)
 {
-    int rc = bounceLimit(c, "rtBakeCubemaps"); if (rc != RT_OK) return rc;
-    if ((rc = prepareQueryScene(c, "rtBakeCubemaps")) != RT_OK) return rc;
-    const unsigned int chunks = ((unsigned int)samples + RT_PROBE_CHUNK - 1) / RT_PROBE_CHUNK;
-    const int per = texelsPerLaunch(samples);
+    int rc = bounceLimit(c, what); if (rc != RT_OK) return rc;
+    if ((rc = prepareQueryScene(c, what)) != RT_OK) return rc;
+    const unsigned int chunks = ((unsigned int)Q.samples + RT_PROBE_CHUNK - 1) / RT_PROBE_CHUNK;
+    const int per = texelsPerLaunch(Q.samples);
     const int first = n < per ? n : per;
     if (c->probeScratch.cap < (size_t)first * chunks * CUBE_WORDS) CK(c->probeScratch.ensure((size_t)first * chunks * CUBE_WORDS));
     const DevParams P = queryParams(c);
-    CubeParams Q = {};
-    Q.positions = dPositions; Q.scratch = c->probeScratch.p; Q.chunks = chunks; Q.faceSize = (unsigned int)faceSize;
-    Q.samples = samples; Q.seed = seed;
+    const RtSurfacePoint* points = Q.points;
+    Q.scratch = c->probeScratch.p; Q.chunks = chunks;
     Q.box = sceneBounds(c);
     for (int i0 = 0; i0 < n; i0 += per)
     {
         Q.out = dOut + i0; Q.n = (unsigned int)(n - i0 < per ? n - i0 : per); Q.t0 = t0 + (unsigned int)i0;
+        if (points) Q.points = points + i0;
         cudaError_t e = cubemaps_launch(P, Q, c->numSMs, c->stream);
-        if (e != cudaSuccess) return failCuda(c, e, "rtBakeCubemaps launch");
+        if (e != cudaSuccess) return failCuda(c, e, (std::string(what) + " launch").c_str());
     }
     return RT_OK;
+}
+
+// Texels t0 .. t0 + n - 1 of the call (dPositions: the call's probes; dOut: texel t0's record)
+static int cubemapsLocal(RtContext* c, const float* dPositions, RtCubeTexel* dOut, int n, unsigned int t0, int faceSize, int samples, uint32_t seed)
+{
+    CubeParams Q = {};
+    Q.positions = dPositions; Q.faceSize = (unsigned int)faceSize; Q.samples = samples; Q.seed = seed;
+    return texelLaunches(c, "rtBakeCubemaps", Q, dOut, n, t0);
 }
 
 // The positions go to the device once; the texels come back a launch at a time
@@ -1499,6 +1507,41 @@ int rtBakeCubemapsDevice(RtContext* c, const void* dPositions, void* dOut, int n
     if (n == 0) return RT_OK;
     CK(cudaSetDevice(c->device));
     return cubemapsLocal(c, (const float*)dPositions, (RtCubeTexel*)dOut, texels, 0u, faceSize, samples, seed);
+}
+
+// ---- lightmaps (rtBakeLightmap: surface texels of k_bake_cubemaps, rt_kernel_cubemaps.cuh) ---------------------------------------------
+// Texels p0 .. p0 + n - 1 of the call (dPoints, dOut: texel p0's point and record); the checks, scratch and launches of rtBakeCubemaps
+static int lightmapLocal(RtContext* c, const RtSurfacePoint* dPoints, RtCubeTexel* dOut, int n, unsigned int p0, int samples, uint32_t seed)
+{
+    CubeParams Q = {};
+    Q.points = dPoints; Q.samples = samples; Q.seed = seed;
+    return texelLaunches(c, "rtBakeLightmap", Q, dOut, n, p0);
+}
+
+// The points travel in queryRays (24 of its 24 bytes per record) and the texels in queryHits (16 of 48), so a lightmap batch needs no
+// memory beyond what a closest-hit batch of the same size keeps.
+int rtBakeLightmap(RtContext* c, const RtSurfacePoint* points, int n, int samples, uint32_t seed, RtCubeTexel* out)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = batchArgs(c, "rtBakeLightmap", "points", points, out, n, samples); if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    const int chunk = n < RT_TRACE_CHUNK_RAYS ? n : RT_TRACE_CHUNK_RAYS;
+    if ((rc = queryBuffers(c, chunk)) != RT_OK) return rc;
+    RtSurfacePoint* dPoints = reinterpret_cast<RtSurfacePoint*>(c->queryRays.p);
+    RtCubeTexel* dOut = reinterpret_cast<RtCubeTexel*>(c->queryHits.p);
+    return hostBatches(c, n, chunk, dPoints, points, sizeof(RtSurfacePoint), dOut, out, sizeof(RtCubeTexel),
+                       [&](int i0, int m) { return lightmapLocal(c, dPoints, dOut, m, (unsigned int)i0, samples, seed); });
+}
+
+int rtBakeLightmapDevice(RtContext* c, const void* dPoints, void* dOut, int n, int samples, uint32_t seed)
+{
+    if (!c) return RT_E_INVALID;
+    int rc = batchArgs(c, "rtBakeLightmapDevice", "points", dPoints, dOut, n, samples); if (rc != RT_OK) return rc;
+    if (((uintptr_t)dPoints & 3u) || ((uintptr_t)dOut & 15u)) return fail(c, RT_E_INVALID, "rtBakeLightmapDevice: dPoints must be 4-byte and dOut 16-byte aligned");
+    if (n == 0) return RT_OK;
+    CK(cudaSetDevice(c->device));
+    return lightmapLocal(c, (const RtSurfacePoint*)dPoints, (RtCubeTexel*)dOut, n, 0u, samples, seed);
 }
 
 // ---- first-hit feature images and the camera's own rays (rtDispatchFeatures, rtCameraRays, rt_kernel_features.cuh) ---------------------

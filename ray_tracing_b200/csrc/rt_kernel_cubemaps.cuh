@@ -1,4 +1,7 @@
-// rt_kernel_cubemaps.cuh — rtBakeCubemaps: HDR cube maps of path-traced radiance at probe positions (reflection probes).
+// rt_kernel_cubemaps.cuh — rtBakeCubemaps: HDR cube maps of path-traced radiance at probe positions (reflection probes), and
+// rtBakeLightmap: cosine-weighted path-traced lighting at surface texels.  A lightmap texel is a second kind of texel of the same two
+// kernels: only its origin and the direction of each sample differ (CubeJob::begin), chosen by CubeParams::points, which is uniform
+// across a launch.
 //
 // Two launches per batch of texels (include/rt_b200.h states the contract):
 //   k_bake_cubemaps  the path tracer's samples.  A job is one (texel, chunk) pair: RT_PROBE_CHUNK consecutive samples of one texel,
@@ -26,6 +29,7 @@ struct CubeParams
     int samples;                                 // 1 .. RT_MAX_BATCH_SAMPLES
     uint32_t seed;
     OriginBox box;
+    const RtSurfacePoint* points;                // rtBakeLightmap: the launch's first texel's point; nullptr for cube maps
 };
 
 // The direction of sample k of texel (x, y) of face f, one binary32 operation at a time (the contract in include/rt_b200.h)
@@ -49,8 +53,28 @@ RT_DI f3 CubeDirection(unsigned int f, unsigned int x, unsigned int y, unsigned 
     return normalize3(w);
 }
 
-// A job is one (texel, chunk) pair: samples k .. kEnd - 1 of texel tau = t0 + job / Q.chunks, each from CreateRay(position, d, 1, 0)
-// (HL:439-448) with state H(H(seed + tau) + k), summed into the lane's registers.
+// Sample k of a lightmap texel at (position P, normal M), one binary32 operation at a time (the contract in include/rt_b200.h): the
+// origin P + n * 0.001 and a cosine-weighted direction about n = normalize(M) through the R2 point (u, v), in Duff et al.'s frame
+RT_DI void SurfaceRay(f3 P, f3 M, unsigned int k, f3& origin, f3& dir)
+{
+    const float u = __uint2float_rn(k * 3242174889u + 2147483648u) * 2.3283064365386963e-10f;     // R2, as CubeDirection
+    const float v = __uint2float_rn(k * 2447445414u + 2147483648u) * 2.3283064365386963e-10f;
+    const f3 n = normalize3(M);
+    const float sg = copysignf(1.0f, n.z);
+    const float a = -1.0f / (sg + n.z);
+    const float b = (n.x * n.y) * a;
+    const f3 T = make_f3(1.0f + ((sg * n.x) * n.x) * a, sg * b, -(sg * n.x));
+    const f3 B = make_f3(b, sg + (n.y * n.y) * a, -n.y);
+    const float r = sqrtf(u);
+    float s, c; sincos_rt(v * 6.28318548f, s, c);
+    const float x = r * c, y = r * s, z = sqrtf(fmaxf(1.0f - u, 0.0f));
+    dir = normalize3(make_f3((T.x * x + B.x * y) + n.x * z, (T.y * x + B.y * y) + n.y * z, (T.z * x + B.z * y) + n.z * z));
+    origin = make_f3(P.x + n.x * 0.001f, P.y + n.y * 0.001f, P.z + n.z * 0.001f);
+}
+
+// A job is one (texel, chunk) pair: samples k .. kEnd - 1 of texel tau = t0 + job / Q.chunks, each from CreateRay(origin, d, 1, 0)
+// (HL:439-448) with state H(H(seed + tau) + k), summed into the lane's registers.  The origin is the probe's position (cube maps) or
+// the surface point lifted off its surface (lightmaps).
 struct CubeJob
 {
     const CubeParams& Q;
@@ -70,11 +94,19 @@ struct CubeJob
     }
     RT_DI void begin(PathState& ray, uint32_t& rngState) const
     {
-        const unsigned int N = Q.faceSize, t = tau();
-        const unsigned int row = t / N, x = t - row * N, face = row / N, y = row - face * N, p = face / 6u, f = face - p * 6u;
-        const float* o = Q.positions + 3u * p;
-        ray.pos = make_f3(__ldg(o), __ldg(o + 1), __ldg(o + 2));
-        ray.dir = CubeDirection(f, x, y, k, N);
+        if (Q.points)                                       // a lightmap texel: point job / chunks of the launch
+        {
+            const float* s = reinterpret_cast<const float*>(Q.points + job / Q.chunks);
+            SurfaceRay(make_f3(__ldg(s), __ldg(s + 1), __ldg(s + 2)), make_f3(__ldg(s + 3), __ldg(s + 4), __ldg(s + 5)), k, ray.pos, ray.dir);
+        }
+        else
+        {
+            const unsigned int N = Q.faceSize, t = tau();
+            const unsigned int row = t / N, x = t - row * N, face = row / N, y = row - face * N, p = face / 6u, f = face - p * 6u;
+            const float* o = Q.positions + 3u * p;
+            ray.pos = make_f3(__ldg(o), __ldg(o + 1), __ldg(o + 2));
+            ray.dir = CubeDirection(f, x, y, k, N);
+        }
         ray.transmittance = splat3(1.0f);
         ray.totalLight = splat3(0.0f);
         rngState = ProbeHash(texelKey + k);

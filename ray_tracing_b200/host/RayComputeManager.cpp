@@ -34,6 +34,7 @@ std::string RtApi::Load(const char* path)
     TracePaths = reinterpret_cast<decltype(TracePaths)>(dlsym(dl, "rtTracePaths"));
     BakeProbesFn = reinterpret_cast<decltype(BakeProbesFn)>(dlsym(dl, "rtBakeProbes"));
     BakeCubemapsFn = reinterpret_cast<decltype(BakeCubemapsFn)>(dlsym(dl, "rtBakeCubemaps"));
+    BakeLightmapFn = reinterpret_cast<decltype(BakeLightmapFn)>(dlsym(dl, "rtBakeLightmap"));
     DispatchFeatures = reinterpret_cast<decltype(DispatchFeatures)>(dlsym(dl, "rtDispatchFeatures"));
     CameraRaysFn = reinterpret_cast<decltype(CameraRaysFn)>(dlsym(dl, "rtCameraRays"));
     DenoiseFn = reinterpret_cast<decltype(DenoiseFn)>(dlsym(dl, "rtDenoise"));
@@ -370,6 +371,16 @@ int RayComputeManager::BakeCubemaps(const float* positions, int n, int faceSize,
     int rc;
     if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
     TRY(api.BakeCubemapsFn(ctx, positions, n, faceSize, samples, seed, out));
+    return RT_OK;
+}
+
+int RayComputeManager::BakeLightmap(const RtSurfacePoint* points, int n, int samples, uint32_t seed, RtCubeTexel* out)
+{
+    if (!ctx) return RT_E_STATE;
+    if (!api.BakeLightmapFn) { lastError = "the library does not export rtBakeLightmap"; return RT_E_STATE; }
+    int rc;
+    if ((rc = InitBVH()) != RT_OK || (rc = UpdateModels()) != RT_OK) return rc;
+    TRY(api.BakeLightmapFn(ctx, points, n, samples, seed, out));
     return RT_OK;
 }
 

@@ -62,6 +62,7 @@ struct RtApi
     decltype(&rtTracePaths) TracePaths = nullptr;           // optional: radiance along caller rays (TracePaths)
     decltype(&rtBakeProbes) BakeProbesFn = nullptr;         // optional: light probes (BakeProbes)
     decltype(&rtBakeCubemaps) BakeCubemapsFn = nullptr;     // optional: reflection probes (BakeCubemaps)
+    decltype(&rtBakeLightmap) BakeLightmapFn = nullptr;     // optional: lightmaps (BakeLightmap)
     decltype(&rtDispatchFeatures) DispatchFeatures = nullptr;   // optional: first-hit feature images (RenderFeatures)
     decltype(&rtCameraRays) CameraRaysFn = nullptr;         // optional: the camera's own rays (CameraRays)
     decltype(&rtDenoise) DenoiseFn = nullptr;               // optional: the a-trous denoiser (Denoise)
@@ -157,6 +158,9 @@ public:
     // not in the reference: reflection probes — an HDR cube map of the radiance at each of n positions, 6 faces of faceSize^2 texels,
     // each texel the mean of `samples` paths over its area (rtBakeCubemaps).  The scene is uploaded first as for TraceRays.
     int BakeCubemaps(const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out);
+    // not in the reference: lightmaps — the cosine-weighted lighting arriving at each of n surface texels (position, normal), each the
+    // mean of `samples` paths over the normal's hemisphere (rtBakeLightmap).  The scene is uploaded first as for TraceRays.
+    int BakeLightmap(const RtSurfacePoint* points, int n, int samples, uint32_t seed, RtCubeTexel* out);
     // not in the reference: the denoiser guides of the frame the NEXT RenderFrame() renders (rtDispatchFeatures over the whole image):
     // the upload sequence of RenderFrame, Frame = numAccumulatedFrames, and no step of the frame counter.  Call it right before that
     // RenderFrame; ResetAccumulatedRender resets the accumulated guides with the colour.

@@ -252,6 +252,9 @@ int rcmBakeProbes(void* hv, const float* positions, int n, int samples, uint32_t
 int rcmBakeCubemaps(void* hv, const float* positions, int n, int faceSize, int samples, uint32_t seed, RtCubeTexel* out)
 { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->BakeCubemaps(positions, n, faceSize, samples, seed, out); } CATCH_ALL(h) }
 
+int rcmBakeLightmap(void* hv, const RtSurfacePoint* points, int n, int samples, uint32_t seed, RtCubeTexel* out)
+{ Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->BakeLightmap(points, n, samples, seed, out); } CATCH_ALL(h) }
+
 int rcmRenderFeatures(void* hv) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->RenderFeatures(); } CATCH_ALL(h) }
 int rcmReadFeatureImage(void* hv, const char* name, void* dst, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); return h->mgr->ReadFeatureImage(name, dst, bytes); }
 int rcmCameraRays(void* hv, RtPathRay* rays, size_t bytes) { Handle* h = (Handle*)hv; GUARD(h); try { return h->mgr->CameraRays(rays, bytes); } CATCH_ALL(h) }

@@ -70,6 +70,7 @@ def host_lib() -> C.CDLL:
         L.rcmTracePaths.argtypes = [vp, vp, ci, ci, vp]
         L.rcmBakeProbes.argtypes = [vp, vp, ci, ci, C.c_uint32, vp]
         L.rcmBakeCubemaps.argtypes = [vp, vp, ci, ci, ci, C.c_uint32, vp]
+        L.rcmBakeLightmap.argtypes = [vp, vp, ci, ci, C.c_uint32, vp]
         L.rcmRenderFeatures.argtypes = [vp]
         L.rcmReadFeatureImage.argtypes = [vp, cp, vp, C.c_size_t]
         L.rcmCameraRays.argtypes = [vp, vp, C.c_size_t]
@@ -125,6 +126,23 @@ def load_obj(path: str, unity_handedness: bool = True):
 def column_major(m) -> np.ndarray:
     """4x4 (row, col) matrix -> 16 floats in Unity Matrix4x4 memory order."""
     return np.ascontiguousarray(np.asarray(m, dtype=np.float32).reshape(4, 4).T).reshape(16)
+
+
+def vertex_texels(vertices, normals, local_to_world) -> np.ndarray:
+    """One lightmap texel (capi.SURFACE_POINT_DTYPE) per vertex of a mesh placed by local_to_world (4x4, row, col): position
+    (M [v, 1]).xyz and normal normalize(M3x3 n), the shading normal of HL:367, each row summed left to right in binary32.  For meshes
+    without lightmap UVs (the reference's have none) this bakes vertex lighting; one texel per shared vertex leaves no seams."""
+    f = np.float32
+    M = np.asarray(local_to_world, dtype=f).reshape(4, 4)
+    v = np.asarray(vertices, dtype=f).reshape(-1, 3)
+    n = np.asarray(normals, dtype=f).reshape(-1, 3)
+    out = np.zeros(len(v), dtype=capi.SURFACE_POINT_DTYPE)
+    for r in range(3):
+        out["position"][:, r] = (((M[r, 0] * v[:, 0] + M[r, 1] * v[:, 1]) + M[r, 2] * v[:, 2]) + M[r, 3]).astype(f)
+        out["normal"][:, r] = ((M[r, 0] * n[:, 0] + M[r, 1] * n[:, 1]) + M[r, 2] * n[:, 2]).astype(f)
+    w = out["normal"]
+    out["normal"] = w * (f(1) / np.sqrt(((w[:, 0] * w[:, 0] + w[:, 1] * w[:, 1]) + w[:, 2] * w[:, 2]).astype(f)))[:, None]
+    return out
 
 
 class RayComputeManager:
@@ -364,6 +382,18 @@ class RayComputeManager:
         N = int(face_size)
         out = np.empty((pos.shape[0], 6, max(N, 0), max(N, 0)), dtype=capi.CUBE_TEXEL_DTYPE)
         self._ck(self._L.rcmBakeCubemaps(self._h, pos.ctypes.data if pos.size else None, int(pos.shape[0]), N, int(samples),
+                                         int(seed) & 0xFFFFFFFF, out.ctypes.data if out.size else None))
+        return out
+
+
+    # -- lightmaps (rtBakeLightmap): the cosine-weighted lighting at surface texels
+    def bake_lightmap(self, points, samples: int, seed: int = 0) -> np.ndarray:
+        """The lighting arriving at each surface texel (SURFACE_POINT_DTYPE records or (n, 6) floats, e.g. from vertex_texels), each
+        the mean of `samples` paths over the normal's hemisphere: (n,) capi.CUBE_TEXEL_DTYPE, "rgb" an estimate of E / pi.  The scene is
+        uploaded as a frame would upload it; the render textures are not touched."""
+        pts = capi.as_surface_points(points)
+        out = np.empty(pts.shape[0], dtype=capi.CUBE_TEXEL_DTYPE)
+        self._ck(self._L.rcmBakeLightmap(self._h, pts.ctypes.data if pts.size else None, int(pts.shape[0]), int(samples),
                                          int(seed) & 0xFFFFFFFF, out.ctypes.data if out.size else None))
         return out
 
